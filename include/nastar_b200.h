@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NASTAR_B200_ABI_VERSION 2
+#define NASTAR_B200_ABI_VERSION 3
 
 /* status codes (the reference only has Python asserts, differentiable_astar.py:147,172-175) */
 enum {
@@ -196,6 +196,20 @@ int nastar_b200_head_taps(const float *x, int64_t P, int32_t C, const float *w_h
  * differs in any bit from the IEEE-rounded sqrtf(i) that get_heuristic needs (differentiable_astar.py:47-50).
  * `mismatches` is a device int the caller zeroed.  n = 2*511*511+1 covers every argument a 512-row map can produce. */
 int nastar_b200_selftest_sqrt(int32_t n, int32_t *mismatches, void *stream);
+
+/* Shortest-path training labels for new maps (replaces the planning-datasets generator's dijkstra_dist +
+ * extract_policy, planning_datasets_utils/dijkstra.py:120-157 and data.py:27-62; Moore mechanism, one orientation).
+ * maps: B fp32 maps of H*W cells, map_stride (>= H*W) elements apart; a cell is passable iff its value != 0.0.
+ * goal_idx: DEVICE int32 [B], flat goal index y*W+x (an index outside [0, H*W) means no goal: every cell unreached).
+ * Writes, for every map, dense [B][H*W] planes:
+ *   dists    fp32  0 at the goal, -(number of moves to the goal) for passable cells that reach it, -(H*W) for every
+ *                  other cell (obstacles and unreachable regions) -- dijkstra_dist's negated distance, exact in fp32;
+ *   act_mask u8    bit a set iff action a (0..7 = N, E, W, S, NE, NW, SE, SW; a move off the grid or into a
+ *                  non-passable cell stays put) leads to a cell of maximal dists -- the set extract_policy draws from;
+ *   action   i8    the lowest set bit of act_mask (the first maximal action, np.argmax's choice).
+ * One kernel launch.  H, W <= 512, else NASTAR_EUNSUPPORTED.  Asynchronous on `stream`. Returns NASTAR_*. */
+int nastar_b200_opt_labels(const float *maps, int64_t map_stride, const int32_t *goal_idx, int32_t B, int32_t H,
+                           int32_t W, float *dists, uint8_t *act_mask, int8_t *action, void *stream);
 
 /* Number of kernel launches issued by this library since load (bench.py's gpu_launches). */
 uint64_t nastar_b200_launch_count(void);

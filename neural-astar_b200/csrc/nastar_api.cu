@@ -11,6 +11,7 @@
 #include "nastar_bin16.cuh"
 #include "nastar_generic.cuh"
 #include "nastar_glue.cuh"
+#include "nastar_labels.cuh"
 #include "nastar_warp32.cuh"
 #include "nastar_warp64.cuh"
 
@@ -503,6 +504,23 @@ int nastar_b200_selftest_sqrt(int32_t n, int32_t* mismatches, void* stream_v) {
     nastar::sqrt_rn_int_check_kernel<<<num_sms() * 4, 256, 0, static_cast<cudaStream_t>(stream_v)>>>(n, mismatches);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e);
+    return NASTAR_OK;
+}
+
+int nastar_b200_opt_labels(const float* maps, int64_t map_stride, const int32_t* goal_idx, int32_t B, int32_t H,
+                           int32_t W, float* dists, uint8_t* act_mask, int8_t* action, void* stream_v) {
+    if (!maps || !goal_idx || !dists || !act_mask || !action || B <= 0 || H <= 0 || W <= 0) return NASTAR_EINVAL;
+    if (map_stride < int64_t(H) * W) return NASTAR_EINVAL;
+    if (H > nastar::kLabelsMaxSide || W > nastar::kLabelsMaxSide) return NASTAR_EUNSUPPORTED;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+    const size_t smem = nastar::labels_smem_bytes(H, W);
+    cudaError_t e = cudaFuncSetAttribute(nastar::opt_labels_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e != cudaSuccess) return cuda_fail(e);
+    nastar::LabelsArgs a{maps, map_stride, goal_idx, B, H, W, dists, act_mask, action};
+    nastar::opt_labels_kernel<<<B, nastar::labels_threads(H, W), smem, stream>>>(a);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e);
     return NASTAR_OK;
 }

@@ -17,7 +17,7 @@ import torch
 _PKG_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))  # neural-astar_b200/
 LIB_PATH = os.environ.get("NASTAR_B200_LIB", os.path.join(_PKG_ROOT, "lib", "libnastar_b200.so"))
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 NASTAR_OK = 0
 TS_CAPPED = -1
 TS_EXHAUSTED = -2
@@ -75,6 +75,7 @@ EXPORTS = (
     "nastar_b200_head_taps",
     "nastar_b200_conv1_marks",
     "nastar_b200_selftest_sqrt",
+    "nastar_b200_opt_labels",
     "nastar_b200_launch_count",
     "nastar_b200_status_string",
     "nastar_b200_last_cuda_error",
@@ -133,6 +134,9 @@ def lib():
     L.nastar_b200_conv1_marks.restype = ctypes.c_int
     L.nastar_b200_selftest_sqrt.argtypes = [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]
     L.nastar_b200_selftest_sqrt.restype = ctypes.c_int
+    L.nastar_b200_opt_labels.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                         ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+    L.nastar_b200_opt_labels.restype = ctypes.c_int
     L.nastar_b200_launch_count.restype = ctypes.c_uint64
     L.nastar_b200_status_string.argtypes = [ctypes.c_int]
     L.nastar_b200_status_string.restype = ctypes.c_char_p
@@ -355,6 +359,43 @@ def batch_steps(t_solve: torch.Tensor, n_steps: torch.Tensor, T: int) -> torch.T
         _check(L.nastar_b200_batch_steps(t_solve.data_ptr(), n_steps.data_ptr(), t_solve.numel(), int(T),
                                          out.data_ptr(), ctypes.c_void_p(stream)), "nastar_b200_batch_steps")
     return out
+
+
+LABELS_MAX_SIDE = 512
+
+
+def opt_labels(maps: torch.Tensor, goal_idx: torch.Tensor):
+    """Shortest-path labels of B maps in one kernel (include/nastar_b200.h, nastar_b200_opt_labels).
+
+    maps: fp32 CUDA [B,H,W] or [B,1,H,W] (a cell is passable iff != 0); goal_idx: int32 CUDA [B], flat goal index.
+    Returns (dists fp32 [B,1,H,W], act_mask uint8 [B,1,H,W], action int8 [B,1,H,W]) on the current stream."""
+    L = lib()
+    if not maps.is_cuda or maps.dtype != torch.float32:
+        raise RuntimeError("opt_labels: fp32 CUDA maps only (there is no CPU fallback)")
+    if maps.ndim == 4:
+        if maps.shape[1] != 1:
+            raise ValueError("opt_labels: maps are [B,H,W] or [B,1,H,W]")
+        maps = maps[:, 0]
+    if maps.ndim != 3:
+        raise ValueError("opt_labels: maps are [B,H,W] or [B,1,H,W]")
+    B, H, W = maps.shape
+    if goal_idx.dtype != torch.int32 or goal_idx.device != maps.device or tuple(goal_idx.shape) != (B,):
+        raise ValueError("opt_labels: goal_idx must be an int32 [B] tensor on the maps' device")
+    if H > LABELS_MAX_SIDE or W > LABELS_MAX_SIDE:
+        raise ValueError(f"opt_labels: maps up to {LABELS_MAX_SIDE}x{LABELS_MAX_SIDE} (got {H}x{W})")
+    m, ptr, stride = _plane(maps)
+    gi = goal_idx.contiguous()
+    dev = maps.device
+    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
+    with guard:
+        dists = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
+        mask = torch.empty((B, 1, H, W), dtype=torch.uint8, device=dev)
+        action = torch.empty((B, 1, H, W), dtype=torch.int8, device=dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _check(L.nastar_b200_opt_labels(ptr, stride, gi.data_ptr(), B, H, W, dists.data_ptr(), mask.data_ptr(),
+                                        action.data_ptr(), ctypes.c_void_p(stream)), "nastar_b200_opt_labels")
+    del m, gi
+    return dists, mask, action
 
 
 def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Tensor, t_solve: torch.Tensor,

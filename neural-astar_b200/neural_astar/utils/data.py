@@ -1,4 +1,5 @@
-"""Dataset readers with the reference's interface (host-side I/O; not part of the GPU hot path).
+"""Dataset readers with the reference's interface (host-side I/O; not part of the GPU hot path), and the labels
+that turn new maps into a planning dataset (optimal distances and policies computed on the GPU).
 
 Same public names and return conventions as /root/reference/src/neural_astar/utils/data.py:
 `create_dataloader` / `MazeDataset` (:54-245), `create_warcraft_dataloader` / `WarCraftDataset`
@@ -12,6 +13,7 @@ import numpy as np
 import torch
 import torch.utils.data as data
 
+from .. import _native
 from ..planner.differentiable_astar import AstarOutput
 
 # Moore-neighbourhood action order used by the dataset's optimal policies (reference :234-243)
@@ -188,5 +190,92 @@ def create_warcraft_dataloader(dirname: str, split: str, batch_size: int, shuffl
     return data.DataLoader(WarCraftDataset(dirname, split), batch_size=batch_size, shuffle=shuffle, num_workers=0)
 
 
-__all__ = ["AstarOutput", "MazeDataset", "WarCraftDataset", "create_dataloader", "create_warcraft_dataloader",
-           "visualize_results"]
+def compute_opt_labels(map_designs: torch.Tensor, goal_maps: torch.Tensor):
+    """Optimal policies and distances of the planning-datasets generator (get_goalMaps_optPolicies_optDists,
+    planning_datasets_utils/data.py:154-159: dijkstra_dist + extract_policy, Moore mechanism), computed on the GPU in
+    one kernel launch.
+
+    map_designs: CUDA [B,H,W] or [B,1,H,W] (a cell is passable iff its value != 0); goal_maps: CUDA [B,1,H,W] or
+    [B,H,W] with one 1 per map (the first maximum is taken).  H, W <= 512.
+    Returns, on the maps' device:
+      opt_policies [B,8,1,H,W] float32 one-hot of the FIRST maximal action per cell (the reference draws one member
+                   of the maximal set at random; MazeDataset rolls a policy out with the same first-maximum rule);
+      opt_dists    [B,1,H,W] float32: 0 at the goal, -(moves to the goal), -(H*W) where the goal is not reachable;
+      act_mask     [B,1,H,W] uint8: bit a set iff action a is maximal (the set the reference draws from)."""
+    if not map_designs.is_cuda or not goal_maps.is_cuda:
+        raise RuntimeError("compute_opt_labels runs on CUDA tensors only (there is no CPU fallback)")
+    maps = map_designs.detach().float()
+    if maps.ndim == 4:
+        maps = maps[:, 0]
+    B, H, W = maps.shape
+    goal_idx = goal_maps.detach().reshape(B, H * W).argmax(1).to(torch.int32)
+    dists, act_mask, action = _native.opt_labels(maps, goal_idx)
+    policies = torch.zeros((B, 8, 1, H, W), dtype=torch.float32, device=maps.device)
+    policies.scatter_(1, action.long().view(B, 1, 1, H, W), 1.0)
+    return policies, dists, act_mask
+
+
+def _largest_component(maze: np.ndarray) -> np.ndarray:
+    """Cells of the largest 4-connected passable region; ties go to the region whose first cell comes first in
+    raster order (reference data.py:129-132, skimage label(connectivity=1) + np.argmax of the pixel counts).  Any
+    non-zero value is passable here, so a non-binary map forms regions by passability, not by equal values."""
+    from scipy import ndimage
+
+    lab, _ = ndimage.label(maze != 0)
+    counts = np.bincount(lab.ravel())
+    counts[0] = 0
+    return lab == np.argmax(counts)
+
+
+def sample_goal_maps(map_designs, edge_size: int = 0, rng=None) -> np.ndarray:
+    """Goal maps for new maps, drawn like the planning-datasets generator (reference data.py:127-152).
+
+    For every map, in order: take the cells of its largest 4-connected passable region; with edge_size > 0 keep only
+    the cells inside the four edge_size x edge_size corner squares when that leaves any; draw one cell with
+    `rng.choice` over them in raster order.  `rng` is a `random.Random` (or the `random` module, as in the
+    reference, which seeds it with random.seed); each map makes exactly one `choice` call.  map_designs: [B,H,W] or
+    [B,1,H,W] array or tensor.  Returns float32 [B,1,H,W] with one 1 per map."""
+    import random as _random
+
+    rng = _random.Random() if rng is None else rng
+    maps = map_designs.detach().cpu().numpy() if isinstance(map_designs, torch.Tensor) else np.asarray(map_designs)
+    if maps.ndim == 4:
+        maps = maps[:, 0]
+    B, H, W = maps.shape
+    goals = np.zeros((B, 1, H, W), np.float32)
+    for i in range(B):
+        cond = _largest_component(maps[i])
+        if edge_size > 0:
+            corner = np.ones_like(cond)
+            corner[edge_size:-edge_size, :] = False
+            corner[:, edge_size:-edge_size] = False
+            if np.any(cond & corner):
+                cond = cond & corner
+        cells = np.flatnonzero(cond)
+        goals[i, 0].reshape(-1)[int(rng.choice(cells))] = 1.0
+    return goals
+
+
+def _np(x) -> np.ndarray:
+    return x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+
+
+def save_planning_dataset(path: str, train, valid, test) -> None:
+    """Write a planning-datasets .npz (np.savez_compressed arr_0..arr_11, reference generate_spp_instances.py:48-62)
+    that MazeDataset / create_dataloader read.  Each split is (maps [N,H,W] or [N,1,H,W], goal_maps [N,1,H,W],
+    opt_policies [N,8,1,H,W], opt_dists [N,1,H,W]), NumPy arrays or tensors; they are stored in the dtype given."""
+    arrays = []
+    for name, split in (("train", train), ("valid", valid), ("test", test)):
+        maps, goals, policies, dists = (_np(x) for x in split)
+        if maps.ndim == 4:
+            maps = maps[:, 0]
+        N, H, W = maps.shape
+        if (goals.shape != (N, 1, H, W) or policies.shape != (N, 8, 1, H, W) or dists.shape != (N, 1, H, W)):
+            raise ValueError(f"{name}: expected maps [N,H,W], goals / dists [N,1,H,W], policies [N,8,1,H,W] "
+                             f"(got {maps.shape}, {goals.shape}, {policies.shape}, {dists.shape})")
+        arrays += [maps, goals, policies, dists]
+    np.savez_compressed(path, *arrays)
+
+
+__all__ = ["AstarOutput", "MazeDataset", "WarCraftDataset", "compute_opt_labels", "create_dataloader",
+           "create_warcraft_dataloader", "sample_goal_maps", "save_planning_dataset", "visualize_results"]
