@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NASTAR_B200_ABI_VERSION 3
+#define NASTAR_B200_ABI_VERSION 4
 
 /* status codes (the reference only has Python asserts, differentiable_astar.py:147,172-175) */
 enum {
@@ -191,6 +191,18 @@ int nastar_b200_conv1_marks(const float *map_designs, const float *start, int64_
  * bank), so it may change between calls without any device copy.  The 9-tap spatial gather + bias + sigmoid * const
  * that finish the layer happen in nastar_b200_forward's NASTAR_COST_TAPS prologue (or nastar_b200_cost_from_taps). */
 int nastar_b200_head_taps(const float *x, int64_t P, int32_t C, const float *w_host, float *taps, void *stream);
+
+/* The encoder's last body layer fused with the head products (encoder.py:60-78, the 128 -> 256 conv + BatchNorm + ReLU
+ * followed by nastar_b200_head_taps): taps[p][k] = sum_c relu(bias[c] + conv3x3(x, w)[p][c]) * head_w[c][k], pad 1,
+ * stride 1, without writing the [P][C_out] activation.  x: channels-last fp32 [B][H][W][C_in], 16-B aligned;
+ * w: fp32 [C_out][3][3][C_in] (OIHW in channels-last memory, BatchNorm folded), 16-B aligned; bias: fp32 [C_out];
+ * head_w_host: HOST pointer to C_out*9 floats ([c][k], passed by value like nastar_b200_head_taps); taps: fp32
+ * [B][H][W][9], the NASTAR_COST_TAPS layout.  The convolution runs on TF32 tensor cores with fp32 accumulation (like
+ * cuDNN with TF32 allowed); bias, ReLU and the head products are fp32.  Deterministic.  C_in = 128, C_out = 256 and
+ * H, W <= 64 only, else NASTAR_EUNSUPPORTED.  One kernel launch, asynchronous on `stream`. */
+int nastar_b200_conv3x3_head_taps(const float *x, int32_t B, int32_t H, int32_t W, int32_t C_in, int32_t C_out,
+                                  const float *w, const float *bias, const float *head_w_host, float *taps,
+                                  void *stream);
 
 /* Self-test of engine 5's branch-free square root: counts, on the device, the integers i in [0, n) for which it
  * differs in any bit from the IEEE-rounded sqrtf(i) that get_heuristic needs (differentiable_astar.py:47-50).

@@ -9,6 +9,7 @@
 
 #include "../../include/nastar_b200.h"
 #include "nastar_bin16.cuh"
+#include "nastar_convhead.cuh"
 #include "nastar_generic.cuh"
 #include "nastar_glue.cuh"
 #include "nastar_labels.cuh"
@@ -494,6 +495,21 @@ int nastar_b200_head_taps(const float* x, int64_t P, int32_t C, const float* w_h
         case 256: e = launch_head<256>(x, P, w_host, taps, stream); break;
         default: return NASTAR_EUNSUPPORTED;
     }
+    if (e != cudaSuccess) return cuda_fail(e);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return NASTAR_OK;
+}
+
+int nastar_b200_conv3x3_head_taps(const float* x, int32_t B, int32_t H, int32_t W, int32_t C_in, int32_t C_out,
+                                  const float* w, const float* bias, const float* head_w_host, float* taps,
+                                  void* stream_v) {
+    if (!x || !w || !bias || !head_w_host || !taps || B <= 0 || H <= 0 || W <= 0 || C_in <= 0 || C_out <= 0)
+        return NASTAR_EINVAL;
+    if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(w) & 15)) return NASTAR_EINVAL;
+    if (C_in != nastar::kCHCin || C_out != nastar::kCHCout) return NASTAR_EUNSUPPORTED;
+    if (H > nastar::kCHMaxSide || W > nastar::kCHMaxSide) return NASTAR_EUNSUPPORTED;
+    if (int64_t(B) * H * W > (int64_t(1) << 30)) return NASTAR_EINVAL;
+    cudaError_t e = nastar::conv3x3_head_launch(x, B, H, W, w, bias, head_w_host, taps, static_cast<cudaStream_t>(stream_v));
     if (e != cudaSuccess) return cuda_fail(e);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return NASTAR_OK;

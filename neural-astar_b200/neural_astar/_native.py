@@ -17,7 +17,7 @@ import torch
 _PKG_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))  # neural-astar_b200/
 LIB_PATH = os.environ.get("NASTAR_B200_LIB", os.path.join(_PKG_ROOT, "lib", "libnastar_b200.so"))
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 NASTAR_OK = 0
 TS_CAPPED = -1
 TS_EXHAUSTED = -2
@@ -74,6 +74,7 @@ EXPORTS = (
     "nastar_b200_cost_from_taps",
     "nastar_b200_head_taps",
     "nastar_b200_conv1_marks",
+    "nastar_b200_conv3x3_head_taps",
     "nastar_b200_selftest_sqrt",
     "nastar_b200_opt_labels",
     "nastar_b200_launch_count",
@@ -132,6 +133,10 @@ def lib():
                                           ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_void_p]
     L.nastar_b200_conv1_marks.restype = ctypes.c_int
+    L.nastar_b200_conv3x3_head_taps.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
+                                                ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,
+                                                ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+    L.nastar_b200_conv3x3_head_taps.restype = ctypes.c_int
     L.nastar_b200_selftest_sqrt.argtypes = [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]
     L.nastar_b200_selftest_sqrt.restype = ctypes.c_int
     L.nastar_b200_opt_labels.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
@@ -329,6 +334,42 @@ def head_taps(x: torch.Tensor, w_host, out: Optional[torch.Tensor] = None) -> to
         stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_head_taps(x.data_ptr(), B * H * W, C, w_host.ctypes.data, out.data_ptr(),
                                        ctypes.c_void_p(stream)), "nastar_b200_head_taps")
+    return out
+
+
+CONVHEAD_CHANNELS = (128, 256)    # (C_in, C_out) of the fused last-conv + head kernel
+CONVHEAD_MAX_SIDE = 64
+
+
+def conv3x3_head_taps(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, head_w_host,
+                      out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """taps [B,H,W,9] = head products of relu(conv3x3(x, w, pad 1) + b) in one kernel, without writing the activation
+    (include/nastar_b200.h, nastar_b200_conv3x3_head_taps).  x: channels-last fp32 CUDA [B,128,H,W], H, W <= 64;
+    w: folded conv weights [256,128,3,3] stored channels-last; b: [256]; head_w_host: C-contiguous float32 NumPy [256,9]
+    on the HOST.  The convolution runs on TF32 tensor cores with fp32 accumulation; the head products are fp32."""
+    L = lib()
+    B, C, H, W = x.shape
+    if (not x.is_cuda or x.dtype != torch.float32 or not x.is_contiguous(memory_format=torch.channels_last)
+            or (C, w.shape[0]) != CONVHEAD_CHANNELS or H > CONVHEAD_MAX_SIDE or W > CONVHEAD_MAX_SIDE):
+        raise ValueError("conv3x3_head_taps expects a channels-last fp32 CUDA activation [B,128,H,W], H, W <= 64")
+    if (tuple(w.shape) != (256, 128, 3, 3) or w.dtype != torch.float32 or w.device != x.device
+            or not w.is_contiguous(memory_format=torch.channels_last)):
+        raise ValueError("conv3x3_head_taps expects fp32 weights [256,128,3,3] stored channels-last on x's device")
+    if tuple(b.shape) != (256,) or b.dtype != torch.float32 or b.device != x.device or not b.is_contiguous():
+        raise ValueError("conv3x3_head_taps expects a contiguous fp32 bias [256] on x's device")
+    if head_w_host.dtype.name != "float32" or head_w_host.shape != (256, 9) or not head_w_host.flags["C_CONTIGUOUS"]:
+        raise ValueError("head_w_host must be a C-contiguous float32 [256,9] array")
+    dev = x.device
+    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
+    with guard:
+        if out is None:
+            out = torch.empty((B, H, W, 9), dtype=torch.float32, device=dev)
+        elif tuple(out.shape) != (B, H, W, 9) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError("out must be a contiguous fp32 [B,H,W,9] tensor")
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _check(L.nastar_b200_conv3x3_head_taps(x.data_ptr(), B, H, W, C, 256, w.data_ptr(), b.data_ptr(),
+                                               head_w_host.ctypes.data, out.data_ptr(), ctypes.c_void_p(stream)),
+               "nastar_b200_conv3x3_head_taps")
     return out
 
 

@@ -110,6 +110,14 @@ class EncoderBase(nn.Module):
             x = _run_plan_inner(body[:-1], x)
             if on_last_conv is not None:
                 on_last_conv()
+            if body and self._fused_last_conv_ok(body[-1], x):
+                # the last conv and the head products in one TF32 tensor-core kernel: its activation never reaches HBM
+                from .. import _native
+
+                w, b = body[-1][0], body[-1][1]
+                x = x.contiguous(memory_format=torch.channels_last)
+                taps = _native.conv3x3_head_taps(x, w, b, self._head_w_host, out=out)
+                return taps, self._head_scalars[0], self._head_scalars[1]
             x = _run_plan_inner(body[-1:], x)
         if not x.is_contiguous(memory_format=torch.channels_last):
             x = x.contiguous(memory_format=torch.channels_last)
@@ -125,6 +133,18 @@ class EncoderBase(nn.Module):
         else:
             taps = torch.mm(a, wm).view(B, H, W, 9)
         return taps, self._head_scalars[0], self._head_scalars[1]
+
+    def _fused_last_conv_ok(self, layer, x: torch.Tensor) -> bool:
+        """The engine's fused last conv + head kernel covers this layer: TF32 convolutions allowed, the head kernel on,
+        a 3x3 / pad 1 / stride 1 128 -> 256 conv with ReLU and no pooling, maps up to 64x64."""
+        from .. import _native
+
+        w, b, stride, padding, dilation, relu, pool, head = layer
+        return (ALLOW_TF32 and HEAD_KERNEL and self._head_w_host is not None and relu and pool is None and head is None
+                and tuple(w.shape) == (_native.CONVHEAD_CHANNELS[1], _native.CONVHEAD_CHANNELS[0], 3, 3)
+                and tuple(stride) == (1, 1) and tuple(padding) == (1, 1) and tuple(dilation) == (1, 1)
+                and x.is_cuda and x.dtype == torch.float32 and x.shape[1] == _native.CONVHEAD_CHANNELS[0]
+                and x.shape[-2] <= _native.CONVHEAD_MAX_SIDE and x.shape[-1] <= _native.CONVHEAD_MAX_SIDE)
 
     # ---- eval-mode cuDNN fast path (SURVEY 8(f) rank 3: encoder -> search hand-off) -----------------
     # Still plain PyTorch/cuDNN: BatchNorm (running stats) is folded into the preceding conv, activations

@@ -216,8 +216,9 @@ class PipelinedPlanner:
 
     `fork` places the search inside the step: "early" (default) at the start of the step, "late" right before the
     encoder's last, widest convolution.  Measured on an H100 SXM at 700 W (tools/pipe_breakdown.py, b=100, 32x32): the
-    encoder branch alone takes 341 us and the search branch 75 us; the device step takes 362 us forked early and
-    391 us forked late, the three-stage host step 362 us early and 401 us late.
+    encoder branch alone takes 321 us and the search branch 93 us; the device step takes 359 us forked early and
+    408 us forked late, the three-stage host step 354 us early and 409 us late (H100 80GB HBM3 at a 400 W power limit,
+    conv4 and the head fused into one TF32 wgmma kernel; the previous cuDNN conv4 + head took 295 us of the branch).
     """
 
     def __init__(self, planner: torch.nn.Module, map_designs: torch.Tensor, start_maps: torch.Tensor,

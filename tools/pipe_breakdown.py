@@ -74,4 +74,6 @@ with torch.no_grad(), enc_mod._conv_flags():
     w, b, st, pad, dil, relu, pool, head = plan[3]
     x3 = [torch.cudnn_convolution_relu(torch.cudnn_convolution_relu(x, *plan[1][:5], 1), *plan[2][:5], 1) for x in x0]
     res["conv4_plus_head_us"] = timed(lambda k: _native.head_taps(torch.cudnn_convolution_relu(x3[k & 3], w, b, st, pad, dil, 1), na.encoder._head_w_host))
+    # the same two layers as the one fused kernel the eval path selects with TF32 on (csrc/nastar_convhead.cuh)
+    res["conv4_head_fused_us"] = timed(lambda k: _native.conv3x3_head_taps(x3[k & 3], w, b, na.encoder._head_w_host))
 print(json.dumps({k: round(v, 1) for k, v in res.items()}))
