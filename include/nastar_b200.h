@@ -223,6 +223,39 @@ int nastar_b200_selftest_sqrt(int32_t n, int32_t *mismatches, void *stream);
 int nastar_b200_opt_labels(const float *maps, int64_t map_stride, const int32_t *goal_idx, int32_t B, int32_t H,
                            int32_t W, float *dists, uint8_t *act_mask, int8_t *action, void *stream);
 
+/* Training-batch sampler, preparation (MazeDataset._prepared's per-map work, once per dataset, one kernel launch).
+ * dists fp32 [B][H*W] (opt_dists), policies fp32 [B][8][H*W] (opt_policies; the first maximal action of each cell
+ * is used), goal_maps fp32 [B][H*W] (the first maximum is the goal), all dense.  q0..q3: the quantile fractions that
+ * np.percentile evaluates, (100*(1 - [pct1, pct2, pct3, 1])) / 100 in double, each in [0, 1].  Writes per map:
+ *   band_bits   u32 [B][3][ceil(H*W/32)]  cell c of band r = bit c%32 of word c/32; band r = the cells with
+ *               od > min(od) and th[r+1] <= od <= th[r] (bands may share boundary cells);
+ *   band_counts i32 [B][3]; goal_idx i32 [B];
+ *   actions     u32 [B][ceil(H*W/8)]  first maximal action of cell c in bits 4*(c%8) of word c/8;
+ *   thresholds  f64 [B][4]  th = np.percentile(od[od > od.min()], 100*(1 - pcts)), bit for bit;
+ *   status      i32 [B]  0, or an OR of: 1 a distance that is not an integer in [-(H*W), 0]; 2 no cell above
+ *               min(od); 4 an empty band; 8 a cell with od > -(H*W), not the goal, whose action leaves the grid or
+ *               does not reach a cell with od + 1; 16 the goal is not the only cell with od == 0.  Maps with status 0
+ *               are the ones nastar_b200_sampler_sample accepts: each of their walks reaches the goal after exactly
+ *               -od[start] moves.
+ * H, W <= 512, else NASTAR_EUNSUPPORTED.  Asynchronous on `stream`. */
+int nastar_b200_sampler_prepare(const float *dists, const float *policies, const float *goal_maps, int32_t B, int32_t H,
+                                int32_t W, double q0, double q1, double q2, double q3, uint32_t *band_bits,
+                                int32_t *band_counts, int32_t *goal_idx, uint32_t *actions, double *thresholds,
+                                int32_t *status, void *stream);
+
+/* Training-batch sampler, one batch in one kernel launch (MazeDataset.__getitem__ for B samples, collated).
+ * maps / goal_maps: fp32 [n_maps][H*W], the prepared arrays of nastar_b200_sampler_prepare for the same n_maps
+ * maps (all of status 0); indices: i64 [B] map of each sample; draws: [B][S][2] u32 (passed as int32): start s of
+ * sample i takes band r = (d0*3) >> 32 and candidate k = (d1*band_counts[r]) >> 32 of that band, in raster order.
+ * Writes out_maps [B][H*W] and out_goals [B][H*W] (copies), out_starts [B][S][H*W] (one 1 per plane) and out_trajs
+ * [B][S][H*W] (the cells visited by following the actions from the start to the goal: start included, goal
+ * excluded), fp32.  An index outside [0, n_maps) gives all-zero planes.  Plane pointers 16-B aligned.  H, W <= 512. */
+int nastar_b200_sampler_sample(const float *maps, const float *goal_maps, int32_t n_maps, int32_t H, int32_t W,
+                               const uint32_t *band_bits, const int32_t *band_counts, const int32_t *goal_idx,
+                               const uint32_t *actions, const int64_t *indices, const int32_t *draws, int32_t B,
+                               int32_t S, float *out_maps, float *out_starts, float *out_goals, float *out_trajs,
+                               void *stream);
+
 /* Number of kernel launches issued by this library since load (bench.py's gpu_launches). */
 uint64_t nastar_b200_launch_count(void);
 

@@ -13,6 +13,7 @@
 #include "nastar_generic.cuh"
 #include "nastar_glue.cuh"
 #include "nastar_labels.cuh"
+#include "nastar_sampler.cuh"
 #include "nastar_warp32.cuh"
 #include "nastar_warp64.cuh"
 
@@ -535,6 +536,58 @@ int nastar_b200_opt_labels(const float* maps, int64_t map_stride, const int32_t*
     if (e != cudaSuccess) return cuda_fail(e);
     nastar::LabelsArgs a{maps, map_stride, goal_idx, B, H, W, dists, act_mask, action};
     nastar::opt_labels_kernel<<<B, nastar::labels_threads(H, W), smem, stream>>>(a);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e);
+    return NASTAR_OK;
+}
+
+int nastar_b200_sampler_prepare(const float* dists, const float* policies, const float* goal_maps, int32_t B, int32_t H,
+                                int32_t W, double q0, double q1, double q2, double q3, uint32_t* band_bits,
+                                int32_t* band_counts, int32_t* goal_idx, uint32_t* actions, double* thresholds,
+                                int32_t* status, void* stream_v) {
+    if (!dists || !policies || !goal_maps || !band_bits || !band_counts || !goal_idx || !actions || !thresholds || !status)
+        return NASTAR_EINVAL;
+    if (B <= 0 || H <= 0 || W <= 0) return NASTAR_EINVAL;
+    const double q[4] = {q0, q1, q2, q3};
+    for (double v : q)
+        if (!(v >= 0.0 && v <= 1.0)) return NASTAR_EINVAL;
+    if (H > nastar::kSamplerMaxSide || W > nastar::kSamplerMaxSide) return NASTAR_EUNSUPPORTED;
+    nastar::SamplerPrepArgs a{dists, policies, goal_maps, B, H, W, {q0, q1, q2, q3}, band_bits, band_counts, goal_idx,
+                              actions, thresholds, status};
+    nastar::sampler_prepare_kernel<<<B, nastar::kSamplerPrepThreads, 0, static_cast<cudaStream_t>(stream_v)>>>(a);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e);
+    return NASTAR_OK;
+}
+
+int nastar_b200_sampler_sample(const float* maps, const float* goal_maps, int32_t n_maps, int32_t H, int32_t W,
+                               const uint32_t* band_bits, const int32_t* band_counts, const int32_t* goal_idx,
+                               const uint32_t* actions, const int64_t* indices, const int32_t* draws, int32_t B,
+                               int32_t S, float* out_maps, float* out_starts, float* out_goals, float* out_trajs,
+                               void* stream_v) {
+    if (!maps || !goal_maps || !band_bits || !band_counts || !goal_idx || !actions || !indices || !draws || !out_maps ||
+        !out_starts || !out_goals || !out_trajs)
+        return NASTAR_EINVAL;
+    if (n_maps <= 0 || H <= 0 || W <= 0 || B <= 0 || S <= 0) return NASTAR_EINVAL;
+    for (const void* p : {static_cast<const void*>(maps), static_cast<const void*>(goal_maps),
+                          static_cast<const void*>(out_maps), static_cast<const void*>(out_starts),
+                          static_cast<const void*>(out_goals), static_cast<const void*>(out_trajs)})
+        if (reinterpret_cast<uintptr_t>(p) & 15) return NASTAR_EINVAL;   // float4 stores
+    if (H > nastar::kSamplerMaxSide || W > nastar::kSamplerMaxSide) return NASTAR_EUNSUPPORTED;
+    // shared memory: the walked-cell bit planes of up to 8 starts at a time, plus the action plane where it fits
+    const size_t traj = size_t(nastar::sampler_band_words(H, W)) * 4, act = size_t(nastar::sampler_action_words(H, W)) * 4;
+    int chunk = S < nastar::kSamplerMaxChunk ? S : nastar::kSamplerMaxChunk;
+    while (chunk > 1 && chunk * traj + act > kMaxDynSmem) --chunk;
+    const int stage = chunk * traj + act <= kMaxDynSmem ? 1 : 0;
+    const size_t smem = chunk * traj + (stage ? act : 0);
+    cudaError_t e = cudaFuncSetAttribute(nastar::sampler_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e != cudaSuccess) return cuda_fail(e);
+    nastar::SamplerArgs a{maps, goal_maps, band_bits, band_counts, goal_idx, actions, indices,
+                          reinterpret_cast<const uint32_t*>(draws), n_maps, H, W, B, S, chunk, stage,
+                          out_maps, out_starts, out_goals, out_trajs};
+    nastar::sampler_sample_kernel<<<B, nastar::kSamplerThreads, smem, static_cast<cudaStream_t>(stream_v)>>>(a);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e);

@@ -77,6 +77,8 @@ EXPORTS = (
     "nastar_b200_conv3x3_head_taps",
     "nastar_b200_selftest_sqrt",
     "nastar_b200_opt_labels",
+    "nastar_b200_sampler_prepare",
+    "nastar_b200_sampler_sample",
     "nastar_b200_launch_count",
     "nastar_b200_status_string",
     "nastar_b200_last_cuda_error",
@@ -142,6 +144,12 @@ def lib():
     L.nastar_b200_opt_labels.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                          ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     L.nastar_b200_opt_labels.restype = ctypes.c_int
+    L.nastar_b200_sampler_prepare.argtypes = ([ctypes.c_void_p] * 3 + [ctypes.c_int32] * 3 + [ctypes.c_double] * 4
+                                              + [ctypes.c_void_p] * 7)
+    L.nastar_b200_sampler_prepare.restype = ctypes.c_int
+    L.nastar_b200_sampler_sample.argtypes = ([ctypes.c_void_p] * 2 + [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 6
+                                             + [ctypes.c_int32] * 2 + [ctypes.c_void_p] * 5)
+    L.nastar_b200_sampler_sample.restype = ctypes.c_int
     L.nastar_b200_launch_count.restype = ctypes.c_uint64
     L.nastar_b200_status_string.argtypes = [ctypes.c_int]
     L.nastar_b200_status_string.restype = ctypes.c_char_p
@@ -437,6 +445,77 @@ def opt_labels(maps: torch.Tensor, goal_idx: torch.Tensor):
                                         action.data_ptr(), ctypes.c_void_p(stream)), "nastar_b200_opt_labels")
     del m, gi
     return dists, mask, action
+
+
+SAMPLER_MAX_SIDE = 512
+
+
+class SamplerTables(tuple):
+    """Per-map output of sampler_prepare: (band_bits i32 [B,3,ceil(N/32)], counts i32 [B,3], goal_idx i32 [B],
+    actions i32 [B,ceil(N/8)], thresholds f64 [B,4], status i32 [B]), N = H*W (u32 words carried as int32)."""
+
+
+def sampler_prepare(dists: torch.Tensor, policies: torch.Tensor, goal_maps: torch.Tensor, quantiles) -> SamplerTables:
+    """MazeDataset._prepared for B maps in one kernel (include/nastar_b200.h, nastar_b200_sampler_prepare).
+
+    dists [B,1,H,W], policies [B,8,1,H,W], goal_maps [B,1,H,W]: fp32 CUDA tensors; quantiles: the four fp64 fractions
+    np.percentile evaluates.  Asynchronous on the current stream."""
+    L = lib()
+    B, _, H, W = dists.shape
+    for name, t_, shape in (("dists", dists, (B, 1, H, W)), ("policies", policies, (B, 8, 1, H, W)),
+                            ("goal_maps", goal_maps, (B, 1, H, W))):
+        if not t_.is_cuda or t_.dtype != torch.float32 or tuple(t_.shape) != shape or t_.device != dists.device:
+            raise ValueError(f"sampler_prepare: {name} must be an fp32 CUDA tensor {list(shape)} on the dists' device")
+    if H > SAMPLER_MAX_SIDE or W > SAMPLER_MAX_SIDE:
+        raise ValueError(f"sampler_prepare: maps up to {SAMPLER_MAX_SIDE}x{SAMPLER_MAX_SIDE} (got {H}x{W})")
+    d, p, g = (t_.detach().contiguous() for t_ in (dists, policies, goal_maps))
+    N = H * W
+    dev = dists.device
+    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
+    with guard:
+        i32 = dict(dtype=torch.int32, device=dev)
+        out = SamplerTables((torch.empty((B, 3, (N + 31) // 32), **i32), torch.empty((B, 3), **i32),
+                             torch.empty((B,), **i32), torch.empty((B, (N + 7) // 8), **i32),
+                             torch.empty((B, 4), dtype=torch.float64, device=dev), torch.empty((B,), **i32)))
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        q = [float(v) for v in quantiles]
+        _check(L.nastar_b200_sampler_prepare(d.data_ptr(), p.data_ptr(), g.data_ptr(), B, H, W, *q,
+                                             *(t_.data_ptr() for t_ in out), ctypes.c_void_p(stream)),
+               "nastar_b200_sampler_prepare")
+    del d, p, g
+    return out
+
+
+def sampler_sample(maps: torch.Tensor, goal_maps: torch.Tensor, tables: SamplerTables, indices: torch.Tensor,
+                   draws: torch.Tensor):
+    """One training batch in one kernel (nastar_b200_sampler_sample): maps / goal_maps fp32 CUDA [n,1,H,W] (contiguous),
+    tables from sampler_prepare for the same n maps, indices int64 CUDA [B], draws int32 CUDA [B,S,2].
+    Returns (map_designs [B,1,H,W], start_maps [B,S,H,W], goal_maps [B,1,H,W], opt_trajs [B,S,H,W]), fp32."""
+    L = lib()
+    n, _, H, W = maps.shape
+    if (maps.dtype != torch.float32 or not maps.is_cuda or not maps.is_contiguous() or goal_maps.shape != maps.shape
+            or goal_maps.dtype != torch.float32 or not goal_maps.is_contiguous() or goal_maps.device != maps.device):
+        raise ValueError("sampler_sample: maps and goal_maps must be contiguous fp32 CUDA tensors [n,1,H,W]")
+    B, S, two = draws.shape
+    if two != 2 or draws.dtype != torch.int32 or not draws.is_contiguous() or draws.device != maps.device:
+        raise ValueError("sampler_sample: draws must be a contiguous int32 [B,S,2] tensor on the maps' device")
+    if (indices.dtype != torch.int64 or tuple(indices.shape) != (B,) or not indices.is_contiguous()
+            or indices.device != maps.device):
+        raise ValueError("sampler_sample: indices must be a contiguous int64 [B] tensor on the maps' device")
+    bits, counts, goal_idx, actions = tables[:4]
+    dev = maps.device
+    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
+    with guard:
+        f32 = dict(dtype=torch.float32, device=dev)
+        out = (torch.empty((B, 1, H, W), **f32), torch.empty((B, S, H, W), **f32), torch.empty((B, 1, H, W), **f32),
+               torch.empty((B, S, H, W), **f32))
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _check(L.nastar_b200_sampler_sample(maps.data_ptr(), goal_maps.data_ptr(), n, H, W, bits.data_ptr(),
+                                            counts.data_ptr(), goal_idx.data_ptr(), actions.data_ptr(),
+                                            indices.data_ptr(), draws.data_ptr(), B, S,
+                                            *(t_.data_ptr() for t_ in out), ctypes.c_void_p(stream)),
+               "nastar_b200_sampler_sample")
+    return out
 
 
 def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Tensor, t_solve: torch.Tensor,

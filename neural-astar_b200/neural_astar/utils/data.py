@@ -166,6 +166,130 @@ def create_dataloader(filename: str, split: str, batch_size: int, num_starts: in
                            shuffle=shuffle, num_workers=0)
 
 
+def _percentile_fractions(pcts) -> np.ndarray:
+    """The fp64 fractions np.percentile(a, 100 * (1 - pcts)) evaluates for a float32 `a` (it divides by float32(100))."""
+    return np.true_divide(100.0 * (1 - np.asarray(pcts, np.float64)), np.float32(100))
+
+
+_SAMPLER_STATUS = ((1, "distances that are not integers in [-(H*W), 0]"), (2, "no cell above the minimum distance"),
+                   (4, "an empty percentile band"),
+                   (8, "a policy action that does not lead to a cell one step closer to the goal"),
+                   (16, "a goal that is not the only cell at distance 0"))
+
+
+class DeviceMazeDataset:
+    def __init__(self, filename: str, split: str, pct1: float = 0.55, pct2: float = 0.70, pct3: float = 0.85,
+                 num_starts: int = 1, device=None):
+        """MazeDataset's shortest-path problems, drawn as whole batches on the GPU (csrc/nastar_sampler.cuh).
+
+        Same file, same bands and the same trajectory rule as MazeDataset, but the draws come from a torch.Generator
+        on the device, so the starts are not np.random's.  The per-map work (bands, goal, first-max actions) runs once,
+        here, in one kernel launch; `sample` then writes a collated batch in one launch, without host synchronisation.
+        Raises ValueError naming the maps that cannot be sampled (see `from_labels`)."""
+        assert filename.endswith("npz")
+        with np.load(filename) as f:
+            k = _SPLIT_OFFSET[split]
+            maps, goals, policies, dists = (f[f"arr_{k + j}"].astype(np.float32) for j in range(4))
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self._setup(*(torch.from_numpy(x).to(dev) for x in (maps[:, None], goals, policies, dists)),
+                    (pct1, pct2, pct3), num_starts)
+
+    @classmethod
+    def from_labels(cls, map_designs: torch.Tensor, goal_maps: torch.Tensor, opt_policies: torch.Tensor,
+                    opt_dists: torch.Tensor, pct1: float = 0.55, pct2: float = 0.70, pct3: float = 0.85,
+                    num_starts: int = 1) -> "DeviceMazeDataset":
+        """A dataset over device tensors, e.g. from compute_opt_labels / sample_goal_maps, without a file or a host
+        copy of the planes: map_designs [N,H,W] or [N,1,H,W], goal_maps [N,1,H,W], opt_policies [N,8,1,H,W],
+        opt_dists [N,1,H,W], on one CUDA device.
+
+        Every map must have integer distances in [-(H*W), 0] with the goal as the only 0, cells above the minimum
+        distance, three non-empty bands, and a first-max action that moves every cell that reaches the goal onto the
+        grid cell exactly one step closer.  This is stricter than MazeDataset, which only asserts against revisiting a
+        cell during a walk; it guarantees that every walk ends at the goal after exactly -opt_dists[start] moves.
+        Every compute_opt_labels policy and every shipped planning dataset satisfies it."""
+        self = cls.__new__(cls)
+        maps = map_designs.detach().float()
+        if maps.ndim == 3:
+            maps = maps[:, None]
+        self._setup(maps, goal_maps.detach().float(), opt_policies.detach().float(), opt_dists.detach().float(),
+                    (pct1, pct2, pct3), num_starts)
+        return self
+
+    def _setup(self, maps, goals, policies, dists, pcts, num_starts):
+        if not maps.is_cuda:
+            raise RuntimeError("DeviceMazeDataset runs on CUDA tensors only (there is no CPU fallback)")
+        if int(num_starts) <= 0:
+            raise ValueError("num_starts must be positive")
+        self.map_designs = maps.contiguous()
+        self.goal_maps = goals.contiguous()
+        self.num_starts = int(num_starts)
+        self.pcts = np.array([*pcts, 1.0])
+        self.device = maps.device
+        self._tables = _native.sampler_prepare(dists, policies, self.goal_maps, _percentile_fractions(self.pcts))
+        status = self._tables[5].cpu().numpy()
+        if status.any():
+            bad = [f"{why}: maps {np.flatnonzero(status & bit).tolist()[:20]}"
+                   for bit, why in _SAMPLER_STATUS if (status & bit).any()]
+            raise ValueError(f"{int((status != 0).sum())} of {len(status)} maps cannot be sampled; " + "; ".join(bad))
+
+    def __len__(self):
+        return self.map_designs.shape[0]
+
+    @property
+    def thresholds(self) -> torch.Tensor:
+        """[N,4] fp64: np.percentile(od[od > od.min()], 100 * (1 - [pct1, pct2, pct3, 1])) per map."""
+        return self._tables[4]
+
+    def sample(self, indices, generator: torch.Generator = None, draws: torch.Tensor = None):
+        """(map_designs [B,1,H,W], start_maps [B,S,H,W], goal_maps [B,1,H,W], opt_trajs [B,S,H,W]) as fp32 tensors on
+        the device, S = num_starts: a collated create_dataloader batch of the maps `indices` (host or device, B
+        of them).  Each start picks one of the three bands uniformly, then a candidate of that band uniformly in
+        raster order: with u32 draws (d0, d1), band (d0*3) >> 32 and candidate (d1*count) >> 32.  The draws are
+        torch.randint on the device with `generator` (a CUDA generator; the default one when None), or the given
+        int32 [B,S,2] tensor `draws`.  One kernel launch; host indices are range-checked, device indices must lie in
+        [0, len(self)) (a row outside comes back all zero)."""
+        idx = torch.as_tensor(indices)
+        if idx.device.type == "cpu":
+            if idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= len(self)):
+                raise IndexError(f"indices must lie in [0, {len(self)})")
+            idx = idx.to(self.device)
+        idx = idx.reshape(-1).to(torch.int64).contiguous()
+        B, S = idx.numel(), self.num_starts
+        if draws is None:
+            draws = torch.randint(-2 ** 31, 2 ** 31, (B, S, 2), dtype=torch.int32, device=self.device,
+                                  generator=generator)
+        elif tuple(draws.shape) != (B, S, 2):
+            raise ValueError(f"draws must be [B, num_starts, 2] = {[B, S, 2]}")
+        return _native.sampler_sample(self.map_designs, self.goal_maps, self._tables, idx,
+                                      draws.to(self.device, torch.int32).contiguous())
+
+
+class DeviceDataLoader:
+    """Batches of a DeviceMazeDataset in DataLoader order: consecutive slices of range(len(dataset)), or of one
+    torch.randperm per pass with `shuffle`, the last batch kept partial."""
+
+    def __init__(self, dataset: DeviceMazeDataset, batch_size: int, shuffle: bool = False,
+                 generator: torch.Generator = None):
+        self.dataset, self.batch_size, self.shuffle, self.generator = dataset, int(batch_size), shuffle, generator
+
+    def __len__(self):
+        return -(-len(self.dataset) // self.batch_size)
+
+    def __iter__(self):
+        n, dev = len(self.dataset), self.dataset.device
+        order = (torch.randperm(n, device=dev, generator=self.generator) if self.shuffle
+                 else torch.arange(n, device=dev))
+        for i in range(0, n, self.batch_size):
+            yield self.dataset.sample(order[i:i + self.batch_size], generator=self.generator)
+
+
+def create_device_dataloader(filename: str, split: str, batch_size: int, num_starts: int = 1, shuffle: bool = False,
+                             generator: torch.Generator = None) -> DeviceDataLoader:
+    """create_dataloader's batches drawn on the GPU (DeviceMazeDataset): an iterable of device batches that
+    GraphedTrainStep and PlannerModule.fit take as they are."""
+    return DeviceDataLoader(DeviceMazeDataset(filename, split, num_starts=num_starts), batch_size, shuffle, generator)
+
+
 class WarCraftDataset(data.Dataset):
     def __init__(self, dirname: str, split: str):
         """WarCraft terrain maps: `<split>_maps.npy` (uint8 HWC) and `<split>_shortest_paths.npy` (reference :273-295)."""
@@ -277,5 +401,6 @@ def save_planning_dataset(path: str, train, valid, test) -> None:
     np.savez_compressed(path, *arrays)
 
 
-__all__ = ["AstarOutput", "MazeDataset", "WarCraftDataset", "compute_opt_labels", "create_dataloader",
-           "create_warcraft_dataloader", "sample_goal_maps", "save_planning_dataset", "visualize_results"]
+__all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "MazeDataset", "WarCraftDataset",
+           "compute_opt_labels", "create_dataloader", "create_device_dataloader", "create_warcraft_dataloader",
+           "sample_goal_maps", "save_planning_dataset", "visualize_results"]
