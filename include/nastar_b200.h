@@ -223,6 +223,34 @@ int nastar_b200_selftest_sqrt(int32_t n, int32_t *mismatches, void *stream);
 int nastar_b200_opt_labels(const float *maps, int64_t map_stride, const int32_t *goal_idx, int32_t B, int32_t H,
                            int32_t W, float *dists, uint8_t *act_mask, int8_t *action, void *stream);
 
+/* Exact vertex-weighted shortest paths to a goal, for cost maps (the labels of WarCraft-style training and the optimum
+ * that learned-cost paths are measured against).  Per map b (DESIGN.md §11):
+ *   cost      B fp32 maps of H*W cells, cost_stride (>= H*W) elements apart;
+ *   passable  B fp32 maps, passable_stride (>= H*W) apart, a cell is passable iff != 0.0; NULL = every cell passable;
+ *   goal_idx  DEVICE int32 [B] flat goal index y*W+x; start_idx DEVICE int32 [B] or NULL (then path_maps and
+ *             path_costs must be NULL too, and with a start both are required).
+ * Moves: actions 0..7 = N, E, W, S, NE, NW, SE, SW from a passable cell into an in-grid cell that is passable or is
+ * the goal (no corner check).  A move charges the cost of the cell it enters: the cost-to-go is D[goal] = +0,
+ * D[v] = min over moves v->t of fl(D[t] + c[t]), each add rounded once; the minimum over all paths of that fp32 fold,
+ * independent of evaluation order.  A move v->t is optimal iff fl(D[t] + c[t]) == D[v]; hop[v] = 1 + the least hop
+ * of v's optimal targets (hop[goal] = 0).  Writes dense [B][H*W] planes:
+ *   dists    fp32  -D: 0 at the goal, -inf where the goal is unreachable;
+ *   hops     i32   hop, -1 where unreachable;
+ *   act_mask u8    bit a set iff action a is optimal and enters a cell with hop one lower (0 at the goal and at
+ *                  unreachable cells);
+ *   action   i8    the lowest set bit of act_mask, -1 where it is 0;
+ *   path_maps fp32 [B][H*W] (with a start) the cells of the roll-out of `action` from the start, start and goal
+ *                  included; path_costs fp32 [B] = fl(c[start] + D[start]) (+inf, empty mask if unreachable);
+ *   status   i32 [B]  0, or an OR of: 1 the goal or a passable cell has a negative, NaN or infinite cost (the planes
+ *                  are then filled as unreachable); 2 goal index outside [0, H*W); 4 a start was given and cannot
+ *                  reach the goal.
+ * One kernel launch, one CTA per map.  H, W <= 128 (H*W <= 16384), else NASTAR_EUNSUPPORTED.  Asynchronous on
+ * `stream`.  Returns NASTAR_*. */
+int nastar_b200_weighted_labels(const float *cost, int64_t cost_stride, const float *passable, int64_t passable_stride,
+                                const int32_t *goal_idx, const int32_t *start_idx, int32_t B, int32_t H, int32_t W,
+                                float *dists, int32_t *hops, uint8_t *act_mask, int8_t *action, float *path_maps,
+                                float *path_costs, int32_t *status, void *stream);
+
 /* Training-batch sampler, preparation (MazeDataset._prepared's per-map work, once per dataset, one kernel launch).
  * dists fp32 [B][H*W] (opt_dists), policies fp32 [B][8][H*W] (opt_policies; the first maximal action of each cell
  * is used), goal_maps fp32 [B][H*W] (the first maximum is the goal), all dense.  q0..q3: the quantile fractions that

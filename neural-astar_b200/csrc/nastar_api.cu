@@ -14,6 +14,7 @@
 #include "nastar_glue.cuh"
 #include "nastar_labels.cuh"
 #include "nastar_sampler.cuh"
+#include "nastar_wlabels.cuh"
 #include "nastar_warp32.cuh"
 #include "nastar_warp64.cuh"
 
@@ -536,6 +537,31 @@ int nastar_b200_opt_labels(const float* maps, int64_t map_stride, const int32_t*
     if (e != cudaSuccess) return cuda_fail(e);
     nastar::LabelsArgs a{maps, map_stride, goal_idx, B, H, W, dists, act_mask, action};
     nastar::opt_labels_kernel<<<B, nastar::labels_threads(H, W), smem, stream>>>(a);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e);
+    return NASTAR_OK;
+}
+
+int nastar_b200_weighted_labels(const float* cost, int64_t cost_stride, const float* passable, int64_t passable_stride,
+                                const int32_t* goal_idx, const int32_t* start_idx, int32_t B, int32_t H, int32_t W,
+                                float* dists, int32_t* hops, uint8_t* act_mask, int8_t* action, float* path_maps,
+                                float* path_costs, int32_t* status, void* stream_v) {
+    if (!cost || !goal_idx || !dists || !hops || !act_mask || !action || !status || B <= 0 || H <= 0 || W <= 0)
+        return NASTAR_EINVAL;
+    if (cost_stride < int64_t(H) * W || (passable && passable_stride < int64_t(H) * W)) return NASTAR_EINVAL;
+    // paths need a start per map, and a start needs somewhere to put its path
+    if (bool(start_idx) != bool(path_maps) || bool(start_idx) != bool(path_costs)) return NASTAR_EINVAL;
+    if (H > nastar::kWLabelsMaxSide || W > nastar::kWLabelsMaxSide || int64_t(H) * W > nastar::kWLabelsMaxCells)
+        return NASTAR_EUNSUPPORTED;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+    const size_t smem = nastar::wlabels_smem_bytes(H, W);
+    cudaError_t e =
+        cudaFuncSetAttribute(nastar::weighted_labels_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e != cudaSuccess) return cuda_fail(e);
+    nastar::WLabelsArgs a{cost,   cost_stride, passable,  passable_stride, goal_idx,   start_idx, B,     H, W,
+                          dists,  hops,        act_mask,  action,          path_maps,  path_costs, status};
+    nastar::weighted_labels_kernel<<<B, nastar::wlabels_threads(H, W), smem, stream>>>(a);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e);

@@ -77,6 +77,7 @@ EXPORTS = (
     "nastar_b200_conv3x3_head_taps",
     "nastar_b200_selftest_sqrt",
     "nastar_b200_opt_labels",
+    "nastar_b200_weighted_labels",
     "nastar_b200_sampler_prepare",
     "nastar_b200_sampler_sample",
     "nastar_b200_launch_count",
@@ -144,6 +145,9 @@ def lib():
     L.nastar_b200_opt_labels.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                          ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     L.nastar_b200_opt_labels.restype = ctypes.c_int
+    L.nastar_b200_weighted_labels.argtypes = ([ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64]
+                                              + [ctypes.c_void_p] * 2 + [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 8)
+    L.nastar_b200_weighted_labels.restype = ctypes.c_int
     L.nastar_b200_sampler_prepare.argtypes = ([ctypes.c_void_p] * 3 + [ctypes.c_int32] * 3 + [ctypes.c_double] * 4
                                               + [ctypes.c_void_p] * 7)
     L.nastar_b200_sampler_prepare.restype = ctypes.c_int
@@ -445,6 +449,68 @@ def opt_labels(maps: torch.Tensor, goal_idx: torch.Tensor):
                                         action.data_ptr(), ctypes.c_void_p(stream)), "nastar_b200_opt_labels")
     del m, gi
     return dists, mask, action
+
+
+WLABELS_MAX_SIDE = 128
+
+
+class WeightedLabels(tuple):
+    """Output of weighted_labels: (dists f32 [B,1,H,W], hops i32 [B,1,H,W], act_mask u8 [B,1,H,W], action i8
+    [B,1,H,W], path_maps f32 [B,1,H,W] or None, path_costs f32 [B] or None, status i32 [B])."""
+
+
+def weighted_labels(cost: torch.Tensor, goal_idx: torch.Tensor, passable: Optional[torch.Tensor] = None,
+                    start_idx: Optional[torch.Tensor] = None) -> WeightedLabels:
+    """Exact vertex-weighted shortest paths of B cost maps in one kernel (include/nastar_b200.h,
+    nastar_b200_weighted_labels).
+
+    cost: fp32 CUDA [B,H,W] or [B,1,H,W]; passable: the same shape (a cell is passable iff != 0) or None (every cell);
+    goal_idx / start_idx: int32 CUDA [B] flat indices (start_idx None: no paths).  H, W <= 128.  Asynchronous on the
+    current stream; the per-map status is not read back here."""
+    L = lib()
+
+    def plane(x, name):
+        if not x.is_cuda or x.dtype != torch.float32:
+            raise RuntimeError(f"weighted_labels: {name} must be fp32 CUDA maps (there is no CPU fallback)")
+        if x.ndim == 4:
+            if x.shape[1] != 1:
+                raise ValueError(f"weighted_labels: {name} are [B,H,W] or [B,1,H,W]")
+            x = x[:, 0]
+        if x.ndim != 3:
+            raise ValueError(f"weighted_labels: {name} are [B,H,W] or [B,1,H,W]")
+        return _plane(x.detach())
+
+    c, cptr, cstride = plane(cost, "cost maps")
+    B, H, W = c.shape
+    dev = c.device
+    p, pptr, pstride = (None, None, 0) if passable is None else plane(passable, "passable maps")
+    if p is not None and (p.shape != c.shape or p.device != dev):
+        raise ValueError("weighted_labels: passable maps must match the cost maps' shape and device")
+    for name, ix in (("goal_idx", goal_idx), ("start_idx", start_idx)):
+        if ix is not None and (ix.dtype != torch.int32 or ix.device != dev or tuple(ix.shape) != (B,)):
+            raise ValueError(f"weighted_labels: {name} must be an int32 [B] tensor on the cost maps' device")
+    if H > WLABELS_MAX_SIDE or W > WLABELS_MAX_SIDE:
+        raise ValueError(f"weighted_labels: maps up to {WLABELS_MAX_SIDE}x{WLABELS_MAX_SIDE} (got {H}x{W})")
+    gi = goal_idx.contiguous()
+    si = None if start_idx is None else start_idx.contiguous()
+    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
+    with guard:
+        dists = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
+        hops = torch.empty((B, 1, H, W), dtype=torch.int32, device=dev)
+        mask = torch.empty((B, 1, H, W), dtype=torch.uint8, device=dev)
+        action = torch.empty((B, 1, H, W), dtype=torch.int8, device=dev)
+        paths = None if si is None else torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
+        pcost = None if si is None else torch.empty((B,), dtype=torch.float32, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _check(L.nastar_b200_weighted_labels(cptr, cstride, pptr, pstride, gi.data_ptr(),
+                                             None if si is None else si.data_ptr(), B, H, W, dists.data_ptr(),
+                                             hops.data_ptr(), mask.data_ptr(), action.data_ptr(),
+                                             None if paths is None else paths.data_ptr(),
+                                             None if pcost is None else pcost.data_ptr(), status.data_ptr(),
+                                             ctypes.c_void_p(stream)), "nastar_b200_weighted_labels")
+    del c, p, gi, si
+    return WeightedLabels((dists, hops, mask, action, paths, pcost, status))
 
 
 SAMPLER_MAX_SIDE = 512

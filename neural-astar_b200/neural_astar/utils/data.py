@@ -339,6 +339,89 @@ def compute_opt_labels(map_designs: torch.Tensor, goal_maps: torch.Tensor):
     return policies, dists, act_mask
 
 
+def _weighted_inputs(cost_maps: torch.Tensor, goal_maps: torch.Tensor, passable, what: str):
+    if not cost_maps.is_cuda or not goal_maps.is_cuda or (passable is not None and not passable.is_cuda):
+        raise RuntimeError(f"{what} runs on CUDA tensors only (there is no CPU fallback)")
+    cost = cost_maps.detach().float()
+    if cost.ndim == 4:
+        cost = cost[:, 0]
+    B, H, W = cost.shape
+    goal_idx = goal_maps.detach().reshape(B, H * W).argmax(1).to(torch.int32)
+    pas = None if passable is None else passable.detach().float().reshape(B, H, W)
+    return cost, pas, goal_idx
+
+
+def _raise_on_bad_costs(status: torch.Tensor, what: str) -> None:
+    bad = torch.nonzero(status & 1).flatten().tolist()
+    if bad:
+        raise ValueError(f"{what}: the goal or a passable cell has a negative, NaN or infinite cost in maps {bad}")
+
+
+def compute_weighted_opt_labels(cost_maps: torch.Tensor, goal_maps: torch.Tensor, passable: torch.Tensor = None):
+    """Exact vertex-weighted shortest-path labels of cost maps, computed on the GPU in one kernel launch
+    (DESIGN.md §11).  A move (8-connected, no corner check) leaves a passable cell, enters an in-grid cell that is
+    passable or is the goal, and costs the cost of the cell it enters; every sum is the fp32 fold from the goal.
+
+    cost_maps: CUDA [B,H,W] or [B,1,H,W], every cost that can be charged finite and >= 0; goal_maps: CUDA [B,1,H,W] or
+    [B,H,W] with one 1 per map (the first maximum is taken); passable: CUDA maps of the same shape (a cell is passable
+    iff != 0), None = every cell.  H, W <= 128.
+    Returns, on the maps' device:
+      opt_policies [B,8,1,H,W] float32 one-hot of the first optimal action that leads one hop closer to the goal,
+                   all zero at the goal and where the goal is unreachable;
+      opt_dists    [B,1,H,W] float32: minus the cost-to-go (0 at the goal, -inf where the goal is unreachable);
+      act_mask     [B,1,H,W] uint8: bit a set iff action a is optimal and leads one hop closer;
+      hops         [B,1,H,W] int32: moves along the policy to the goal, -1 where unreachable.
+    Raises ValueError naming the maps with a negative, NaN or infinite cost on the goal or a passable cell (this
+    reads the per-map status back to the host)."""
+    cost, pas, goal_idx = _weighted_inputs(cost_maps, goal_maps, passable, "compute_weighted_opt_labels")
+    B, H, W = cost.shape
+    dists, hops, act_mask, action, _, _, status = _native.weighted_labels(cost, goal_idx, pas)
+    _raise_on_bad_costs(status, "compute_weighted_opt_labels")
+    policies = torch.zeros((B, 9, 1, H, W), dtype=torch.float32, device=cost.device)
+    policies.scatter_(1, (action.long() % 9).view(B, 1, 1, H, W), 1.0)    # action -1 lands in the dropped slot 8
+    return policies[:, :8].contiguous(), dists, act_mask, hops
+
+
+def shortest_path_maps(cost_maps: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
+                       passable: torch.Tensor = None):
+    """Minimum-cost paths from the start to the goal of every map, in one kernel launch (the inputs and moves of
+    compute_weighted_opt_labels; start_maps [B,1,H,W] or [B,H,W] with one 1 per map).
+
+    Returns (path_maps [B,1,H,W] float32: the cells of the path, start and goal included -- the layout of WarCraft's
+    shortest_paths and of DifferentiableAstar's paths; path_costs [B] float32: the sum of the costs of every cell of
+    the path, as the fp32 fold from the goal).  A start that cannot reach the goal gives an empty mask and +inf; a
+    start on the goal gives the goal alone and its cost.  Raises ValueError like compute_weighted_opt_labels."""
+    cost, pas, goal_idx = _weighted_inputs(cost_maps, goal_maps, passable, "shortest_path_maps")
+    B, H, W = cost.shape
+    start_idx = start_maps.detach().reshape(B, H * W).argmax(1).to(torch.int32)
+    out = _native.weighted_labels(cost, goal_idx, pas, start_idx)
+    _raise_on_bad_costs(out[6], "shortest_path_maps")
+    return out[4], out[5]
+
+
+def save_warcraft_dataset(dirname: str, split: str, map_images, shortest_paths) -> None:
+    """Write `{split}_maps.npy` and `{split}_shortest_paths.npy` under `dirname`, the files WarCraftDataset /
+    create_warcraft_dataloader read.  map_images: uint8 [N,H,W,C] (stored as is) or float [N,C,H,W] in [0, 1] (the
+    layout WarCraftDataset returns; stored as round(255 * x) in uint8 [N,H,W,C]); shortest_paths: [N,h,w] or
+    [N,1,h,w] masks, e.g. shortest_path_maps' path_maps, stored as float32 [N,h,w]."""
+    import os
+
+    imgs, paths = _np(map_images), _np(shortest_paths)
+    if imgs.dtype != np.uint8:
+        if imgs.ndim != 4:
+            raise ValueError(f"map_images: expected [N,C,H,W] floats in [0, 1] or uint8 [N,H,W,C] (got {imgs.shape})")
+        imgs = np.rint(np.clip(imgs.transpose(0, 2, 3, 1), 0.0, 1.0) * 255.0).astype(np.uint8)
+    if paths.ndim == 4:
+        if paths.shape[1] != 1:
+            raise ValueError(f"shortest_paths: expected [N,h,w] or [N,1,h,w] (got {paths.shape})")
+        paths = paths[:, 0]
+    if imgs.ndim != 4 or paths.ndim != 3 or imgs.shape[0] != paths.shape[0]:
+        raise ValueError(f"expected N images [N,H,W,C] and N masks [N,h,w] (got {imgs.shape}, {paths.shape})")
+    os.makedirs(dirname, exist_ok=True)
+    np.save(os.path.join(dirname, f"{split}_maps.npy"), np.ascontiguousarray(imgs))
+    np.save(os.path.join(dirname, f"{split}_shortest_paths.npy"), paths.astype(np.float32))
+
+
 def _largest_component(maze: np.ndarray) -> np.ndarray:
     """Cells of the largest 4-connected passable region; ties go to the region whose first cell comes first in
     raster order (reference data.py:129-132, skimage label(connectivity=1) + np.argmax of the pixel counts).  Any
@@ -402,5 +485,6 @@ def save_planning_dataset(path: str, train, valid, test) -> None:
 
 
 __all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "MazeDataset", "WarCraftDataset",
-           "compute_opt_labels", "create_dataloader", "create_device_dataloader", "create_warcraft_dataloader",
-           "sample_goal_maps", "save_planning_dataset", "visualize_results"]
+           "compute_opt_labels", "compute_weighted_opt_labels", "create_dataloader", "create_device_dataloader",
+           "create_warcraft_dataloader", "sample_goal_maps", "save_planning_dataset", "save_warcraft_dataset",
+           "shortest_path_maps", "visualize_results"]

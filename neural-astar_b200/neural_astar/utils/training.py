@@ -72,6 +72,24 @@ def planner_metrics_from_counts(n_closed: torch.Tensor, path_len: torch.Tensor):
     return vals[0], vals[1], vals[2]
 
 
+def path_cost_metrics(paths: torch.Tensor, cost_maps: torch.Tensor, opt_path_costs: torch.Tensor, rtol: float = 1e-5):
+    """(p_opt, cost_ratio) of paths on cost maps against their optimal path costs, reduced on the device.
+
+    paths / cost_maps: [B,...] masks and costs of the same shape (e.g. a planner's `paths` and the true cost maps);
+    opt_path_costs: [B], e.g. shortest_path_maps' path_costs.  A path's cost is the fp64 sum of the costs of its
+    cells (mask != 0).  p_opt: share of maps whose path costs at most opt * (1 + rtol) -- the fp32 optimum is a
+    rounded fold, so an optimal path may sum a few ulps away from it; cost_ratio: mean of path cost / optimum.
+    Keep maps with a finite, positive optimum: others give inf or NaN ratios.  One device->host read."""
+    B = paths.shape[0]
+    mask = paths.detach().reshape(B, -1) != 0
+    cost = torch.where(mask, cost_maps.detach().reshape(B, -1).double(), 0.0).sum(1)
+    opt = opt_path_costs.detach().reshape(B).double()
+    p_opt = (cost <= opt * (1.0 + rtol)).double().mean()
+    ratio = (cost / opt).mean()
+    vals = torch.stack((p_opt, ratio)).tolist()
+    return vals[0], vals[1]
+
+
 class GraphedTrainStep:
     """One training step of scripts/train.py (forward, L1 loss on histories, backward through the search kernels
     and the encoder, RMSprop update; reference utils/training.py:52-61) captured ONCE as a CUDA graph and replayed.
