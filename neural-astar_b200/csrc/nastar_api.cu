@@ -6,6 +6,7 @@
 
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "../../include/nastar_b200.h"
 #include "nastar_bin16.cuh"
@@ -35,40 +36,87 @@ int num_sms() {
     return n;
 }
 
-// one-time fill of the 32x32 heuristic table on the current device (stream-ordered before first use)
-cudaError_t ensure_heur32(cudaStream_t stream) {
+// grid of a kernel that loops over its work: `want` CTAs, but no more than `ctas_per_sm` per SM
+int capped_grid(int64_t want, int ctas_per_sm) {
+    const int64_t cap = int64_t(num_sms()) * ctas_per_sm;
+    return int(want < cap ? want : cap);
+}
+
+inline int cuda_fail(cudaError_t e) {
+    g_last_err = e;
+    return NASTAR_ECUDA;
+}
+
+// the last step of every entry point that launched a kernel: the launch counts once issued, then its error is read
+int launched() {
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? NASTAR_OK : cuda_fail(e);
+}
+
+// opts `kernel` in to `smem` bytes of dynamic shared memory, then launches it; returns the opt-in's error (the launch's
+// own error is left for launched())
+template <class... P, class... A>
+cudaError_t launch_smem(void (*kernel)(P...), int grid, int block, size_t smem, cudaStream_t stream, const A&... args) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e == cudaSuccess) kernel<<<grid, block, smem, stream>>>(args...);
+    return e;
+}
+
+// f(std::bool_constant<flags>...): turns runtime flags into template arguments, one instantiation per combination
+template <class F>
+auto with_flags(F&& f) {
+    return f();
+}
+template <class F, class... Rest>
+auto with_flags(F&& f, bool flag, Rest... rest) {
+    if (flag) return with_flags([&](auto... t) { return f(std::true_type{}, t...); }, rest...);
+    return with_flags([&](auto... t) { return f(std::false_type{}, t...); }, rest...);
+}
+
+// one-time fill of the kSide x kSide heuristic table (g_heur32 / g_heur64) on the current device, stream-ordered
+// before first use; each table has its own per-device done mask
+template <int kSide>
+cudaError_t ensure_heur(cudaStream_t stream) {
     static std::atomic<uint64_t> done_mask{0};
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
     const uint64_t bit = uint64_t(1) << (dev & 63);
     if (done_mask.load(std::memory_order_acquire) & bit) return cudaSuccess;
-    nastar::heur32_init_kernel<<<4, 256, 0, stream>>>();
+    auto* const init = kSide == 32 ? nastar::heur32_init_kernel : nastar::heur64_init_kernel;
+    init<<<kSide * kSide / 256, 256, 0, stream>>>();
+    g_launches.fetch_add(1, std::memory_order_relaxed);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     // later launches on OTHER streams must also see the table: finish the fill before publishing
     e = cudaStreamSynchronize(stream);
     if (e != cudaSuccess) return e;
     done_mask.fetch_or(bit, std::memory_order_release);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaSuccess;
 }
 
-cudaError_t ensure_heur64(cudaStream_t stream) {
-    static std::atomic<uint64_t> done_mask{0};
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    const uint64_t bit = uint64_t(1) << (dev & 63);
-    if (done_mask.load(std::memory_order_acquire) & bit) return cudaSuccess;
-    nastar::heur64_init_kernel<<<16, 256, 0, stream>>>();
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    e = cudaStreamSynchronize(stream);
-    if (e != cudaSuccess) return e;
-    done_mask.fetch_or(bit, std::memory_order_release);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return cudaSuccess;
+// W32Args / W64Args / GenArgs of a backward call: the search inputs in `f`, then the backward-only fields
+template <class A>
+A bwd_kernel_args(const nastar_bwd_params* p) {
+    A a{};
+    a.f.cost = p->cost;   a.f.cost_stride = p->cost_stride;
+    a.f.start = p->start; a.f.start_stride = p->start_stride;
+    a.f.goal = p->goal;   a.f.goal_stride = p->goal_stride;
+    a.f.obst = p->obst;   a.f.obst_stride = p->obst_stride;
+    a.f.B = p->B; a.f.H = p->H; a.f.W = p->W;
+    a.f.g_ratio = p->g_ratio;
+    a.f.one_minus_g_ratio = p->one_minus_g_ratio;
+    a.f.T = 0;   // the loop bound comes from *T_batch on the device
+    a.f.workspace = p->workspace;
+    a.f.workspace_bytes = p->workspace_bytes;
+    a.sqrt_w = p->sqrt_w;
+    a.T_batch = p->T_batch;
+    a.t_solve_in = p->t_solve;
+    a.grad_hist = p->grad_histories;
+    a.grad_stride = p->grad_stride;
+    a.grad_cost = p->grad_cost;
+    return a;
 }
 
 // generic engine variant for a shape: 2 = state in shared memory, 3 = state in the HBM workspace, 0 = too large
@@ -80,10 +128,7 @@ int generic_engine_for(int32_t H, int32_t W) {
     return 0;
 }
 
-int generic_slots(int B) {
-    const int cap = num_sms() * kGlobalCtasPerSm;
-    return B < cap ? B : cap;
-}
+int generic_slots(int B) { return capped_grid(B, kGlobalCtasPerSm); }
 
 // ---- engine 5 (nastar_bin16.cuh): binary-cost maps, one CTA per map --------------------------------------
 // NASTAR_B200_BIN16=0 in the environment disables it (A/B measurements against engines 2/3)
@@ -105,11 +150,6 @@ bool bin16_shape_ok(int32_t H, int32_t W) {
 
 // head of the workspace when engine 5 may run: [0,256) work-queue counter, then B redo flags (256-B granules)
 size_t bin16_aux_bytes(int32_t B) { return 256 + ((size_t(B) * 4 + 255) & ~size_t(255)); }
-
-inline int cuda_fail(cudaError_t e) {
-    g_last_err = e;
-    return NASTAR_ECUDA;
-}
 
 __global__ void batch_steps_kernel(const int32_t* __restrict__ t_solve, const int32_t* __restrict__ n_steps,
                                    int B, int T, int32_t* __restrict__ out) {
@@ -133,17 +173,13 @@ __global__ void batch_steps_kernel(const int32_t* __restrict__ t_solve, const in
         if (threadIdx.x == 0) out[0] = min(m, T);
     }
 }
-}  // namespace
 
-namespace {
 template <int C>
-cudaError_t launch_head(const float* x, int64_t P, const float* w_host, float* taps, cudaStream_t stream) {
+void launch_head(const float* x, int64_t P, const float* w_host, float* taps, cudaStream_t stream) {
     nastar::HeadWeights<C> hw;
     for (int i = 0; i < C * 9; ++i) hw.w[i] = w_host[i];
     const int64_t want = ((P + 31) / 32 + nastar::kHeadWarps - 1) / nastar::kHeadWarps;   // one 32-pixel group per warp
-    const int64_t cap = int64_t(num_sms()) * 16;
-    nastar::head_taps_kernel<C><<<unsigned(want < cap ? want : cap), 32 * nastar::kHeadWarps, 0, stream>>>(x, P, hw, taps);
-    return cudaGetLastError();
+    nastar::head_taps_kernel<C><<<capped_grid(want, 16), 32 * nastar::kHeadWarps, 0, stream>>>(x, P, hw, taps);
 }
 }  // namespace
 
@@ -209,108 +245,76 @@ int nastar_b200_forward(const nastar_fwd_params* p, void* stream_v) {
         cudaError_t e = cudaMemsetAsync(p->trace, 0xFF, size_t(nmaps) * size_t(p->T) * sizeof(int32_t), stream);
         if (e != cudaSuccess) return cuda_fail(e);
     }
+    const bool trace = p->trace != nullptr;
+    const bool noexit = (p->flags & NASTAR_FWD_NO_EARLY_EXIT) != 0;
+    const bool fused = p->cost_kind != NASTAR_COST_PLANE;
     if (engine == 1) {
-        cudaError_t he = ensure_heur32(stream);
-        if (he != cudaSuccess) return cuda_fail(he);
+        const cudaError_t e = ensure_heur<32>(stream);
+        if (e != cudaSuccess) return cuda_fail(e);
         nastar::W32Args a{};
         a.f = *p;
-        const bool noexit = (p->flags & NASTAR_FWD_NO_EARLY_EXIT) != 0;
-        const bool fused = (p->cost_kind != NASTAR_COST_PLANE);
-        auto go = [&](auto kernel) { kernel<<<nmaps, 32, 0, stream>>>(a); };
-        if (fused) {
-            if (p->trace) { if (noexit) go(nastar::astar_warp32_kernel<true, false, true, true>); else go(nastar::astar_warp32_kernel<true, false, false, true>); }
-            else          { if (noexit) go(nastar::astar_warp32_kernel<false, false, true, true>); else go(nastar::astar_warp32_kernel<false, false, false, true>); }
-        } else {
-            if (p->trace) { if (noexit) go(nastar::astar_warp32_kernel<true, false, true>); else go(nastar::astar_warp32_kernel<true, false, false>); }
-            else          { if (noexit) go(nastar::astar_warp32_kernel<false, false, true>); else go(nastar::astar_warp32_kernel<false, false, false>); }
-        }
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-    } else if (engine == 4) {
-        cudaError_t he = ensure_heur64(stream);
-        if (he != cudaSuccess) return cuda_fail(he);
-        const bool noexit = (p->flags & NASTAR_FWD_NO_EARLY_EXIT) != 0;
-        const size_t smem = sizeof(nastar::W64Smem);
+        with_flags([&](auto kTrace, auto kNoExit, auto kFused) {
+            nastar::astar_warp32_kernel<kTrace, false, kNoExit, kFused><<<nmaps, 32, 0, stream>>>(a);
+        }, trace, noexit, fused);
+        return launched();
+    }
+    if (engine == 4) {
+        cudaError_t e = ensure_heur<64>(stream);
+        if (e != cudaSuccess) return cuda_fail(e);
         nastar::W64Args wa{};
         wa.f = *p;
-        auto launch = [&](auto kernel) -> cudaError_t {
-            cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-            if (e != cudaSuccess) return e;
-            kernel<<<p->B, 32, smem, stream>>>(wa);
-            return cudaSuccess;
-        };
-        cudaError_t e;
-        if (p->cost_kind != NASTAR_COST_PLANE) {
-            if (p->trace) e = noexit ? launch(nastar::astar_warp64_kernel<true, true, false, true>) : launch(nastar::astar_warp64_kernel<true, false, false, true>);
-            else e = noexit ? launch(nastar::astar_warp64_kernel<false, true, false, true>) : launch(nastar::astar_warp64_kernel<false, false, false, true>);
-        } else if (p->trace) e = noexit ? launch(nastar::astar_warp64_kernel<true, true>) : launch(nastar::astar_warp64_kernel<true, false>);
-        else e = noexit ? launch(nastar::astar_warp64_kernel<false, true>) : launch(nastar::astar_warp64_kernel<false, false>);
+        e = with_flags([&](auto kTrace, auto kNoExit, auto kFused) {
+            return launch_smem(nastar::astar_warp64_kernel<kTrace, kNoExit, false, kFused>, p->B, 32,
+                               sizeof(nastar::W64Smem), stream, wa);
+        }, trace, noexit, fused);
         if (e != cudaSuccess) return cuda_fail(e);
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-    } else {
-        const nastar::GenericLayout L(p->H, p->W);
-        const bool global = (engine == 3);
-        const size_t smem = L.smem_common() + (global ? 0 : L.smem_planes());
-        int grid = p->B;
-        const size_t slots_bytes = global ? size_t(generic_slots(p->B)) * L.slot_bytes() : 0;
-        if (global) {
-            grid = generic_slots(p->B);
-            if (!p->workspace || p->workspace_bytes < slots_bytes) return NASTAR_EWORKSPACE;
-        }
-        nastar::GenArgs ga{};
-        ga.f = *p;
-        // engine 5 first when the cost plane IS the binary obstacle plane (VanillaAstar / Config 5): whole map on
-        // chip, one CTA per SM pulling maps from a queue; maps it flags are re-run below by the generic engine
-        const bool aliased = (p->obst == p->cost) && (p->obst_stride == p->cost_stride);
-        const size_t aux = bin16_aux_bytes(p->B);
-        if (bin16_enabled() && aliased && !p->trace && p->flags == 0 && bin16_shape_ok(p->H, p->W) && p->workspace &&
-            p->workspace_bytes >= aux + slots_bytes) {
-            unsigned char* ws = static_cast<unsigned char*>(p->workspace);
-            nastar::Bin16Args ba{};
-            ba.f = *p;
-            ba.queue = reinterpret_cast<int32_t*>(ws);
-            ba.redo = reinterpret_cast<int32_t*>(ws + 256);
-            cudaError_t e = cudaMemsetAsync(ba.queue, 0, 256, stream);
-            if (e != cudaSuccess) return cuda_fail(e);
-            const size_t bsmem = nastar::Bin16Layout(p->H, p->W).smem_bytes();
-            auto launch16 = [&](auto kernel) -> cudaError_t {
-                cudaError_t e2 = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bsmem));
-                if (e2 != cudaSuccess) return e2;
-                int per_sm = 1;   // resident CTAs per SM (1 at 256x256, a few for smaller maps)
-                e2 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, nastar::kBin16Threads, bsmem);
-                if (e2 != cudaSuccess) return e2;
-                per_sm = per_sm < 1 ? 1 : per_sm;
-                const int bgrid = p->B < num_sms() * per_sm ? p->B : num_sms() * per_sm;
-                kernel<<<bgrid, nastar::kBin16Threads, bsmem, stream>>>(ba);
-                return cudaGetLastError();
-            };
-            e = (p->H <= 256) ? launch16(nastar::astar_bin16_kernel<8>) : launch16(nastar::astar_bin16_kernel<16>);
-            if (e != cudaSuccess) return cuda_fail(e);
-            g_launches.fetch_add(1, std::memory_order_relaxed);
-            ga.redo = ba.redo;
-            ga.f.workspace = ws + aux;
-            ga.f.workspace_bytes = p->workspace_bytes - aux;
-        }
-        auto launch = [&](auto kernel) -> cudaError_t {
-            cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-            if (e != cudaSuccess) return e;
-            kernel<<<grid, 32, smem, stream>>>(ga);
-            return cudaSuccess;
-        };
-        const bool noexit = (p->flags & NASTAR_FWD_NO_EARLY_EXIT) != 0;
-        cudaError_t e;
-        if (noexit) {
-            if (global) e = p->trace ? launch(nastar::astar_generic_kernel<true, true, false, true>) : launch(nastar::astar_generic_kernel<true, false, false, true>);
-            else e = p->trace ? launch(nastar::astar_generic_kernel<false, true, false, true>) : launch(nastar::astar_generic_kernel<false, false, false, true>);
-        } else {
-            if (global) e = p->trace ? launch(nastar::astar_generic_kernel<true, true, false>) : launch(nastar::astar_generic_kernel<true, false, false>);
-            else e = p->trace ? launch(nastar::astar_generic_kernel<false, true, false>) : launch(nastar::astar_generic_kernel<false, false, false>);
-        }
-        if (e != cudaSuccess) return cuda_fail(e);
-        g_launches.fetch_add(1, std::memory_order_relaxed);
+        return launched();
     }
-    cudaError_t e = cudaGetLastError();
+    const nastar::GenericLayout L(p->H, p->W);
+    const bool global = (engine == 3);
+    const size_t smem = L.smem_common() + (global ? 0 : L.smem_planes());
+    const int grid = global ? generic_slots(p->B) : p->B;
+    const size_t slots_bytes = global ? size_t(grid) * L.slot_bytes() : 0;
+    if (global && (!p->workspace || p->workspace_bytes < slots_bytes)) return NASTAR_EWORKSPACE;
+    nastar::GenArgs ga{};
+    ga.f = *p;
+    // engine 5 first when the cost plane IS the binary obstacle plane (VanillaAstar / Config 5): whole map on
+    // chip, one CTA per SM pulling maps from a queue; maps it flags are re-run below by the generic engine
+    const bool aliased = (p->obst == p->cost) && (p->obst_stride == p->cost_stride);
+    const size_t aux = bin16_aux_bytes(p->B);
+    if (bin16_enabled() && aliased && !p->trace && p->flags == 0 && bin16_shape_ok(p->H, p->W) && p->workspace &&
+        p->workspace_bytes >= aux + slots_bytes) {
+        unsigned char* ws = static_cast<unsigned char*>(p->workspace);
+        nastar::Bin16Args ba{};
+        ba.f = *p;
+        ba.queue = reinterpret_cast<int32_t*>(ws);
+        ba.redo = reinterpret_cast<int32_t*>(ws + 256);
+        cudaError_t e = cudaMemsetAsync(ba.queue, 0, 256, stream);
+        if (e != cudaSuccess) return cuda_fail(e);
+        const size_t bsmem = nastar::Bin16Layout(p->H, p->W).smem_bytes();
+        auto launch16 = [&](auto kernel) -> cudaError_t {
+            // the occupancy query needs the shared-memory opt-in, and the grid needs the occupancy
+            cudaError_t e2 = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bsmem));
+            if (e2 != cudaSuccess) return e2;
+            int per_sm = 1;   // resident CTAs per SM (1 at 256x256, a few for smaller maps)
+            e2 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, nastar::kBin16Threads, bsmem);
+            if (e2 != cudaSuccess) return e2;
+            kernel<<<capped_grid(p->B, per_sm < 1 ? 1 : per_sm), nastar::kBin16Threads, bsmem, stream>>>(ba);
+            return cudaSuccess;
+        };
+        e = (p->H <= 256) ? launch16(nastar::astar_bin16_kernel<8>) : launch16(nastar::astar_bin16_kernel<16>);
+        if (e != cudaSuccess) return cuda_fail(e);
+        const int st = launched();
+        if (st != NASTAR_OK) return st;
+        ga.redo = ba.redo;
+        ga.f.workspace = ws + aux;
+        ga.f.workspace_bytes = p->workspace_bytes - aux;
+    }
+    const cudaError_t e = with_flags([&](auto kGlobal, auto kTrace, auto kNoExit) {
+        return launch_smem(nastar::astar_generic_kernel<kGlobal, kTrace, false, kNoExit>, grid, 32, smem, stream, ga);
+    }, global, trace, noexit);
     if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    return launched();
 }
 
 int nastar_b200_backward(const nastar_bwd_params* p, void* stream_v) {
@@ -319,116 +323,42 @@ int nastar_b200_backward(const nastar_bwd_params* p, void* stream_v) {
         return NASTAR_EINVAL;
     if (p->B <= 0 || p->H <= 0 || p->W <= 0) return NASTAR_EINVAL;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-    int engine = nastar_b200_engine_for(p->H, p->W);
-    if (engine == 4) {
-        // warp-resident 64-wide engine: event-based closed form next to the forward state in shared memory
-        cudaError_t he = ensure_heur64(stream);
-        if (he != cudaSuccess) return cuda_fail(he);
-        nastar::W64Args wa{};
-        wa.f.cost = p->cost;   wa.f.cost_stride = p->cost_stride;
-        wa.f.start = p->start; wa.f.start_stride = p->start_stride;
-        wa.f.goal = p->goal;   wa.f.goal_stride = p->goal_stride;
-        wa.f.obst = p->obst;   wa.f.obst_stride = p->obst_stride;
-        wa.f.B = p->B; wa.f.H = p->H; wa.f.W = p->W;
-        wa.f.g_ratio = p->g_ratio;
-        wa.f.one_minus_g_ratio = p->one_minus_g_ratio;
-        wa.f.T = 0;   // the loop bound comes from *T_batch on the device
-        wa.sqrt_w = p->sqrt_w;
-        wa.T_batch = p->T_batch;
-        wa.t_solve_in = p->t_solve;
-        wa.grad_hist = p->grad_histories;
-        wa.grad_stride = p->grad_stride;
-        wa.grad_cost = p->grad_cost;
-        const size_t smem = sizeof(nastar::W64Smem) + sizeof(nastar::W64Bwd);
-        cudaError_t e = cudaFuncSetAttribute(nastar::astar_warp64_kernel<false, false, true>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-        if (e != cudaSuccess) return cuda_fail(e);
-        nastar::astar_warp64_kernel<false, false, true><<<p->B, 32, smem, stream>>>(wa);
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return cuda_fail(e);
-        return NASTAR_OK;
-    }
-    if (engine != 1) engine = generic_engine_for(p->H, p->W);
+    const int engine = nastar_b200_engine_for(p->H, p->W);
     if (engine == 0) return NASTAR_EUNSUPPORTED;
-    if (engine >= 2) {
+    cudaError_t e;
+    if (engine == 1) {
+        // dynamic shared memory = the per-cell interval state of the event-based closed form (W32Bwd, 32 KB); with the
+        // 17.4 KB of static planes that is above the 48 KB default, hence the opt-in
+        e = ensure_heur<32>(stream);
+        if (e == cudaSuccess)
+            e = launch_smem(nastar::astar_warp32_kernel<false, true>, p->B, 32, sizeof(nastar::W32Bwd), stream,
+                            bwd_kernel_args<nastar::W32Args>(p));
+    } else if (engine == 4) {
+        // warp-resident 64-wide engine: event-based closed form next to the forward state in shared memory
+        e = ensure_heur<64>(stream);
+        if (e == cudaSuccess)
+            e = launch_smem(nastar::astar_warp64_kernel<false, false, true>, p->B, 32,
+                            sizeof(nastar::W64Smem) + sizeof(nastar::W64Bwd), stream, bwd_kernel_args<nastar::W64Args>(p));
+    } else {
         const nastar::GenericLayout L(p->H, p->W);
         const bool global = (engine == 3);
         const int grid = generic_slots(p->B);
         if (!p->workspace || p->workspace_bytes < size_t(grid) * L.slot_total(global, true)) return NASTAR_EWORKSPACE;
-        nastar::GenArgs ga{};
-        ga.f.cost = p->cost;   ga.f.cost_stride = p->cost_stride;
-        ga.f.start = p->start; ga.f.start_stride = p->start_stride;
-        ga.f.goal = p->goal;   ga.f.goal_stride = p->goal_stride;
-        ga.f.obst = p->obst;   ga.f.obst_stride = p->obst_stride;
-        ga.f.B = p->B; ga.f.H = p->H; ga.f.W = p->W;
-        ga.f.g_ratio = p->g_ratio;
-        ga.f.one_minus_g_ratio = p->one_minus_g_ratio;
-        ga.f.workspace = p->workspace;
-        ga.f.workspace_bytes = p->workspace_bytes;
-        ga.sqrt_w = p->sqrt_w;
-        ga.T_batch = p->T_batch;
-        ga.t_solve_in = p->t_solve;
-        ga.grad_hist = p->grad_histories;
-        ga.grad_stride = p->grad_stride;
-        ga.grad_cost = p->grad_cost;
         const size_t smem = L.smem_common() + (global ? 0 : L.smem_planes());
-        cudaError_t e;
-        if (global) {
-            e = cudaFuncSetAttribute(nastar::astar_generic_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-            if (e == cudaSuccess) nastar::astar_generic_kernel<true, false, true><<<grid, 32, smem, stream>>>(ga);
-        } else {
-            e = cudaFuncSetAttribute(nastar::astar_generic_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-            if (e == cudaSuccess) nastar::astar_generic_kernel<false, false, true><<<grid, 32, smem, stream>>>(ga);
-        }
-        if (e != cudaSuccess) return cuda_fail(e);
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return cuda_fail(e);
-        return NASTAR_OK;
+        const nastar::GenArgs ga = bwd_kernel_args<nastar::GenArgs>(p);
+        e = with_flags([&](auto kGlobal) {
+            return launch_smem(nastar::astar_generic_kernel<kGlobal, false, true>, grid, 32, smem, stream, ga);
+        }, global);
     }
-    {
-        cudaError_t he = ensure_heur32(stream);
-        if (he != cudaSuccess) return cuda_fail(he);
-    }
-    nastar::W32Args a{};
-    a.f.cost = p->cost;   a.f.cost_stride = p->cost_stride;
-    a.f.start = p->start; a.f.start_stride = p->start_stride;
-    a.f.goal = p->goal;   a.f.goal_stride = p->goal_stride;
-    a.f.obst = p->obst;   a.f.obst_stride = p->obst_stride;
-    a.f.B = p->B; a.f.H = p->H; a.f.W = p->W;
-    a.f.g_ratio = p->g_ratio;
-    a.f.one_minus_g_ratio = p->one_minus_g_ratio;
-    a.f.T = 0;  // the loop bound comes from *T_batch on the device
-    a.sqrt_w = p->sqrt_w;
-    a.T_batch = p->T_batch;
-    a.t_solve_in = p->t_solve;
-    a.grad_hist = p->grad_histories;
-    a.grad_stride = p->grad_stride;
-    a.grad_cost = p->grad_cost;
-    // dynamic shared memory = the per-cell interval state of the event-based closed form (W32Bwd, 32 KB); with the
-    // 17.4 KB of static planes that is above the 48 KB default, hence the opt-in
-    {
-        cudaError_t ea = cudaFuncSetAttribute(nastar::astar_warp32_kernel<false, true>,
-                                              cudaFuncAttributeMaxDynamicSharedMemorySize, int(sizeof(nastar::W32Bwd)));
-        if (ea != cudaSuccess) return cuda_fail(ea);
-    }
-    nastar::astar_warp32_kernel<false, true><<<p->B, 32, sizeof(nastar::W32Bwd), stream>>>(a);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    return launched();
 }
 
 int nastar_b200_batch_steps(const int32_t* t_solve, const int32_t* n_steps, int32_t B, int32_t T, int32_t* T_batch,
                             void* stream_v) {
     if (!t_solve || !T_batch || B <= 0 || T < 1) return NASTAR_EINVAL;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-    batch_steps_kernel<<<1, 256, 0, stream>>>(t_solve, n_steps, B, T, T_batch);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    batch_steps_kernel<<<1, 256, 0, static_cast<cudaStream_t>(stream_v)>>>(t_solve, n_steps, B, T, T_batch);
+    return launched();
 }
 
 int nastar_b200_pack_inputs(const float* map_designs, int32_t C, int32_t Hm, int32_t Wm, const float* start,
@@ -438,30 +368,19 @@ int nastar_b200_pack_inputs(const float* map_designs, int32_t C, int32_t Hm, int
         return NASTAR_EINVAL;
     if ((C == 1 && (reinterpret_cast<uintptr_t>(out) & 7)) || (C == 3 && (reinterpret_cast<uintptr_t>(out) & 15)))
         return NASTAR_EINVAL;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
     const int64_t npix = int64_t(B) * Hm * Wm;
-    const int64_t want = (npix + 255) / 256;
-    const int grid = int(want < int64_t(num_sms()) * 16 ? want : int64_t(num_sms()) * 16);
-    nastar::pack_inputs_kernel<<<grid, 256, 0, stream>>>(map_designs, C, Hm, Wm, start, start_stride, goal, goal_stride,
-                                                         B, H, W, out);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    nastar::pack_inputs_kernel<<<capped_grid((npix + 255) / 256, 16), 256, 0, static_cast<cudaStream_t>(stream_v)>>>(
+        map_designs, C, Hm, Wm, start, start_stride, goal, goal_stride, B, H, W, out);
+    return launched();
 }
 
 int nastar_b200_cost_from_taps(const float* taps, int32_t B, int32_t H, int32_t W, float bias, float scale,
                                float* cost, void* stream_v) {
     if (!taps || !cost || B <= 0 || H <= 0 || W <= 0) return NASTAR_EINVAL;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
     const int64_t total = int64_t(B) * H * W;
-    const int64_t want = (total + 255) / 256;
-    const int grid = int(want < int64_t(num_sms()) * 16 ? want : int64_t(num_sms()) * 16);
-    nastar::cost_from_taps_kernel<<<grid, 256, 0, stream>>>(taps, B, H, W, bias, scale, cost);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    nastar::cost_from_taps_kernel<<<capped_grid((total + 255) / 256, 16), 256, 0, static_cast<cudaStream_t>(stream_v)>>>(
+        taps, B, H, W, bias, scale, cost);
+    return launched();
 }
 
 int nastar_b200_conv1_marks(const float* map_designs, const float* start, int64_t start_stride, const float* goal,
@@ -471,35 +390,27 @@ int nastar_b200_conv1_marks(const float* map_designs, const float* start, int64_
     if (reinterpret_cast<uintptr_t>(out) & 15) return NASTAR_EINVAL;
     const int64_t n_pix = int64_t(B) * H * W;
     if (n_pix > (int64_t(1) << 30)) return NASTAR_EINVAL;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
     nastar::Conv1Weights cw;
     std::memcpy(cw.w, w_host, sizeof(cw.w));
     std::memcpy(cw.b, bias_host, sizeof(cw.b));
     const int64_t want = (n_pix + 32 * nastar::kConv1Warps - 1) / (32 * nastar::kConv1Warps);
-    const int grid = int(want < int64_t(num_sms()) * 8 ? want : int64_t(num_sms()) * 8);
-    nastar::conv1_marks_kernel<<<grid, 32 * nastar::kConv1Warps, 0, stream>>>(map_designs, start, start_stride, goal,
-                                                                             goal_stride, int(n_pix), H, W, cw, out);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    nastar::conv1_marks_kernel<<<capped_grid(want, 8), 32 * nastar::kConv1Warps, 0, static_cast<cudaStream_t>(stream_v)>>>(
+        map_designs, start, start_stride, goal, goal_stride, int(n_pix), H, W, cw, out);
+    return launched();
 }
 
 int nastar_b200_head_taps(const float* x, int64_t P, int32_t C, const float* w_host, float* taps, void* stream_v) {
     if (!x || !w_host || !taps || P <= 0 || (reinterpret_cast<uintptr_t>(x) & 15)) return NASTAR_EINVAL;
     if (P > (int64_t(1) << 31) * 127) return NASTAR_EINVAL;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-    cudaError_t e;
     switch (C) {
-        case 32: e = launch_head<32>(x, P, w_host, taps, stream); break;
-        case 64: e = launch_head<64>(x, P, w_host, taps, stream); break;
-        case 128: e = launch_head<128>(x, P, w_host, taps, stream); break;
-        case 256: e = launch_head<256>(x, P, w_host, taps, stream); break;
+        case 32: launch_head<32>(x, P, w_host, taps, stream); break;
+        case 64: launch_head<64>(x, P, w_host, taps, stream); break;
+        case 128: launch_head<128>(x, P, w_host, taps, stream); break;
+        case 256: launch_head<256>(x, P, w_host, taps, stream); break;
         default: return NASTAR_EUNSUPPORTED;
     }
-    if (e != cudaSuccess) return cuda_fail(e);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return NASTAR_OK;
+    return launched();
 }
 
 int nastar_b200_conv3x3_head_taps(const float* x, int32_t B, int32_t H, int32_t W, int32_t C_in, int32_t C_out,
@@ -511,19 +422,16 @@ int nastar_b200_conv3x3_head_taps(const float* x, int32_t B, int32_t H, int32_t 
     if (C_in != nastar::kCHCin || C_out != nastar::kCHCout) return NASTAR_EUNSUPPORTED;
     if (H > nastar::kCHMaxSide || W > nastar::kCHMaxSide) return NASTAR_EUNSUPPORTED;
     if (int64_t(B) * H * W > (int64_t(1) << 30)) return NASTAR_EINVAL;
+    // the launcher sets up tensor maps and the cluster grid first; any error, the launch's included, comes back here
     cudaError_t e = nastar::conv3x3_head_launch(x, B, H, W, w, bias, head_w_host, taps, static_cast<cudaStream_t>(stream_v));
     if (e != cudaSuccess) return cuda_fail(e);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return NASTAR_OK;
+    return launched();
 }
 
 int nastar_b200_selftest_sqrt(int32_t n, int32_t* mismatches, void* stream_v) {
     if (n <= 0 || !mismatches) return NASTAR_EINVAL;
     nastar::sqrt_rn_int_check_kernel<<<num_sms() * 4, 256, 0, static_cast<cudaStream_t>(stream_v)>>>(n, mismatches);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    return launched();
 }
 
 int nastar_b200_opt_labels(const float* maps, int64_t map_stride, const int32_t* goal_idx, int32_t B, int32_t H,
@@ -531,16 +439,11 @@ int nastar_b200_opt_labels(const float* maps, int64_t map_stride, const int32_t*
     if (!maps || !goal_idx || !dists || !act_mask || !action || B <= 0 || H <= 0 || W <= 0) return NASTAR_EINVAL;
     if (map_stride < int64_t(H) * W) return NASTAR_EINVAL;
     if (H > nastar::kLabelsMaxSide || W > nastar::kLabelsMaxSide) return NASTAR_EUNSUPPORTED;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-    const size_t smem = nastar::labels_smem_bytes(H, W);
-    cudaError_t e = cudaFuncSetAttribute(nastar::opt_labels_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    const nastar::LabelsArgs a{maps, map_stride, goal_idx, B, H, W, dists, act_mask, action};
+    const cudaError_t e = launch_smem(nastar::opt_labels_kernel, B, nastar::labels_threads(H, W),
+                                      nastar::labels_smem_bytes(H, W), static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
-    nastar::LabelsArgs a{maps, map_stride, goal_idx, B, H, W, dists, act_mask, action};
-    nastar::opt_labels_kernel<<<B, nastar::labels_threads(H, W), smem, stream>>>(a);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    return launched();
 }
 
 int nastar_b200_weighted_labels(const float* cost, int64_t cost_stride, const float* passable, int64_t passable_stride,
@@ -554,18 +457,12 @@ int nastar_b200_weighted_labels(const float* cost, int64_t cost_stride, const fl
     if (bool(start_idx) != bool(path_maps) || bool(start_idx) != bool(path_costs)) return NASTAR_EINVAL;
     if (H > nastar::kWLabelsMaxSide || W > nastar::kWLabelsMaxSide || int64_t(H) * W > nastar::kWLabelsMaxCells)
         return NASTAR_EUNSUPPORTED;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-    const size_t smem = nastar::wlabels_smem_bytes(H, W);
-    cudaError_t e =
-        cudaFuncSetAttribute(nastar::weighted_labels_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    const nastar::WLabelsArgs a{cost,   cost_stride, passable,  passable_stride, goal_idx,   start_idx, B,     H, W,
+                                dists,  hops,        act_mask,  action,          path_maps,  path_costs, status};
+    const cudaError_t e = launch_smem(nastar::weighted_labels_kernel, B, nastar::wlabels_threads(H, W),
+                                      nastar::wlabels_smem_bytes(H, W), static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
-    nastar::WLabelsArgs a{cost,   cost_stride, passable,  passable_stride, goal_idx,   start_idx, B,     H, W,
-                          dists,  hops,        act_mask,  action,          path_maps,  path_costs, status};
-    nastar::weighted_labels_kernel<<<B, nastar::wlabels_threads(H, W), smem, stream>>>(a);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    return launched();
 }
 
 int nastar_b200_sampler_prepare(const float* dists, const float* policies, const float* goal_maps, int32_t B, int32_t H,
@@ -582,10 +479,7 @@ int nastar_b200_sampler_prepare(const float* dists, const float* policies, const
     nastar::SamplerPrepArgs a{dists, policies, goal_maps, B, H, W, {q0, q1, q2, q3}, band_bits, band_counts, goal_idx,
                               actions, thresholds, status};
     nastar::sampler_prepare_kernel<<<B, nastar::kSamplerPrepThreads, 0, static_cast<cudaStream_t>(stream_v)>>>(a);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    return launched();
 }
 
 int nastar_b200_sampler_sample(const float* maps, const float* goal_maps, int32_t n_maps, int32_t H, int32_t W,
@@ -608,16 +502,13 @@ int nastar_b200_sampler_sample(const float* maps, const float* goal_maps, int32_
     while (chunk > 1 && chunk * traj + act > kMaxDynSmem) --chunk;
     const int stage = chunk * traj + act <= kMaxDynSmem ? 1 : 0;
     const size_t smem = chunk * traj + (stage ? act : 0);
-    cudaError_t e = cudaFuncSetAttribute(nastar::sampler_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    const nastar::SamplerArgs a{maps, goal_maps, band_bits, band_counts, goal_idx, actions, indices,
+                                reinterpret_cast<const uint32_t*>(draws), n_maps, H, W, B, S, chunk, stage,
+                                out_maps, out_starts, out_goals, out_trajs};
+    const cudaError_t e = launch_smem(nastar::sampler_sample_kernel, B, nastar::kSamplerThreads, smem,
+                                      static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
-    nastar::SamplerArgs a{maps, goal_maps, band_bits, band_counts, goal_idx, actions, indices,
-                          reinterpret_cast<const uint32_t*>(draws), n_maps, H, W, B, S, chunk, stage,
-                          out_maps, out_starts, out_goals, out_trajs};
-    nastar::sampler_sample_kernel<<<B, nastar::kSamplerThreads, smem, static_cast<cudaStream_t>(stream_v)>>>(a);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e);
-    return NASTAR_OK;
+    return launched();
 }
 
 uint64_t nastar_b200_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }

@@ -53,12 +53,6 @@ struct GenArgs {
     const int32_t* redo;
 };
 
-__device__ __forceinline__ float gen_warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-    return v;
-}
-
 // kBwd = true replays the search for *T_batch steps and accumulates the closed-form gradient (SURVEY App. B)
 //   dL/dcost[p] = -(1-g_ratio)/sqrt(W) * sum_t y_t[p] * (Gh[p] - <Gh, y_t>),   y_t = v_t / S_t over the open set,
 // EVENT-BASED: v_t[p] = exp(-f_t[p]/sqrt(W)) only changes when p is opened, relaxed or closed, so a cell's

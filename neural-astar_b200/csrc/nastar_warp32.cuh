@@ -50,12 +50,6 @@ __global__ void heur32_init_kernel() {
     if (i < kCells) g_heur32[i] = heuristic(i >> 5, i & 31, 0, 0);
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-    return v;
-}
-
 // backward-only planes (dynamic shared memory), event-based closed form (see nastar_generic.cuh / DESIGN.md):
 struct __align__(16) W32Bwd {
     double acc[kCells];   // closed intervals: sum of v * (Gh * dA - dB)

@@ -22,8 +22,6 @@ NASTAR_OK = 0
 TS_CAPPED = -1
 TS_EXHAUSTED = -2
 
-_f32p = ctypes.POINTER(ctypes.c_float)
-
 
 class FwdParams(ctypes.Structure):
     """struct nastar_fwd_params (include/nastar_b200.h)"""
@@ -61,29 +59,33 @@ class BwdParams(ctypes.Structure):
     ]
 
 
-EXPORTS = (
-    "nastar_b200_abi_version",
-    "nastar_b200_forward_workspace_bytes",
-    "nastar_b200_backward_workspace_bytes",
-    "nastar_b200_forward",
-    "nastar_b200_backward",
-    "nastar_b200_batch_steps",
-    "nastar_b200_engine_for",
-    "nastar_b200_bin16_supported",
-    "nastar_b200_pack_inputs",
-    "nastar_b200_cost_from_taps",
-    "nastar_b200_head_taps",
-    "nastar_b200_conv1_marks",
-    "nastar_b200_conv3x3_head_taps",
-    "nastar_b200_selftest_sqrt",
-    "nastar_b200_opt_labels",
-    "nastar_b200_weighted_labels",
-    "nastar_b200_sampler_prepare",
-    "nastar_b200_sampler_sample",
-    "nastar_b200_launch_count",
-    "nastar_b200_status_string",
-    "nastar_b200_last_cuda_error",
-)
+_p, _i32, _i64, _int = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_int
+
+# every entry point of include/nastar_b200.h: symbol -> (restype, argtypes)
+_SIGNATURES = {
+    "nastar_b200_abi_version": (_int, []),
+    "nastar_b200_forward_workspace_bytes": (ctypes.c_size_t, [_i32] * 3),
+    "nastar_b200_backward_workspace_bytes": (ctypes.c_size_t, [_i32] * 3),
+    "nastar_b200_forward": (_int, [ctypes.POINTER(FwdParams), _p]),
+    "nastar_b200_backward": (_int, [ctypes.POINTER(BwdParams), _p]),
+    "nastar_b200_batch_steps": (_int, [_p, _p, _i32, _i32, _p, _p]),
+    "nastar_b200_engine_for": (_int, [_i32, _i32]),
+    "nastar_b200_bin16_supported": (_int, [_i32, _i32]),
+    "nastar_b200_pack_inputs": (_int, [_p, _i32, _i32, _i32, _p, _i64, _p, _i64, _i32, _i32, _i32, _p, _p]),
+    "nastar_b200_cost_from_taps": (_int, [_p, _i32, _i32, _i32, ctypes.c_float, ctypes.c_float, _p, _p]),
+    "nastar_b200_head_taps": (_int, [_p, _i64, _i32, _p, _p, _p]),
+    "nastar_b200_conv1_marks": (_int, [_p, _p, _i64, _p, _i64, _i32, _i32, _i32, _p, _p, _p, _p]),
+    "nastar_b200_conv3x3_head_taps": (_int, [_p] + [_i32] * 5 + [_p] * 5),
+    "nastar_b200_selftest_sqrt": (_int, [_i32, _p, _p]),
+    "nastar_b200_opt_labels": (_int, [_p, _i64, _p, _i32, _i32, _i32, _p, _p, _p, _p]),
+    "nastar_b200_weighted_labels": (_int, [_p, _i64, _p, _i64] + [_p] * 2 + [_i32] * 3 + [_p] * 8),
+    "nastar_b200_sampler_prepare": (_int, [_p] * 3 + [_i32] * 3 + [ctypes.c_double] * 4 + [_p] * 7),
+    "nastar_b200_sampler_sample": (_int, [_p] * 2 + [_i32] * 3 + [_p] * 6 + [_i32] * 2 + [_p] * 5),
+    "nastar_b200_launch_count": (ctypes.c_uint64, []),
+    "nastar_b200_status_string": (ctypes.c_char_p, [_int]),
+    "nastar_b200_last_cuda_error": (ctypes.c_char_p, []),
+}
+EXPORTS = tuple(_SIGNATURES)
 
 _lib = None
 _ws_cache = {}
@@ -105,59 +107,9 @@ def lib():
             "neural_astar (H100) has no CPU fallback."
         )
     L = ctypes.CDLL(LIB_PATH)
-    L.nastar_b200_abi_version.restype = ctypes.c_int
-    L.nastar_b200_forward_workspace_bytes.argtypes = [ctypes.c_int32] * 3
-    L.nastar_b200_forward_workspace_bytes.restype = ctypes.c_size_t
-    L.nastar_b200_backward_workspace_bytes.argtypes = [ctypes.c_int32] * 3
-    L.nastar_b200_backward_workspace_bytes.restype = ctypes.c_size_t
-    L.nastar_b200_forward.argtypes = [ctypes.POINTER(FwdParams), ctypes.c_void_p]
-    L.nastar_b200_forward.restype = ctypes.c_int
-    L.nastar_b200_backward.argtypes = [ctypes.POINTER(BwdParams), ctypes.c_void_p]
-    L.nastar_b200_backward.restype = ctypes.c_int
-    L.nastar_b200_batch_steps.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
-                                          ctypes.c_void_p, ctypes.c_void_p]
-    L.nastar_b200_batch_steps.restype = ctypes.c_int
-    L.nastar_b200_engine_for.argtypes = [ctypes.c_int32, ctypes.c_int32]
-    L.nastar_b200_engine_for.restype = ctypes.c_int
-    L.nastar_b200_bin16_supported.argtypes = [ctypes.c_int32, ctypes.c_int32]
-    L.nastar_b200_bin16_supported.restype = ctypes.c_int
-    L.nastar_b200_pack_inputs.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
-                                          ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64,
-                                          ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p,
-                                          ctypes.c_void_p]
-    L.nastar_b200_pack_inputs.restype = ctypes.c_int
-    L.nastar_b200_cost_from_taps.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
-                                             ctypes.c_float, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]
-    L.nastar_b200_cost_from_taps.restype = ctypes.c_int
-    L.nastar_b200_head_taps.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,
-                                        ctypes.c_void_p]
-    L.nastar_b200_head_taps.restype = ctypes.c_int
-    L.nastar_b200_conv1_marks.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64,
-                                          ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,
-                                          ctypes.c_void_p, ctypes.c_void_p]
-    L.nastar_b200_conv1_marks.restype = ctypes.c_int
-    L.nastar_b200_conv3x3_head_taps.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
-                                                ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p,
-                                                ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.nastar_b200_conv3x3_head_taps.restype = ctypes.c_int
-    L.nastar_b200_selftest_sqrt.argtypes = [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]
-    L.nastar_b200_selftest_sqrt.restype = ctypes.c_int
-    L.nastar_b200_opt_labels.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
-                                         ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    L.nastar_b200_opt_labels.restype = ctypes.c_int
-    L.nastar_b200_weighted_labels.argtypes = ([ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64]
-                                              + [ctypes.c_void_p] * 2 + [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 8)
-    L.nastar_b200_weighted_labels.restype = ctypes.c_int
-    L.nastar_b200_sampler_prepare.argtypes = ([ctypes.c_void_p] * 3 + [ctypes.c_int32] * 3 + [ctypes.c_double] * 4
-                                              + [ctypes.c_void_p] * 7)
-    L.nastar_b200_sampler_prepare.restype = ctypes.c_int
-    L.nastar_b200_sampler_sample.argtypes = ([ctypes.c_void_p] * 2 + [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 6
-                                             + [ctypes.c_int32] * 2 + [ctypes.c_void_p] * 5)
-    L.nastar_b200_sampler_sample.restype = ctypes.c_int
-    L.nastar_b200_launch_count.restype = ctypes.c_uint64
-    L.nastar_b200_status_string.argtypes = [ctypes.c_int]
-    L.nastar_b200_status_string.restype = ctypes.c_char_p
-    L.nastar_b200_last_cuda_error.restype = ctypes.c_char_p
+    for name, (restype, argtypes) in _SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     if L.nastar_b200_abi_version() != ABI_VERSION:
         raise ImportError(f"{LIB_PATH}: ABI {L.nastar_b200_abi_version()} != expected {ABI_VERSION}")
     _lib = L
@@ -187,6 +139,37 @@ def _plane(x: torch.Tensor) -> Tuple[torch.Tensor, int, int]:
     if x.stride(-1) != 1 or x.stride(-2) != W:
         x = x.contiguous()
     return x, x.data_ptr(), x.stride(0)
+
+
+def _set_planes(p: ctypes.Structure, planes) -> list:
+    """Write the channel-0 pointer and map stride of each (name, plane) into p.<name> / p.<name>_stride (FwdParams,
+    BwdParams).  Returns the tensors that must stay alive until the call has been issued."""
+    keep = []
+    for name, t_ in planes:
+        k, ptr, stride = _plane(t_.detach())
+        keep.append(k)
+        setattr(p, name, ptr)
+        setattr(p, name + "_stride", stride)
+    return keep
+
+
+def _maps(x: torch.Tensor, cuda_msg: str, shape_msg: str) -> Tuple[torch.Tensor, int, int]:
+    """_plane of fp32 CUDA maps given as [B,H,W] or [B,1,H,W]; the tensor kept alive is [B,H,W]."""
+    if not x.is_cuda or x.dtype != torch.float32:
+        raise RuntimeError(cuda_msg)
+    if x.ndim == 4 and x.shape[1] == 1:
+        x = x[:, 0]
+    if x.ndim != 3:
+        raise ValueError(shape_msg)
+    return _plane(x.detach())
+
+
+@contextlib.contextmanager
+def _on_device(dev: torch.device):
+    """Make `dev` the current device (entering the guard only when it is not already) and yield its current stream
+    as the `void* stream` argument of the C ABI."""
+    with contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev):
+        yield ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def launch_count() -> int:
@@ -226,24 +209,18 @@ def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: t
     if start.ndim != 4:
         raise ValueError("planes are [B,C,H,W]")
     B, _, H, W = start.shape
-    planes = [("start", start.detach()), ("goal", goal.detach()), ("obst", obst.detach())]
-    keep = []
+    planes = [("start", start), ("goal", goal), ("obst", obst)]
     p = FwdParams()
     if cost_kind == COST_TAPS:
         if cost.dtype != torch.float32 or tuple(cost.shape) != (B, H, W, 9) or not cost.is_contiguous():
             raise ValueError("COST_TAPS expects a contiguous fp32 [B,H,W,9] tensor")
-        keep.append(cost)
         p.cost, p.cost_stride = cost.data_ptr(), 9 * H * W
     else:
-        planes.insert(0, ("cost", cost.detach()))
+        planes.insert(0, ("cost", cost))
     for _, t_ in planes:
         if t_.shape[0] != B or t_.shape[-2:] != (H, W):
             raise ValueError("plane shapes differ")
-    for name, t_ in planes:
-        k, ptr, stride = _plane(t_)
-        keep.append(k)
-        setattr(p, name, ptr)
-        setattr(p, name + "_stride", stride)
+    keep = _set_planes(p, planes)
     gr, omg, _ = host_scalars(g_ratio, W)
     p.B, p.H, p.W = B, H, W
     p.g_ratio, p.one_minus_g_ratio = gr, omg
@@ -254,8 +231,7 @@ def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: t
     ws_bytes = _ws_cache.get((B, H, W))
     if ws_bytes is None:
         ws_bytes = _ws_cache[(B, H, W)] = int(L.nastar_b200_forward_workspace_bytes(B, H, W))
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         hist = torch.empty((Bo, 1, H, W), dtype=torch.float32, device=dev)
         paths = torch.empty((Bo, 1, H, W), dtype=torch.int64, device=dev)
         counters = torch.empty((4 if want_counts else 2, Bo), dtype=torch.int32, device=dev)   # [t_solve | n_steps | ...]
@@ -269,8 +245,7 @@ def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: t
         p.trace = trace.data_ptr() if want_trace else None
         p.workspace = ws.data_ptr() if ws is not None else None
         p.workspace_bytes = ws_bytes
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _check(L.nastar_b200_forward(ctypes.byref(p), ctypes.c_void_p(stream)), "nastar_b200_forward")
+        _check(L.nastar_b200_forward(ctypes.byref(p), stream), "nastar_b200_forward")
     del keep
     if want_counts:
         return hist, paths, t_solve, n_steps, trace, SearchCounts((counters[2], counters[3]))
@@ -289,12 +264,10 @@ def pack_inputs(map_designs: torch.Tensor, start: torch.Tensor, goal: torch.Tens
     ks, ps, ss = _plane(start.detach())
     kg, pg, sg = _plane(goal.detach())
     dev = map_designs.device
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         out = torch.empty((B, Hm, Wm, C + 1), dtype=torch.float32, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_pack_inputs(md.data_ptr(), C, Hm, Wm, ps, ss, pg, sg, B, H, W, out.data_ptr(),
-                                         ctypes.c_void_p(stream)), "nastar_b200_pack_inputs")
+                                         stream), "nastar_b200_pack_inputs")
     del ks, kg
     return out.permute(0, 3, 1, 2)   # logical NCHW view with channels-last strides
 
@@ -318,12 +291,10 @@ def conv1_marks(map_designs: torch.Tensor, start: torch.Tensor, goal: torch.Tens
     ks, ps, ss = _plane(start.detach())
     kg, pg, sg = _plane(goal.detach())
     dev = map_designs.device
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         out = torch.empty((B, H, W, 32), dtype=torch.float32, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_conv1_marks(md.data_ptr(), ps, ss, pg, sg, B, H, W, w_host.ctypes.data,
-                                         bias_host.ctypes.data, out.data_ptr(), ctypes.c_void_p(stream)),
+                                         bias_host.ctypes.data, out.data_ptr(), stream),
                "nastar_b200_conv1_marks")
     del ks, kg
     return out.permute(0, 3, 1, 2)
@@ -339,13 +310,11 @@ def head_taps(x: torch.Tensor, w_host, out: Optional[torch.Tensor] = None) -> to
     if w_host.dtype.name != "float32" or w_host.shape != (C, 9) or not w_host.flags["C_CONTIGUOUS"]:
         raise ValueError("w_host must be a C-contiguous float32 [C,9] array")
     dev = x.device
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         if out is None:
             out = torch.empty((B, H, W, 9), dtype=torch.float32, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_head_taps(x.data_ptr(), B * H * W, C, w_host.ctypes.data, out.data_ptr(),
-                                       ctypes.c_void_p(stream)), "nastar_b200_head_taps")
+                                       stream), "nastar_b200_head_taps")
     return out
 
 
@@ -372,15 +341,13 @@ def conv3x3_head_taps(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, head_w_
     if head_w_host.dtype.name != "float32" or head_w_host.shape != (256, 9) or not head_w_host.flags["C_CONTIGUOUS"]:
         raise ValueError("head_w_host must be a C-contiguous float32 [256,9] array")
     dev = x.device
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         if out is None:
             out = torch.empty((B, H, W, 9), dtype=torch.float32, device=dev)
         elif tuple(out.shape) != (B, H, W, 9) or out.dtype != torch.float32 or not out.is_contiguous():
             raise ValueError("out must be a contiguous fp32 [B,H,W,9] tensor")
-        stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_conv3x3_head_taps(x.data_ptr(), B, H, W, C, 256, w.data_ptr(), b.data_ptr(),
-                                               head_w_host.ctypes.data, out.data_ptr(), ctypes.c_void_p(stream)),
+                                               head_w_host.ctypes.data, out.data_ptr(), stream),
                "nastar_b200_conv3x3_head_taps")
     return out
 
@@ -393,12 +360,10 @@ def cost_from_taps(taps: torch.Tensor, bias: float, scale: float) -> torch.Tenso
     if nine != 9 or taps.dtype != torch.float32 or not taps.is_contiguous() or not taps.is_cuda:
         raise ValueError("cost_from_taps expects a contiguous fp32 CUDA [B,H,W,9] tensor")
     dev = taps.device
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         cost = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_cost_from_taps(taps.data_ptr(), B, H, W, float(bias), float(scale), cost.data_ptr(),
-                                            ctypes.c_void_p(stream)), "nastar_b200_cost_from_taps")
+                                            stream), "nastar_b200_cost_from_taps")
     return cost
 
 
@@ -406,11 +371,10 @@ def batch_steps(t_solve: torch.Tensor, n_steps: torch.Tensor, T: int) -> torch.T
     """Device-side T_batch (int32[1]); replaces the per-step host sync of differentiable_astar.py:251."""
     L = lib()
     dev = t_solve.device
-    with torch.cuda.device(dev):
+    with _on_device(dev) as stream:
         out = torch.empty((1,), dtype=torch.int32, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_batch_steps(t_solve.data_ptr(), n_steps.data_ptr(), t_solve.numel(), int(T),
-                                         out.data_ptr(), ctypes.c_void_p(stream)), "nastar_b200_batch_steps")
+                                         out.data_ptr(), stream), "nastar_b200_batch_steps")
     return out
 
 
@@ -423,30 +387,21 @@ def opt_labels(maps: torch.Tensor, goal_idx: torch.Tensor):
     maps: fp32 CUDA [B,H,W] or [B,1,H,W] (a cell is passable iff != 0); goal_idx: int32 CUDA [B], flat goal index.
     Returns (dists fp32 [B,1,H,W], act_mask uint8 [B,1,H,W], action int8 [B,1,H,W]) on the current stream."""
     L = lib()
-    if not maps.is_cuda or maps.dtype != torch.float32:
-        raise RuntimeError("opt_labels: fp32 CUDA maps only (there is no CPU fallback)")
-    if maps.ndim == 4:
-        if maps.shape[1] != 1:
-            raise ValueError("opt_labels: maps are [B,H,W] or [B,1,H,W]")
-        maps = maps[:, 0]
-    if maps.ndim != 3:
-        raise ValueError("opt_labels: maps are [B,H,W] or [B,1,H,W]")
-    B, H, W = maps.shape
-    if goal_idx.dtype != torch.int32 or goal_idx.device != maps.device or tuple(goal_idx.shape) != (B,):
+    m, ptr, stride = _maps(maps, "opt_labels: fp32 CUDA maps only (there is no CPU fallback)",
+                           "opt_labels: maps are [B,H,W] or [B,1,H,W]")
+    B, H, W = m.shape
+    dev = m.device
+    if goal_idx.dtype != torch.int32 or goal_idx.device != dev or tuple(goal_idx.shape) != (B,):
         raise ValueError("opt_labels: goal_idx must be an int32 [B] tensor on the maps' device")
     if H > LABELS_MAX_SIDE or W > LABELS_MAX_SIDE:
         raise ValueError(f"opt_labels: maps up to {LABELS_MAX_SIDE}x{LABELS_MAX_SIDE} (got {H}x{W})")
-    m, ptr, stride = _plane(maps)
     gi = goal_idx.contiguous()
-    dev = maps.device
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         dists = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
         mask = torch.empty((B, 1, H, W), dtype=torch.uint8, device=dev)
         action = torch.empty((B, 1, H, W), dtype=torch.int8, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_opt_labels(ptr, stride, gi.data_ptr(), B, H, W, dists.data_ptr(), mask.data_ptr(),
-                                        action.data_ptr(), ctypes.c_void_p(stream)), "nastar_b200_opt_labels")
+                                        action.data_ptr(), stream), "nastar_b200_opt_labels")
     del m, gi
     return dists, mask, action
 
@@ -470,15 +425,8 @@ def weighted_labels(cost: torch.Tensor, goal_idx: torch.Tensor, passable: Option
     L = lib()
 
     def plane(x, name):
-        if not x.is_cuda or x.dtype != torch.float32:
-            raise RuntimeError(f"weighted_labels: {name} must be fp32 CUDA maps (there is no CPU fallback)")
-        if x.ndim == 4:
-            if x.shape[1] != 1:
-                raise ValueError(f"weighted_labels: {name} are [B,H,W] or [B,1,H,W]")
-            x = x[:, 0]
-        if x.ndim != 3:
-            raise ValueError(f"weighted_labels: {name} are [B,H,W] or [B,1,H,W]")
-        return _plane(x.detach())
+        return _maps(x, f"weighted_labels: {name} must be fp32 CUDA maps (there is no CPU fallback)",
+                     f"weighted_labels: {name} are [B,H,W] or [B,1,H,W]")
 
     c, cptr, cstride = plane(cost, "cost maps")
     B, H, W = c.shape
@@ -493,8 +441,7 @@ def weighted_labels(cost: torch.Tensor, goal_idx: torch.Tensor, passable: Option
         raise ValueError(f"weighted_labels: maps up to {WLABELS_MAX_SIDE}x{WLABELS_MAX_SIDE} (got {H}x{W})")
     gi = goal_idx.contiguous()
     si = None if start_idx is None else start_idx.contiguous()
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         dists = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
         hops = torch.empty((B, 1, H, W), dtype=torch.int32, device=dev)
         mask = torch.empty((B, 1, H, W), dtype=torch.uint8, device=dev)
@@ -502,13 +449,12 @@ def weighted_labels(cost: torch.Tensor, goal_idx: torch.Tensor, passable: Option
         paths = None if si is None else torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
         pcost = None if si is None else torch.empty((B,), dtype=torch.float32, device=dev)
         status = torch.empty((B,), dtype=torch.int32, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_weighted_labels(cptr, cstride, pptr, pstride, gi.data_ptr(),
                                              None if si is None else si.data_ptr(), B, H, W, dists.data_ptr(),
                                              hops.data_ptr(), mask.data_ptr(), action.data_ptr(),
                                              None if paths is None else paths.data_ptr(),
                                              None if pcost is None else pcost.data_ptr(), status.data_ptr(),
-                                             ctypes.c_void_p(stream)), "nastar_b200_weighted_labels")
+                                             stream), "nastar_b200_weighted_labels")
     del c, p, gi, si
     return WeightedLabels((dists, hops, mask, action, paths, pcost, status))
 
@@ -537,16 +483,14 @@ def sampler_prepare(dists: torch.Tensor, policies: torch.Tensor, goal_maps: torc
     d, p, g = (t_.detach().contiguous() for t_ in (dists, policies, goal_maps))
     N = H * W
     dev = dists.device
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         i32 = dict(dtype=torch.int32, device=dev)
         out = SamplerTables((torch.empty((B, 3, (N + 31) // 32), **i32), torch.empty((B, 3), **i32),
                              torch.empty((B,), **i32), torch.empty((B, (N + 7) // 8), **i32),
                              torch.empty((B, 4), dtype=torch.float64, device=dev), torch.empty((B,), **i32)))
-        stream = torch.cuda.current_stream(dev).cuda_stream
         q = [float(v) for v in quantiles]
         _check(L.nastar_b200_sampler_prepare(d.data_ptr(), p.data_ptr(), g.data_ptr(), B, H, W, *q,
-                                             *(t_.data_ptr() for t_ in out), ctypes.c_void_p(stream)),
+                                             *(t_.data_ptr() for t_ in out), stream),
                "nastar_b200_sampler_prepare")
     del d, p, g
     return out
@@ -570,16 +514,14 @@ def sampler_sample(maps: torch.Tensor, goal_maps: torch.Tensor, tables: SamplerT
         raise ValueError("sampler_sample: indices must be a contiguous int64 [B] tensor on the maps' device")
     bits, counts, goal_idx, actions = tables[:4]
     dev = maps.device
-    guard = contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev)
-    with guard:
+    with _on_device(dev) as stream:
         f32 = dict(dtype=torch.float32, device=dev)
         out = (torch.empty((B, 1, H, W), **f32), torch.empty((B, S, H, W), **f32), torch.empty((B, 1, H, W), **f32),
                torch.empty((B, S, H, W), **f32))
-        stream = torch.cuda.current_stream(dev).cuda_stream
         _check(L.nastar_b200_sampler_sample(maps.data_ptr(), goal_maps.data_ptr(), n, H, W, bits.data_ptr(),
                                             counts.data_ptr(), goal_idx.data_ptr(), actions.data_ptr(),
                                             indices.data_ptr(), draws.data_ptr(), B, S,
-                                            *(t_.data_ptr() for t_ in out), ctypes.c_void_p(stream)),
+                                            *(t_.data_ptr() for t_ in out), stream),
                "nastar_b200_sampler_sample")
     return out
 
@@ -590,30 +532,21 @@ def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Te
     L = lib()
     dev = cost.device
     B, _, H, W = cost.shape
-    keep = []
     p = BwdParams()
-    for name, t_ in (("cost", cost.detach()), ("start", start.detach()), ("goal", goal.detach()),
-                     ("obst", obst.detach())):
-        k, ptr, stride = _plane(t_)
-        keep.append(k)
-        setattr(p, name, ptr)
-        setattr(p, name + "_stride", stride)
-    gh, ptr, stride = _plane(grad_hist.detach().to(torch.float32))
-    keep.append(gh)
-    p.grad_histories, p.grad_stride = ptr, stride
+    keep = _set_planes(p, (("cost", cost), ("start", start), ("goal", goal), ("obst", obst)))
+    gh, p.grad_histories, p.grad_stride = _plane(grad_hist.detach().to(torch.float32))
     gr, omg, sq = host_scalars(g_ratio, W)
     p.B, p.H, p.W = B, H, W
     p.g_ratio, p.one_minus_g_ratio, p.sqrt_w = gr, omg, sq
     p.T_batch = T_batch.data_ptr()
     p.t_solve = t_solve.data_ptr()
-    with torch.cuda.device(dev):
+    with _on_device(dev) as stream:
         grad_cost = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
         ws_bytes = L.nastar_b200_backward_workspace_bytes(B, H, W)
         ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None
         p.grad_cost = grad_cost.data_ptr()
         p.workspace = ws.data_ptr() if ws is not None else None
         p.workspace_bytes = ws_bytes
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        _check(L.nastar_b200_backward(ctypes.byref(p), ctypes.c_void_p(stream)), "nastar_b200_backward")
+        _check(L.nastar_b200_backward(ctypes.byref(p), stream), "nastar_b200_backward")
     del keep
     return grad_cost

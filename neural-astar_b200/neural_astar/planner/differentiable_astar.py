@@ -4,7 +4,7 @@ Mirrors /root/reference/src/neural_astar/planner/differentiable_astar.py:
   AstarOutput (:16-23), get_heuristic (:26-52), DifferentiableAstar (:128-267).
 The T-step Python loop (:203-252), `expand` (:77-93), `_st_softmax_noexp` (:55-74) and
 `backtrack` (:96-125) do not exist here as Python: they run inside one persistent sm_90a kernel
-per map batch (csrc/nastar_fwd_*.cuh) reached through the C ABI in include/nastar_b200.h.
+per map batch (csrc/nastar_{warp32,warp64,bin16,generic}.cuh) reached through the C ABI in include/nastar_b200.h.
 Autograd (only cost -> h -> f -> softmax -> histories is live in the reference, :237-243) is a
 second kernel evaluating the closed form of SURVEY.md App. B.
 """
