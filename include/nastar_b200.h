@@ -284,6 +284,22 @@ int nastar_b200_sampler_sample(const float *maps, const float *goal_maps, int32_
                                int32_t S, float *out_maps, float *out_starts, float *out_goals, float *out_trajs,
                                void *stream);
 
+/* Goals for new maps (the planning-datasets generator's from_largest rule, planning_datasets_utils/data.py:128-147,
+ * with the random draw supplied by the caller).  maps: B fp32 maps of H*W cells, map_stride (>= H*W) elements apart; a
+ * cell is passable iff its value != 0.0.  Per map b:
+ *   region      the largest 4-connected region of passable cells; ties go to the region whose first cell comes first
+ *               in raster order (scipy.ndimage.label + argmax of the counts);
+ *   candidates  with edge_size e > 0, the region's cells with (y < e || y >= H-e) && (x < e || x >= W-e) (the four
+ *               e x e corner squares, NumPy's corner[e:-e] slicing for every e) if there is one, else the whole region;
+ *               e == 0: the whole region;
+ *   goal        candidate k = (draws[b] * count) >> 32 in raster order, draws read as u32 (passed as int32).
+ * Writes goal_idx i32 [B] (flat y*W+x), goal_maps fp32 [B][H*W] (dense: 1.0 at the goal, 0 elsewhere) and
+ * status i32 [B]: 0, or 1 = the map has no passable cell (then goal_idx = -1 and an all-zero plane).
+ * Needs no workspace.  One kernel launch.  edge_size >= 0; H, W <= 512, else NASTAR_EUNSUPPORTED.  Asynchronous on
+ * `stream`.  Returns NASTAR_*. */
+int nastar_b200_sample_goals(const float *maps, int64_t map_stride, int32_t B, int32_t H, int32_t W, int32_t edge_size,
+                             const int32_t *draws, int32_t *goal_idx, float *goal_maps, int32_t *status, void *stream);
+
 /* Number of kernel launches issued by this library since load (bench.py's gpu_launches). */
 uint64_t nastar_b200_launch_count(void);
 

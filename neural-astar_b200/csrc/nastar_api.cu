@@ -13,6 +13,7 @@
 #include "nastar_convhead.cuh"
 #include "nastar_generic.cuh"
 #include "nastar_glue.cuh"
+#include "nastar_goals.cuh"
 #include "nastar_labels.cuh"
 #include "nastar_sampler.cuh"
 #include "nastar_wlabels.cuh"
@@ -507,6 +508,20 @@ int nastar_b200_sampler_sample(const float* maps, const float* goal_maps, int32_
                                 out_maps, out_starts, out_goals, out_trajs};
     const cudaError_t e = launch_smem(nastar::sampler_sample_kernel, B, nastar::kSamplerThreads, smem,
                                       static_cast<cudaStream_t>(stream_v), a);
+    if (e != cudaSuccess) return cuda_fail(e);
+    return launched();
+}
+
+int nastar_b200_sample_goals(const float* maps, int64_t map_stride, int32_t B, int32_t H, int32_t W, int32_t edge_size,
+                             const int32_t* draws, int32_t* goal_idx, float* goal_maps, int32_t* status, void* stream_v) {
+    if (!maps || !draws || !goal_idx || !goal_maps || !status || B <= 0 || H <= 0 || W <= 0 || edge_size < 0)
+        return NASTAR_EINVAL;
+    if (map_stride < int64_t(H) * W) return NASTAR_EINVAL;
+    if (H > nastar::kGoalsMaxSide || W > nastar::kGoalsMaxSide) return NASTAR_EUNSUPPORTED;
+    const nastar::GoalsArgs a{maps, map_stride, B, H, W, edge_size, reinterpret_cast<const uint32_t*>(draws),
+                              nastar::goals_plane_in_smem(H, W) ? 1 : 0, goal_idx, goal_maps, status};
+    const cudaError_t e = launch_smem(nastar::sample_goals_kernel, B, nastar::goals_threads(H, W),
+                                      nastar::goals_smem_bytes(H, W), static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();
 }

@@ -81,6 +81,7 @@ _SIGNATURES = {
     "nastar_b200_weighted_labels": (_int, [_p, _i64, _p, _i64] + [_p] * 2 + [_i32] * 3 + [_p] * 8),
     "nastar_b200_sampler_prepare": (_int, [_p] * 3 + [_i32] * 3 + [ctypes.c_double] * 4 + [_p] * 7),
     "nastar_b200_sampler_sample": (_int, [_p] * 2 + [_i32] * 3 + [_p] * 6 + [_i32] * 2 + [_p] * 5),
+    "nastar_b200_sample_goals": (_int, [_p, _i64] + [_i32] * 4 + [_p] * 5),
     "nastar_b200_launch_count": (ctypes.c_uint64, []),
     "nastar_b200_status_string": (ctypes.c_char_p, [_int]),
     "nastar_b200_last_cuda_error": (ctypes.c_char_p, []),
@@ -524,6 +525,41 @@ def sampler_sample(maps: torch.Tensor, goal_maps: torch.Tensor, tables: SamplerT
                                             *(t_.data_ptr() for t_ in out), stream),
                "nastar_b200_sampler_sample")
     return out
+
+
+GOALS_MAX_SIDE = 512
+
+
+def sample_goals(maps: torch.Tensor, draws: torch.Tensor, edge_size: int = 0):
+    """Goals of B maps in one kernel (include/nastar_b200.h, nastar_b200_sample_goals): a cell of the largest
+    4-connected passable region, in its edge_size corner squares when it reaches one, chosen by the map's u32 draw.
+
+    maps: fp32 CUDA [B,H,W] or [B,1,H,W] (a cell is passable iff != 0); draws: int32 [B] on the maps' device.
+    Returns (goal_idx int32 [B], goal_maps fp32 [B,1,H,W], status int32 [B]) on the current stream; status 1 marks a map
+    without a passable cell (goal_idx -1, all-zero plane) and is not read back here."""
+    L = lib()
+    B = maps.shape[0] if maps.ndim in (3, 4) else None
+    if not isinstance(draws, torch.Tensor) or draws.dtype != torch.int32 or tuple(draws.shape) != (B,):
+        raise ValueError(f"sample_goals: draws must be an int32 [B] tensor, B = {B} maps")
+    m, ptr, stride = _maps(maps, "sample_goals: fp32 CUDA maps only (there is no CPU fallback)",
+                           "sample_goals: maps are [B,H,W] or [B,1,H,W]")
+    _, H, W = m.shape
+    dev = m.device
+    if draws.device != dev:
+        raise ValueError("sample_goals: draws must be on the maps' device")
+    if H > GOALS_MAX_SIDE or W > GOALS_MAX_SIDE:
+        raise ValueError(f"sample_goals: maps up to {GOALS_MAX_SIDE}x{GOALS_MAX_SIDE} (got {H}x{W})")
+    if int(edge_size) < 0:
+        raise ValueError(f"sample_goals: edge_size must be >= 0 (got {edge_size})")
+    d = draws.contiguous()
+    with _on_device(dev) as stream:
+        goal_idx = torch.empty((B,), dtype=torch.int32, device=dev)
+        goal_maps = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        _check(L.nastar_b200_sample_goals(ptr, stride, B, H, W, int(edge_size), d.data_ptr(), goal_idx.data_ptr(),
+                                          goal_maps.data_ptr(), status.data_ptr(), stream), "nastar_b200_sample_goals")
+    del m, d
+    return goal_idx, goal_maps, status
 
 
 def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Tensor, t_solve: torch.Tensor,

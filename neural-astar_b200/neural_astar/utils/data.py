@@ -463,6 +463,35 @@ def sample_goal_maps(map_designs, edge_size: int = 0, rng=None) -> np.ndarray:
     return goals
 
 
+def sample_device_goal_maps(map_designs: torch.Tensor, edge_size: int = 0, generator: torch.Generator = None,
+                            draws: torch.Tensor = None) -> torch.Tensor:
+    """sample_goal_maps' rule on the GPU, one kernel launch for the whole batch (DESIGN.md §12).
+
+    For every map: the largest 4-connected passable region (a cell is passable iff its value != 0; ties go to the
+    region whose first cell comes first in raster order), restricted to the four edge_size x edge_size corner squares
+    when that leaves any cell (edge_size = 0: no restriction); then candidate (d * count) >> 32 in raster order, d the
+    map's u32 draw.  The draws are torch.randint on the device with `generator` (a CUDA generator; the default one when
+    None), or the given int32 [B] tensor `draws`, so the goals are not `random.choice`'s: sample_goal_maps stays the
+    path that follows the `random` module.
+
+    map_designs: CUDA [B,H,W] or [B,1,H,W], H, W <= 512.  Returns float32 [B,1,H,W] goal maps with one 1 per map on the
+    maps' device, ready for compute_opt_labels, compute_weighted_opt_labels and DeviceMazeDataset.from_labels.  Raises
+    ValueError naming the maps without a passable cell (this reads the per-map status back to the host)."""
+    if not map_designs.is_cuda:
+        raise RuntimeError("sample_device_goal_maps runs on CUDA tensors only (there is no CPU fallback)")
+    maps = map_designs.detach().float()
+    B = maps.shape[0]
+    if draws is None:
+        draws = torch.randint(-2 ** 31, 2 ** 31, (B,), dtype=torch.int32, device=maps.device, generator=generator)
+    elif tuple(draws.shape) != (B,):
+        raise ValueError(f"draws must be [B] = [{B}]")
+    _, goal_maps, status = _native.sample_goals(maps, draws.to(maps.device, torch.int32), edge_size)
+    bad = torch.nonzero(status & 1).flatten().tolist()
+    if bad:
+        raise ValueError(f"sample_device_goal_maps: maps {bad[:20]} have no passable cell")
+    return goal_maps
+
+
 def _np(x) -> np.ndarray:
     return x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
 
@@ -486,5 +515,6 @@ def save_planning_dataset(path: str, train, valid, test) -> None:
 
 __all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "MazeDataset", "WarCraftDataset",
            "compute_opt_labels", "compute_weighted_opt_labels", "create_dataloader", "create_device_dataloader",
-           "create_warcraft_dataloader", "sample_goal_maps", "save_planning_dataset", "save_warcraft_dataset",
+           "create_warcraft_dataloader", "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset",
+           "save_warcraft_dataset",
            "shortest_path_maps", "visualize_results"]
