@@ -300,6 +300,29 @@ int nastar_b200_sampler_sample(const float *maps, const float *goal_maps, int32_
 int nastar_b200_sample_goals(const float *maps, int64_t map_stride, int32_t B, int32_t H, int32_t W, int32_t edge_size,
                              const int32_t *draws, int32_t *goal_idx, float *goal_maps, int32_t *status, void *stream);
 
+/* Planning maps from decoded map images (the planning-datasets generator's load_maze_from_directory:
+ * Image.resize((W, H)) + skimage threshold_otsu + image > threshold).  images: B uint8 L images of H0*W0 levels (rows
+ * W0 apart), image_stride (>= H0*W0) elements apart.  Per image b:
+ *   resized     Pillow's BICUBIC resize to H x W (reducing_gap=None), bit for bit: a horizontal pass into a uint8
+ *               intermediate when W != W0, then a vertical pass when H != H0, with Pillow's 22-bit fixed-point weights;
+ *   threshold   threshold_otsu (skimage >= 0.19) of the resized levels as float32: the level of a uniform image,
+ *               else the center of the first bin that maximises the between-class variance of the 256-bin histogram
+ *               over [min, max], with sequential float64 cumulative sums;
+ *   map         1.0 where level > threshold, else 0.0.
+ * Writes maps fp32 [B][H*W], resized uint8 [B][H*W] (optional: NULL skips it), thresholds fp32 [B] and status i32 [B]:
+ * 0, or 1 = uniform resized image (all-zero map).  Needs no workspace.  One kernel launch.  H, W <= 512 and H0, W0 <=
+ * 2048, else NASTAR_EUNSUPPORTED.  Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_maps_from_images(const uint8_t *images, int64_t image_stride, int32_t B, int32_t H0, int32_t W0,
+                                 int32_t H, int32_t W, float *maps, uint8_t *resized, float *thresholds,
+                                 int32_t *status, void *stream);
+
+/* One-hot policies drawn from maximal action sets.  act_mask: uint8 [B][N] (bit a = action a is maximal, the act_mask
+ * of nastar_b200_opt_labels); draws: [B][N] u32 (passed as int32).  Cell c of map b takes set bit k = (d * popc) >> 32
+ * of its mask in action order, d = its draw, and writes policies fp32 [B][8][N] one-hot (all zero for an empty mask).
+ * One kernel launch.  Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_draw_policies(const uint8_t *act_mask, const int32_t *draws, int32_t B, int32_t N, float *policies,
+                              void *stream);
+
 /* Number of kernel launches issued by this library since load (bench.py's gpu_launches). */
 uint64_t nastar_b200_launch_count(void);
 

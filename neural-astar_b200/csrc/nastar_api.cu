@@ -15,6 +15,7 @@
 #include "nastar_glue.cuh"
 #include "nastar_goals.cuh"
 #include "nastar_labels.cuh"
+#include "nastar_maps.cuh"
 #include "nastar_sampler.cuh"
 #include "nastar_wlabels.cuh"
 #include "nastar_warp32.cuh"
@@ -523,6 +524,34 @@ int nastar_b200_sample_goals(const float* maps, int64_t map_stride, int32_t B, i
     const cudaError_t e = launch_smem(nastar::sample_goals_kernel, B, nastar::goals_threads(H, W),
                                       nastar::goals_smem_bytes(H, W), static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
+    return launched();
+}
+
+int nastar_b200_maps_from_images(const uint8_t* images, int64_t image_stride, int32_t B, int32_t H0, int32_t W0,
+                                 int32_t H, int32_t W, float* maps, uint8_t* resized, float* thresholds,
+                                 int32_t* status, void* stream_v) {
+    if (!images || !maps || !thresholds || !status || B <= 0 || H0 <= 0 || W0 <= 0 || H <= 0 || W <= 0)
+        return NASTAR_EINVAL;
+    if (image_stride < int64_t(H0) * W0) return NASTAR_EINVAL;
+    if (H > nastar::kMapsMaxSide || W > nastar::kMapsMaxSide || H0 > nastar::kMapsMaxSrcSide ||
+        W0 > nastar::kMapsMaxSrcSide)
+        return NASTAR_EUNSUPPORTED;
+    const size_t smem = nastar::maps_smem_bytes(H0, W0, H, W);
+    if (smem > kMaxDynSmem) return NASTAR_EUNSUPPORTED;
+    const nastar::MapsArgs a{images, image_stride, B, H0, W0, H, W, nastar::maps_taps(W0, W), nastar::maps_taps(H0, H),
+                             nastar::maps_strip_cols(H0, W), maps, resized, thresholds, status};
+    const cudaError_t e = launch_smem(nastar::maps_from_images_kernel, B, nastar::kMapsThreads, smem,
+                                      static_cast<cudaStream_t>(stream_v), a);
+    if (e != cudaSuccess) return cuda_fail(e);
+    return launched();
+}
+
+int nastar_b200_draw_policies(const uint8_t* act_mask, const int32_t* draws, int32_t B, int32_t N, float* policies,
+                              void* stream_v) {
+    if (!act_mask || !draws || !policies || B <= 0 || N <= 0) return NASTAR_EINVAL;
+    const int64_t total = int64_t(B) * N;
+    nastar::draw_policies_kernel<<<capped_grid((total + 255) / 256, 16), 256, 0, static_cast<cudaStream_t>(stream_v)>>>(
+        act_mask, reinterpret_cast<const uint32_t*>(draws), B, N, policies);
     return launched();
 }
 

@@ -82,6 +82,8 @@ _SIGNATURES = {
     "nastar_b200_sampler_prepare": (_int, [_p] * 3 + [_i32] * 3 + [ctypes.c_double] * 4 + [_p] * 7),
     "nastar_b200_sampler_sample": (_int, [_p] * 2 + [_i32] * 3 + [_p] * 6 + [_i32] * 2 + [_p] * 5),
     "nastar_b200_sample_goals": (_int, [_p, _i64] + [_i32] * 4 + [_p] * 5),
+    "nastar_b200_maps_from_images": (_int, [_p, _i64] + [_i32] * 5 + [_p] * 5),
+    "nastar_b200_draw_policies": (_int, [_p, _p, _i32, _i32, _p, _p]),
     "nastar_b200_launch_count": (ctypes.c_uint64, []),
     "nastar_b200_status_string": (ctypes.c_char_p, [_int]),
     "nastar_b200_last_cuda_error": (ctypes.c_char_p, []),
@@ -560,6 +562,71 @@ def sample_goals(maps: torch.Tensor, draws: torch.Tensor, edge_size: int = 0):
                                           goal_maps.data_ptr(), status.data_ptr(), stream), "nastar_b200_sample_goals")
     del m, d
     return goal_idx, goal_maps, status
+
+
+MAPS_MAX_SIDE = 512
+MAPS_MAX_SOURCE_SIDE = 2048
+
+
+def maps_from_images(images: torch.Tensor, H: int, W: int, want_resized: bool = False):
+    """Planning maps of B decoded L images in one kernel (include/nastar_b200.h, nastar_b200_maps_from_images): Pillow's
+    bicubic resize to H x W, skimage's Otsu threshold, level > threshold.
+
+    images: uint8 CUDA [B,H0,W0].  Returns (maps fp32 [B,1,H,W], resized uint8 [B,H,W] or None, thresholds fp32 [B],
+    status int32 [B]) on the current stream; status 1 marks a uniform resized image (all-zero map) and is not read back
+    here."""
+    L = lib()
+    if not isinstance(images, torch.Tensor) or not images.is_cuda or images.dtype != torch.uint8:
+        raise RuntimeError("maps_from_images: uint8 CUDA images only (there is no CPU fallback)")
+    if images.ndim != 3 or min(images.shape) < 1:
+        raise ValueError(f"maps_from_images: images are [B,H0,W0] with B, H0, W0 >= 1 (got {tuple(images.shape)})")
+    B, H0, W0 = images.shape
+    H, W = int(H), int(W)
+    if not (1 <= H <= MAPS_MAX_SIDE and 1 <= W <= MAPS_MAX_SIDE):
+        raise ValueError(f"maps_from_images: maps from 1x1 up to {MAPS_MAX_SIDE}x{MAPS_MAX_SIDE} (got {H}x{W})")
+    if H0 > MAPS_MAX_SOURCE_SIDE or W0 > MAPS_MAX_SOURCE_SIDE:
+        raise ValueError(f"maps_from_images: images up to {MAPS_MAX_SOURCE_SIDE}x{MAPS_MAX_SOURCE_SIDE} "
+                         f"(got {H0}x{W0})")
+    x = images.contiguous()
+    dev = x.device
+    with _on_device(dev) as stream:
+        maps = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
+        resized = torch.empty((B, H, W), dtype=torch.uint8, device=dev) if want_resized else None
+        thresholds = torch.empty((B,), dtype=torch.float32, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        _check(L.nastar_b200_maps_from_images(x.data_ptr(), H0 * W0, B, H0, W0, H, W, maps.data_ptr(),
+                                              resized.data_ptr() if want_resized else None, thresholds.data_ptr(),
+                                              status.data_ptr(), stream), "nastar_b200_maps_from_images")
+    del x
+    return maps, resized, thresholds, status
+
+
+def draw_policies(act_mask: torch.Tensor, draws: torch.Tensor) -> torch.Tensor:
+    """One-hot policies drawn from maximal action sets in one kernel (include/nastar_b200.h, nastar_b200_draw_policies).
+
+    act_mask: uint8 CUDA [B,1,H,W] or [B,H,W] (bit a = action a is maximal); draws: int32 tensor of the same number of
+    cells on the mask's device.  Returns policies fp32 [B,8,1,H,W] on the current stream: cell c takes set bit
+    (d * popc) >> 32 of its mask in action order, an empty mask gives an all-zero column."""
+    L = lib()
+    if not isinstance(act_mask, torch.Tensor) or not act_mask.is_cuda or act_mask.dtype != torch.uint8:
+        raise RuntimeError("draw_policies: uint8 CUDA action masks only (there is no CPU fallback)")
+    if act_mask.ndim == 4 and act_mask.shape[1] == 1:
+        act_mask = act_mask[:, 0]
+    if act_mask.ndim != 3 or act_mask.numel() == 0:
+        raise ValueError("draw_policies: act_mask is [B,H,W] or [B,1,H,W]")
+    B, H, W = act_mask.shape
+    dev = act_mask.device
+    if (not isinstance(draws, torch.Tensor) or draws.dtype != torch.int32 or draws.device != dev
+            or draws.numel() != B * H * W):
+        raise ValueError(f"draw_policies: draws must be an int32 tensor of B*H*W = {B * H * W} cells on the mask's "
+                         "device")
+    m, d = act_mask.contiguous(), draws.contiguous()
+    with _on_device(dev) as stream:
+        policies = torch.empty((B, 8, 1, H, W), dtype=torch.float32, device=dev)
+        _check(L.nastar_b200_draw_policies(m.data_ptr(), d.data_ptr(), B, H * W, policies.data_ptr(), stream),
+               "nastar_b200_draw_policies")
+    del m, d
+    return policies
 
 
 def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Tensor, t_solve: torch.Tensor,

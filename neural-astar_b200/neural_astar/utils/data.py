@@ -492,6 +492,104 @@ def sample_device_goal_maps(map_designs: torch.Tensor, edge_size: int = 0, gener
     return goal_maps
 
 
+def _natural_key(s: str):
+    """natsort's default ordering for file names: runs of digits compare as integers."""
+    import re
+
+    return [int(p) if p.isdigit() else p for p in re.split(r"(\d+)", s)]
+
+
+def load_map_images(input_path: str, split: str):
+    """Decode the map images `<input_path>/<split>/*.png` on the host, as the planning-datasets generator does
+    (load_maze_from_directory): natural-sort order of the paths, `*` allowed in input_path, each image converted to L.
+
+    split: "train", "validation" or "test".  Returns a list of (positions int64 [n], images uint8 [n,H0,W0]) NumPy
+    pairs, one per source size: positions are the images' places in the sorted file list.  maps_from_images takes the
+    list as it is and returns the maps in file order."""
+    import glob
+    import os
+
+    from PIL import Image
+
+    if split not in ("train", "validation", "test"):
+        raise ValueError(f"split must be train, validation or test (got {split!r})")
+    paths = sorted(glob.glob(os.path.join(input_path, split, "*.png")), key=_natural_key)
+    if not paths:
+        raise FileNotFoundError(f"no PNG images match {os.path.join(input_path, split, '*.png')}")
+    groups = {}
+    for i, path in enumerate(paths):
+        with Image.open(path) as im:
+            img = np.asarray(im.convert("L"), dtype=np.uint8)
+        groups.setdefault(img.shape, []).append((i, img))
+    return [(np.array([i for i, _ in g], np.int64), np.stack([img for _, img in g])) for g in groups.values()]
+
+
+def maps_from_images(images, size, device=None) -> torch.Tensor:
+    """Planning maps from decoded map images on the GPU, as the planning-datasets generator makes them
+    (load_maze_from_directory, DESIGN.md §13): Pillow's bicubic Image.resize to H x W, skimage's threshold_otsu of the
+    resized levels, 1.0 where level > threshold, else 0.0.  Bit-equal to the generator; a uniform resized image gives
+    an all-zero map, as there.
+
+    images: CUDA uint8 [B,H0,W0] (one kernel launch), or the list load_map_images returns (one launch per source size,
+    moved to `device`, the current CUDA device when None).  H0, W0 <= 2048.  size: int or (H, W), H, W <= 512.
+    Returns float32 [B,1,H,W] on the device, in the images' order, ready for sample_device_goal_maps."""
+    H, W = (int(size), int(size)) if np.ndim(size) == 0 else (int(size[0]), int(size[1]))
+    if isinstance(images, torch.Tensor):
+        if not images.is_cuda:
+            raise RuntimeError("maps_from_images runs on CUDA tensors only (there is no CPU fallback)")
+        return _native.maps_from_images(images, H, W)[0]
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    n = sum(len(pos) for pos, _ in images)
+    out = torch.empty((n, 1, H, W), dtype=torch.float32, device=dev)
+    for pos, imgs in images:
+        out[torch.from_numpy(pos).to(dev)] = _native.maps_from_images(torch.from_numpy(imgs).to(dev), H, W)[0]
+    return out
+
+
+def tile_maps(maps: torch.Tensor, tile_size: int, indices=None, generator: torch.Generator = None,
+              num: int = None) -> torch.Tensor:
+    """Tiled maps, skimage.util.montage of tile_size**2 maps each, as the planning-datasets generator lays them out
+    with --tile-size (Tiled MP): map k of a tile goes to grid cell (k // tile_size, k % tile_size).
+
+    maps: [N,h,w] or [N,1,h,w]; indices: [M, tile_size**2] map indices (a tensor or array), or None to draw `num`
+    tiles (N when None) uniformly with torch.randint on the maps' device with `generator`.  The generator's own tiles
+    come from np.random.choice: pass those indices to replay them.  Returns [M,1,t*h,t*w] in the maps' dtype."""
+    t = int(tile_size)
+    m = maps[:, 0] if maps.ndim == 4 else maps
+    N, h, w = m.shape
+    if indices is None:
+        idx = torch.randint(0, N, (N if num is None else int(num), t * t), device=m.device, generator=generator)
+    else:
+        idx = torch.as_tensor(np.asarray(indices) if not isinstance(indices, torch.Tensor) else indices)
+        if idx.ndim != 2 or idx.shape[1] != t * t:
+            raise ValueError(f"indices must be [M, tile_size**2] = [M, {t * t}] (got {tuple(idx.shape)})")
+        if idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= N):
+            raise IndexError(f"indices must lie in [0, {N})")
+        idx = idx.to(m.device, torch.int64)
+    M = idx.shape[0]
+    return m[idx].reshape(M, t, t, h, w).permute(0, 1, 3, 2, 4).reshape(M, 1, t * h, t * w)
+
+
+def draw_opt_policies(act_mask: torch.Tensor, generator: torch.Generator = None,
+                      draws: torch.Tensor = None) -> torch.Tensor:
+    """One-hot optimal policies with the planning-datasets generator's rule (extract_policy): every cell takes one
+    member of its maximal action set uniformly, instead of compute_opt_labels' first maximum.  One kernel launch.
+
+    act_mask: CUDA uint8 [B,1,H,W] from compute_opt_labels (bit a set iff action a is maximal).  Cell c takes set bit
+    (d * popc) >> 32 in action order, d its u32 draw: torch.randint on the device with `generator` (a CUDA generator;
+    the default one when None), or the given int32 [B,1,H,W] / [B,H,W] tensor `draws`.  Returns float32 [B,8,1,H,W]
+    (a cell with an empty mask gets an all-zero column)."""
+    if not act_mask.is_cuda:
+        raise RuntimeError("draw_opt_policies runs on CUDA tensors only (there is no CPU fallback)")
+    mask = act_mask[:, 0] if act_mask.ndim == 4 else act_mask
+    if draws is None:
+        draws = torch.randint(-2 ** 31, 2 ** 31, tuple(mask.shape), dtype=torch.int32, device=mask.device,
+                              generator=generator)
+    elif draws.numel() != mask.numel():
+        raise ValueError(f"draws must have one entry per cell, {list(mask.shape)}")
+    return _native.draw_policies(mask, draws.to(mask.device, torch.int32))
+
+
 def _np(x) -> np.ndarray:
     return x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
 
@@ -515,6 +613,6 @@ def save_planning_dataset(path: str, train, valid, test) -> None:
 
 __all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "MazeDataset", "WarCraftDataset",
            "compute_opt_labels", "compute_weighted_opt_labels", "create_dataloader", "create_device_dataloader",
-           "create_warcraft_dataloader", "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset",
-           "save_warcraft_dataset",
-           "shortest_path_maps", "visualize_results"]
+           "create_warcraft_dataloader", "draw_opt_policies", "load_map_images", "maps_from_images",
+           "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset", "save_warcraft_dataset",
+           "shortest_path_maps", "tile_maps", "visualize_results"]
