@@ -223,6 +223,20 @@ int nastar_b200_selftest_sqrt(int32_t n, int32_t *mismatches, void *stream);
 int nastar_b200_opt_labels(const float *maps, int64_t map_stride, const int32_t *goal_idx, int32_t B, int32_t H,
                            int32_t W, float *dists, uint8_t *act_mask, int8_t *action, void *stream);
 
+/* mechanism of nastar_b200_opt_labels_mech: the planning-datasets generator's --mechanism (mechanism.py:267-277) */
+#define NASTAR_MECH_MOORE 0   /* 8 actions: N, E, W, S, NE, NW, SE, SW (the labels of nastar_b200_opt_labels) */
+#define NASTAR_MECH_NEWS  1   /* 4 actions: N, E, W, S (NorthEastWestSouth, mechanism.py:52-131) */
+
+/* nastar_b200_opt_labels for either mechanism.  NASTAR_MECH_MOORE gives exactly nastar_b200_opt_labels' output.
+ * NASTAR_MECH_NEWS: distances are unit-step BFS distances over the 4 neighbours (same fills: 0 at the goal, -(H*W)
+ * where the goal is not reached; the goal is the source even when it is not passable); act_mask holds the maximal
+ * actions among the 4 targets of N, E, W, S (bits 0..3; bits 4..7 are never set) and action its lowest member.  Every
+ * argument is checked before the launch: a mechanism other than these two is NASTAR_EINVAL.  One kernel launch.
+ * H, W <= 512, else NASTAR_EUNSUPPORTED.  Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_opt_labels_mech(const float *maps, int64_t map_stride, const int32_t *goal_idx, int32_t B, int32_t H,
+                                int32_t W, int32_t mechanism, float *dists, uint8_t *act_mask, int8_t *action,
+                                void *stream);
+
 /* Exact vertex-weighted shortest paths to a goal, for cost maps (the labels of WarCraft-style training and the optimum
  * that learned-cost paths are measured against).  Per map b (DESIGN.md §11):
  *   cost      B fp32 maps of H*W cells, cost_stride (>= H*W) elements apart;

@@ -436,16 +436,26 @@ int nastar_b200_selftest_sqrt(int32_t n, int32_t* mismatches, void* stream_v) {
     return launched();
 }
 
-int nastar_b200_opt_labels(const float* maps, int64_t map_stride, const int32_t* goal_idx, int32_t B, int32_t H,
-                           int32_t W, float* dists, uint8_t* act_mask, int8_t* action, void* stream_v) {
+int nastar_b200_opt_labels_mech(const float* maps, int64_t map_stride, const int32_t* goal_idx, int32_t B, int32_t H,
+                                int32_t W, int32_t mechanism, float* dists, uint8_t* act_mask, int8_t* action,
+                                void* stream_v) {
     if (!maps || !goal_idx || !dists || !act_mask || !action || B <= 0 || H <= 0 || W <= 0) return NASTAR_EINVAL;
     if (map_stride < int64_t(H) * W) return NASTAR_EINVAL;
+    if (mechanism != NASTAR_MECH_MOORE && mechanism != NASTAR_MECH_NEWS) return NASTAR_EINVAL;
     if (H > nastar::kLabelsMaxSide || W > nastar::kLabelsMaxSide) return NASTAR_EUNSUPPORTED;
     const nastar::LabelsArgs a{maps, map_stride, goal_idx, B, H, W, dists, act_mask, action};
-    const cudaError_t e = launch_smem(nastar::opt_labels_kernel, B, nastar::labels_threads(H, W),
-                                      nastar::labels_smem_bytes(H, W), static_cast<cudaStream_t>(stream_v), a);
+    auto* const kernel = mechanism == NASTAR_MECH_NEWS ? nastar::opt_labels_kernel<nastar::kMechNews>
+                                                       : nastar::opt_labels_kernel<nastar::kMechMoore>;
+    const cudaError_t e = launch_smem(kernel, B, nastar::labels_threads(H, W), nastar::labels_smem_bytes(H, W),
+                                      static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();
+}
+
+int nastar_b200_opt_labels(const float* maps, int64_t map_stride, const int32_t* goal_idx, int32_t B, int32_t H,
+                           int32_t W, float* dists, uint8_t* act_mask, int8_t* action, void* stream_v) {
+    return nastar_b200_opt_labels_mech(maps, map_stride, goal_idx, B, H, W, NASTAR_MECH_MOORE, dists, act_mask, action,
+                                       stream_v);
 }
 
 int nastar_b200_weighted_labels(const float* cost, int64_t cost_stride, const float* passable, int64_t passable_stride,

@@ -15,6 +15,10 @@
 //   (mechanism.py:140-149, neighbors_func :209-219), no corner-cutting check; unit step cost, distances of
 //   dijkstra_dist (dijkstra.py:120-157, stored negated); max set of extract_policy (data.py:40-58).
 //
+// The NEWS mechanism (mechanism.py:52-131: actions 0..3 = N, E, W, S, the first four Moore actions in the same order)
+// is the kMech = kMechNews instantiation: dilate4 = the word's own left/right shifts with carries OR the vertically
+// adjacent rows unshifted, and the policy reads 4 targets, so act_mask uses bits 0..3 only.
+//
 // Limits: H, W <= kLabelsMaxSide (512).  Then H*W <= 2^18, so every distance is exact in fp32, and the four bit
 // planes take at most 4 * 512 * 16 * 4 B = 128 KB of shared memory.
 #pragma once
@@ -24,6 +28,8 @@ namespace nastar {
 
 constexpr int kLabelsMaxSide = 512;
 constexpr int kLabelsMaxThreads = 512;
+constexpr int kMechMoore = 0;   // NASTAR_MECH_MOORE
+constexpr int kMechNews = 1;    // NASTAR_MECH_NEWS
 
 struct LabelsArgs {
     const float* maps;        // [B] maps of H*W fp32 cells, map_stride elements apart
@@ -42,7 +48,9 @@ inline int labels_threads(int H, int W) {
     return t < 32 ? 32 : (t > kLabelsMaxThreads ? kLabelsMaxThreads : t);
 }
 
+template <int kMech>
 __global__ void __launch_bounds__(kLabelsMaxThreads) opt_labels_kernel(LabelsArgs a) {
+    constexpr int kActions = kMech == kMechNews ? 4 : 8;
     extern __shared__ uint32_t lbl_smem[];
     const int H = a.H, W = a.W, nw = (W + 31) >> 5, nwords = H * nw, N = H * W;
     uint32_t* pas = lbl_smem;
@@ -89,6 +97,10 @@ __global__ void __launch_bounds__(kLabelsMaxThreads) opt_labels_kernel(LabelsArg
                 if (yy < 0 || yy >= H) continue;
                 const uint32_t* row = cur + yy * nw;
                 const uint32_t c = row[w];
+                if (kMech == kMechNews && dy != 0) {   // 4-connected: the rows above and below contribute unshifted
+                    h |= c;
+                    continue;
+                }
                 const uint32_t l = w > 0 ? row[w - 1] : 0u;
                 const uint32_t r = w + 1 < nw ? row[w + 1] : 0u;
                 h |= c | (c << 1) | (l >> 31) | (c >> 1) | (r << 31);
@@ -108,8 +120,8 @@ __global__ void __launch_bounds__(kLabelsMaxThreads) opt_labels_kernel(LabelsArg
         nxt = t;
     }
 
-    // policy: max set over the 8 move targets with the stay rule (the distances written above are visible to the
-    // whole block after the barrier that ended the loop)
+    // policy: max set over the kActions move targets with the stay rule (the distances written above are visible to
+    // the whole block after the barrier that ended the loop)
     const int dys[8] = {-1, 0, 0, +1, -1, -1, +1, +1};
     const int dxs[8] = {0, +1, -1, 0, +1, -1, +1, -1};
     for (int c = threadIdx.x; c < N; c += blockDim.x) {
@@ -117,7 +129,7 @@ __global__ void __launch_bounds__(kLabelsMaxThreads) opt_labels_kernel(LabelsArg
         float best = 0.0f;
         uint32_t mask = 0;
 #pragma unroll
-        for (int act = 0; act < 8; ++act) {
+        for (int act = 0; act < kActions; ++act) {
             const int ty = y + dys[act], tx = x + dxs[act];
             int t = c;
             if (ty >= 0 && ty < H && tx >= 0 && tx < W && ((pas[ty * nw + (tx >> 5)] >> (tx & 31)) & 1u)) t = ty * W + tx;

@@ -78,6 +78,7 @@ _SIGNATURES = {
     "nastar_b200_conv3x3_head_taps": (_int, [_p] + [_i32] * 5 + [_p] * 5),
     "nastar_b200_selftest_sqrt": (_int, [_i32, _p, _p]),
     "nastar_b200_opt_labels": (_int, [_p, _i64, _p, _i32, _i32, _i32, _p, _p, _p, _p]),
+    "nastar_b200_opt_labels_mech": (_int, [_p, _i64, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _p]),
     "nastar_b200_weighted_labels": (_int, [_p, _i64, _p, _i64] + [_p] * 2 + [_i32] * 3 + [_p] * 8),
     "nastar_b200_sampler_prepare": (_int, [_p] * 3 + [_i32] * 3 + [ctypes.c_double] * 4 + [_p] * 7),
     "nastar_b200_sampler_sample": (_int, [_p] * 2 + [_i32] * 3 + [_p] * 6 + [_i32] * 2 + [_p] * 5),
@@ -382,13 +383,18 @@ def batch_steps(t_solve: torch.Tensor, n_steps: torch.Tensor, T: int) -> torch.T
 
 
 LABELS_MAX_SIDE = 512
+# NASTAR_MECH_*: the planning-datasets generator's --mechanism values
+MECHANISMS = {"moore": 0, "news": 1}
 
 
-def opt_labels(maps: torch.Tensor, goal_idx: torch.Tensor):
-    """Shortest-path labels of B maps in one kernel (include/nastar_b200.h, nastar_b200_opt_labels).
+def opt_labels(maps: torch.Tensor, goal_idx: torch.Tensor, mechanism: str = "moore"):
+    """Shortest-path labels of B maps in one kernel (include/nastar_b200.h, nastar_b200_opt_labels_mech).
 
-    maps: fp32 CUDA [B,H,W] or [B,1,H,W] (a cell is passable iff != 0); goal_idx: int32 CUDA [B], flat goal index.
+    maps: fp32 CUDA [B,H,W] or [B,1,H,W] (a cell is passable iff != 0); goal_idx: int32 CUDA [B], flat goal index;
+    mechanism: "moore" (8 actions) or "news" (4 actions, act_mask bits 0..3 only).
     Returns (dists fp32 [B,1,H,W], act_mask uint8 [B,1,H,W], action int8 [B,1,H,W]) on the current stream."""
+    if mechanism not in MECHANISMS:
+        raise ValueError(f"opt_labels: mechanism must be one of {sorted(MECHANISMS)} (got {mechanism!r})")
     L = lib()
     m, ptr, stride = _maps(maps, "opt_labels: fp32 CUDA maps only (there is no CPU fallback)",
                            "opt_labels: maps are [B,H,W] or [B,1,H,W]")
@@ -403,8 +409,9 @@ def opt_labels(maps: torch.Tensor, goal_idx: torch.Tensor):
         dists = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
         mask = torch.empty((B, 1, H, W), dtype=torch.uint8, device=dev)
         action = torch.empty((B, 1, H, W), dtype=torch.int8, device=dev)
-        _check(L.nastar_b200_opt_labels(ptr, stride, gi.data_ptr(), B, H, W, dists.data_ptr(), mask.data_ptr(),
-                                        action.data_ptr(), stream), "nastar_b200_opt_labels")
+        _check(L.nastar_b200_opt_labels_mech(ptr, stride, gi.data_ptr(), B, H, W, MECHANISMS[mechanism],
+                                             dists.data_ptr(), mask.data_ptr(), action.data_ptr(), stream),
+               "nastar_b200_opt_labels_mech")
     del m, gi
     return dists, mask, action
 

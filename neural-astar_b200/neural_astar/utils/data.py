@@ -199,8 +199,8 @@ class DeviceMazeDataset:
                     opt_dists: torch.Tensor, pct1: float = 0.55, pct2: float = 0.70, pct3: float = 0.85,
                     num_starts: int = 1) -> "DeviceMazeDataset":
         """A dataset over device tensors, e.g. from compute_opt_labels / sample_goal_maps, without a file or a host
-        copy of the planes: map_designs [N,H,W] or [N,1,H,W], goal_maps [N,1,H,W], opt_policies [N,8,1,H,W],
-        opt_dists [N,1,H,W], on one CUDA device.
+        copy of the planes: map_designs [N,H,W] or [N,1,H,W], goal_maps [N,1,H,W], opt_policies [N,8,1,H,W] (or
+        [N,4,1,H,W] for the NEWS mechanism), opt_dists [N,1,H,W], on one CUDA device.
 
         Every map must have integer distances in [-(H*W), 0] with the goal as the only 0, cells above the minimum
         distance, three non-empty bands, and a first-max action that moves every cell that reaches the goal onto the
@@ -225,6 +225,10 @@ class DeviceMazeDataset:
         self.num_starts = int(num_starts)
         self.pcts = np.array([*pcts, 1.0])
         self.device = maps.device
+        if policies.ndim == 5 and policies.shape[1] == 4:
+            # NEWS policies: actions 0..3 are the sampler's first four moves (N, E, W, S), so zero planes 4..7 make them
+            # the 8-plane policies it reads, with the same first maximal action on every cell
+            policies = torch.cat((policies, torch.zeros_like(policies)), 1)
         self._tables = _native.sampler_prepare(dists, policies, self.goal_maps, _percentile_fractions(self.pcts))
         status = self._tables[5].cpu().numpy()
         if status.any():
@@ -314,15 +318,15 @@ def create_warcraft_dataloader(dirname: str, split: str, batch_size: int, shuffl
     return data.DataLoader(WarCraftDataset(dirname, split), batch_size=batch_size, shuffle=shuffle, num_workers=0)
 
 
-def compute_opt_labels(map_designs: torch.Tensor, goal_maps: torch.Tensor):
+def compute_opt_labels(map_designs: torch.Tensor, goal_maps: torch.Tensor, mechanism: str = "moore"):
     """Optimal policies and distances of the planning-datasets generator (get_goalMaps_optPolicies_optDists,
-    planning_datasets_utils/data.py:154-159: dijkstra_dist + extract_policy, Moore mechanism), computed on the GPU in
-    one kernel launch.
+    planning_datasets_utils/data.py:154-159: dijkstra_dist + extract_policy), computed on the GPU in one kernel launch.
 
     map_designs: CUDA [B,H,W] or [B,1,H,W] (a cell is passable iff its value != 0); goal_maps: CUDA [B,1,H,W] or
-    [B,H,W] with one 1 per map (the first maximum is taken).  H, W <= 512.
-    Returns, on the maps' device:
-      opt_policies [B,8,1,H,W] float32 one-hot of the FIRST maximal action per cell (the reference draws one member
+    [B,H,W] with one 1 per map (the first maximum is taken).  H, W <= 512.  mechanism: the generator's --mechanism,
+    "moore" (8 actions N, E, W, S, NE, NW, SE, SW) or "news" (4 actions N, E, W, S and 4-connected distances).
+    Returns, on the maps' device, with A = 8 (moore) or 4 (news):
+      opt_policies [B,A,1,H,W] float32 one-hot of the FIRST maximal action per cell (the reference draws one member
                    of the maximal set at random; MazeDataset rolls a policy out with the same first-maximum rule);
       opt_dists    [B,1,H,W] float32: 0 at the goal, -(moves to the goal), -(H*W) where the goal is not reachable;
       act_mask     [B,1,H,W] uint8: bit a set iff action a is maximal (the set the reference draws from)."""
@@ -333,8 +337,8 @@ def compute_opt_labels(map_designs: torch.Tensor, goal_maps: torch.Tensor):
         maps = maps[:, 0]
     B, H, W = maps.shape
     goal_idx = goal_maps.detach().reshape(B, H * W).argmax(1).to(torch.int32)
-    dists, act_mask, action = _native.opt_labels(maps, goal_idx)
-    policies = torch.zeros((B, 8, 1, H, W), dtype=torch.float32, device=maps.device)
+    dists, act_mask, action = _native.opt_labels(maps, goal_idx, mechanism)
+    policies = torch.zeros((B, 4 if mechanism == "news" else 8, 1, H, W), dtype=torch.float32, device=maps.device)
     policies.scatter_(1, action.long().view(B, 1, 1, H, W), 1.0)
     return policies, dists, act_mask
 
@@ -571,23 +575,27 @@ def tile_maps(maps: torch.Tensor, tile_size: int, indices=None, generator: torch
 
 
 def draw_opt_policies(act_mask: torch.Tensor, generator: torch.Generator = None,
-                      draws: torch.Tensor = None) -> torch.Tensor:
+                      draws: torch.Tensor = None, num_actions: int = 8) -> torch.Tensor:
     """One-hot optimal policies with the planning-datasets generator's rule (extract_policy): every cell takes one
     member of its maximal action set uniformly, instead of compute_opt_labels' first maximum.  One kernel launch.
 
     act_mask: CUDA uint8 [B,1,H,W] from compute_opt_labels (bit a set iff action a is maximal).  Cell c takes set bit
     (d * popc) >> 32 in action order, d its u32 draw: torch.randint on the device with `generator` (a CUDA generator;
-    the default one when None), or the given int32 [B,1,H,W] / [B,H,W] tensor `draws`.  Returns float32 [B,8,1,H,W]
-    (a cell with an empty mask gets an all-zero column)."""
+    the default one when None), or the given int32 [B,1,H,W] / [B,H,W] tensor `draws`.  Returns float32
+    [B,num_actions,1,H,W] (a cell with an empty mask gets an all-zero column).  num_actions = 4 is for the masks of
+    compute_opt_labels(..., mechanism="news"), which never set bits 4..7: the draw then lies in planes 0..3."""
     if not act_mask.is_cuda:
         raise RuntimeError("draw_opt_policies runs on CUDA tensors only (there is no CPU fallback)")
+    if num_actions not in (4, 8):
+        raise ValueError(f"num_actions must be 4 (news) or 8 (moore) (got {num_actions})")
     mask = act_mask[:, 0] if act_mask.ndim == 4 else act_mask
     if draws is None:
         draws = torch.randint(-2 ** 31, 2 ** 31, tuple(mask.shape), dtype=torch.int32, device=mask.device,
                               generator=generator)
     elif draws.numel() != mask.numel():
         raise ValueError(f"draws must have one entry per cell, {list(mask.shape)}")
-    return _native.draw_policies(mask, draws.to(mask.device, torch.int32))
+    policies = _native.draw_policies(mask, draws.to(mask.device, torch.int32))
+    return policies if num_actions == 8 else policies[:, :num_actions].contiguous()
 
 
 def _np(x) -> np.ndarray:
@@ -597,15 +605,17 @@ def _np(x) -> np.ndarray:
 def save_planning_dataset(path: str, train, valid, test) -> None:
     """Write a planning-datasets .npz (np.savez_compressed arr_0..arr_11, reference generate_spp_instances.py:48-62)
     that MazeDataset / create_dataloader read.  Each split is (maps [N,H,W] or [N,1,H,W], goal_maps [N,1,H,W],
-    opt_policies [N,8,1,H,W], opt_dists [N,1,H,W]), NumPy arrays or tensors; they are stored in the dtype given."""
+    opt_policies [N,8,1,H,W] (moore) or [N,4,1,H,W] (news), opt_dists [N,1,H,W]), NumPy arrays or tensors; they are
+    stored in the dtype given."""
     arrays = []
     for name, split in (("train", train), ("valid", valid), ("test", test)):
         maps, goals, policies, dists = (_np(x) for x in split)
         if maps.ndim == 4:
             maps = maps[:, 0]
         N, H, W = maps.shape
-        if (goals.shape != (N, 1, H, W) or policies.shape != (N, 8, 1, H, W) or dists.shape != (N, 1, H, W)):
-            raise ValueError(f"{name}: expected maps [N,H,W], goals / dists [N,1,H,W], policies [N,8,1,H,W] "
+        if (goals.shape != (N, 1, H, W) or policies.shape not in ((N, 8, 1, H, W), (N, 4, 1, H, W))
+                or dists.shape != (N, 1, H, W)):
+            raise ValueError(f"{name}: expected maps [N,H,W], goals / dists [N,1,H,W], policies [N,8|4,1,H,W] "
                              f"(got {maps.shape}, {goals.shape}, {policies.shape}, {dists.shape})")
         arrays += [maps, goals, policies, dists]
     np.savez_compressed(path, *arrays)

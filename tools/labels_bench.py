@@ -5,7 +5,9 @@ dijkstra_dist on the same machine's host cores (staged into oracle/_ref by build
 
 Workloads: the 1000 mazes_032 maps with their shipped goals (tests/golden/inputs_mazes032_all1000.npz) and 1024
 Config-5-style 256x256 maps (tools/c5_data.py, seed 1234).  Timing: CUDA events around 10 back-to-back calls, median
-of 3 trials, inputs device-resident.  Prints one JSON object; --out also writes it to a file.
+of 3 trials, inputs device-resident.  Each workload is timed with the Moore labels and, in the same run, with the NEWS
+labels (mechanism="news": 4-connected wavefronts, 4 policy targets; the "news" row).  Prints one JSON object; --out
+also writes it to a file.
 
     python tools/labels_bench.py [--out profiles/h100_labels_bench.json]
 """
@@ -94,14 +96,16 @@ def main():
         gi = torch.from_numpy(np.asarray(goal_idx, np.int32)).to(dev)
         goals = torch.zeros_like(maps).view(len(maps), -1).scatter_(1, gi.long()[:, None], 1.0).view_as(maps)
         B = maps.shape[0]
-        k_ms, k_trials = timed(lambda: _native.opt_labels(maps, gi))
-        a_ms, _ = timed(lambda: compute_opt_labels(maps, goals))
-        d = _native.opt_labels(maps, gi)[0].view(B, -1)
-        reached = d.masked_fill(d <= -d.shape[1], 0)
-        out[name] = {"maps": B, "grid": f"{maps.shape[-2]}x{maps.shape[-1]}", "kernel_ms": k_ms,
-                     "kernel_ms_trials": k_trials, "maps_per_s": B / (k_ms * 1e-3),
-                     "compute_opt_labels_ms": a_ms, "compute_opt_labels_maps_per_s": B / (a_ms * 1e-3),
-                     "max_bfs_depth": int(-reached.min())}
+        rows = {}
+        for mech in ("moore", "news"):
+            k_ms, k_trials = timed(lambda: _native.opt_labels(maps, gi, mech))
+            a_ms, _ = timed(lambda: compute_opt_labels(maps, goals, mech))
+            d = _native.opt_labels(maps, gi, mech)[0].view(B, -1)
+            reached = d.masked_fill(d <= -d.shape[1], 0)
+            rows[mech] = {"kernel_ms": k_ms, "kernel_ms_trials": k_trials, "maps_per_s": B / (k_ms * 1e-3),
+                          "compute_opt_labels_ms": a_ms, "compute_opt_labels_maps_per_s": B / (a_ms * 1e-3),
+                          "max_bfs_depth": int(-reached.min())}
+        out[name] = {"maps": B, "grid": f"{maps.shape[-2]}x{maps.shape[-1]}", **rows["moore"], "news": rows["news"]}
     out["cpu_reference"] = cpu_reference(o1k, g.z["goal_idx"])
     line = json.dumps(out)
     print(line)
