@@ -75,6 +75,28 @@ def test_backward_status_codes(built_lib, no_launch, kw, status):
     assert no_launch.nastar_b200_backward(_bwd(built_lib, **kw), None) == status
 
 
+# (H, W) -> (nastar_b200_engine_for, nastar_b200_bin16_supported) for the shapes the GPU tests choose per engine
+# (test_gpu_forward_parity.py, test_gpu_backward_parity.py, test_gpu_engine_schedules.py): a threshold change must not
+# move one of them to another engine unnoticed.  1 = warp32, 4 = warp64, 2 / 3 = generic with state in shared memory /
+# in the HBM workspace; bin16 = engine 5 takes binary aliased planes of this shape.
+ENGINE_TABLE = {
+    (32, 32): (1, 0),
+    **{hw: (4, 0) for hw in [(33, 33), (1, 64), (64, 1), (2, 64), (64, 2), (32, 33), (33, 32), (40, 20), (20, 40),
+                             (63, 64), (47, 61), (64, 64), (48, 64), (50, 47), (48, 40)]},
+    **{hw: (2, 1) for hw in [(65, 40), (1, 65), (70, 3), (97, 131), (131, 131), (96, 64), (96, 50), (65, 41),
+                             (100, 72)]},
+    **{hw: (3, 1) for hw in [(131, 132), (132, 132), (144, 136), (160, 128), (256, 256)]},
+    (512, 512): (3, 0),
+    (600, 64): (3, 0),
+}
+
+
+def test_engine_table(built_lib):
+    L = built_lib.lib()
+    got = {hw: (L.nastar_b200_engine_for(*hw), L.nastar_b200_bin16_supported(*hw)) for hw in ENGINE_TABLE}
+    assert got == ENGINE_TABLE
+
+
 def test_glue_entry_points_status_codes(no_launch):
     L = no_launch
     assert L.nastar_b200_batch_steps(0x10000, 0x20000, 4, 0, 0x30000, None) == EINVAL               # T = 0

@@ -30,6 +30,17 @@ def _relerr(a, b):
     return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
+def _assert_grad(gc, want, G, what):
+    """gc within TOL of `want` relative to its largest magnitude.  A loop of one step (T = int(Tmax * W * W) = 1, e.g.
+    a 2-wide map in training) selects the start with softmax weight 1, so the exact gradient is 0 everywhere and there is
+    no magnitude to compare with: the kernel's event sums then cancel to fp64 rounding of the upstream gradient."""
+    assert np.isfinite(gc).all()
+    if not np.abs(want).any():
+        assert float(np.abs(gc).max()) < 1e-12 * float(np.abs(G).max()), what
+    else:
+        assert _relerr(gc, want) < TOL, what
+
+
 def _fwd_bwd(native, cost, start, goal, obst, G, g_ratio, T):
     c, s, g, o = _dev(cost), _dev(start), _dev(goal), _dev(obst)
     hist, paths, ts, ns, _ = native.forward(c, s, g, o, g_ratio, T)
@@ -65,10 +76,13 @@ def test_random_upstream_gradient_vs_reference_autograd(native, name, T_key, out
     assert _relerr(gc, g.plane(out_key)) < TOL
 
 
-@pytest.mark.parametrize("H,W", [(32, 32), (12, 12), (7, 5), (16, 32), (31, 29)])
+@pytest.mark.parametrize("H,W", [(32, 32), (12, 12), (7, 5), (16, 32), (31, 29),
+                                 (33, 33), (64, 2), (40, 20), (131, 131), (131, 132)])
 @pytest.mark.parametrize("g_ratio", [0.5, 0.8, 0.3])
 def test_random_problems_vs_oracle(native, oracle, H, W, g_ratio):
-    """g_ratio < 0.5 exercises the non-stationary post-solve emulation (SURVEY App. A.4)."""
+    """g_ratio < 0.5 exercises the non-stationary post-solve emulation (SURVEY App. A.4).  Engine 1 up to 32x32, engine 4
+    for (33, 33), (64, 2) and (40, 20), and the generic engine on both sides of its shared-memory limit: (131, 131) keeps
+    its state on chip, (131, 132) in the HBM workspace."""
     rng = np.random.RandomState(H * 100 + W + int(g_ratio * 10))
     B = 16
     obst = (rng.rand(B, 1, H, W) > 0.2).astype(np.float32)
@@ -78,8 +92,13 @@ def test_random_problems_vs_oracle(native, oracle, H, W, g_ratio):
     obst[:, 0, -1, -1] = 1
     start[:, 0, 0, 0] = 1
     goal[:, 0, -1, -1] = 1
-    # keep only solvable maps (the reference cannot differentiate through NaN)
-    ref = oracle.forward(obst, start, goal, obst, mode="spec")
+    # a row of obstacles cuts a 2-wide map in two: open its first cell (no row of the wider maps here is all obstacles)
+    planes = obst[:, 0]
+    planes[planes.max(-1) == 0, 0] = 1
+    # keep only solvable maps (the reference cannot differentiate through NaN); max(H, W)^2 >= H*W steps reach every
+    # reachable goal, and for H <= W it is the loop bound itself.  With H > W the loop bound W*W may stop before the
+    # goal: (64, 2) takes 4 steps and checks capped maps only
+    ref = oracle.forward(obst, start, goal, obst, mode="spec", T=max(H, W) ** 2)
     keep = ref.t_solve >= 0
     assert keep.sum() >= 2, "seeded draw must contain solvable maps"
     obst, start, goal = obst[keep], start[keep], goal[keep]
@@ -100,13 +119,11 @@ def test_random_problems_vs_oracle(native, oracle, H, W, g_ratio):
                 lit = oracle.forward(cost[sl], start[sl], goal[sl], obst[sl], g_ratio=g_ratio, mode="literal", T=T)
                 assert lit.T_batch == Tb
                 want = oracle.backward(cost[sl], start[sl], goal[sl], obst[sl], G[sl], Tb, g_ratio=g_ratio)
-                assert np.isfinite(gc).all()
-                assert _relerr(gc, want) < TOL, (H, W, g_ratio, Tmax, i)
+                _assert_grad(gc, want, G[sl], (H, W, g_ratio, Tmax, i))
             continue
         _, gc, Tb, ts = _fwd_bwd(native, cost, start, goal, obst, G, g_ratio, T)
         want = oracle.backward(cost, start, goal, obst, G, Tb, g_ratio=g_ratio)
-        assert np.isfinite(gc).all()
-        assert _relerr(gc, want) < TOL, (H, W, g_ratio, Tmax)
+        _assert_grad(gc, want, G, (H, W, g_ratio, Tmax))
 
 
 def test_module_api_backward_reaches_encoder(native, oracle):
@@ -138,7 +155,8 @@ def test_module_api_backward_reaches_encoder(native, oracle):
     assert _relerr(cost.grad.cpu().numpy(), want) < TOL
 
 
-@pytest.mark.parametrize("H,W,B", [(64, 64, 6), (40, 48, 5), (33, 70, 4), (144, 136, 2), (33, 64, 4), (65, 96, 2)])
+@pytest.mark.parametrize("H,W,B", [(64, 64, 6), (40, 48, 5), (33, 70, 4), (144, 136, 2), (33, 64, 4), (65, 96, 2),
+                                   (131, 131, 3), (131, 132, 3)])
 def test_generic_engine_backward_vs_oracle(native, oracle, H, W, B):
     """Backward for maps larger than 32x32 (engine 2: smem state; engine 3: HBM workspace)."""
     rng = np.random.RandomState(H * 7 + W)

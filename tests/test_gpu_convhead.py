@@ -59,7 +59,8 @@ def _fp64_taps_and_bound(x, w, b, hw):
     return taps, bound + 1e-12
 
 
-@pytest.mark.parametrize("B,H,W", [(1, 32, 32), (7, 32, 32), (100, 32, 32), (3, 64, 64), (5, 20, 27), (4, 5, 3)])
+@pytest.mark.parametrize("B,H,W", [(1, 32, 32), (7, 32, 32), (100, 32, 32), (3, 64, 64), (5, 20, 27), (4, 5, 3),
+                                   (100, 64, 64), (1000, 32, 32)])   # production batches: 3200 and 8000 tiles
 def test_fused_taps_within_tf32_bound_of_fp64(native, B, H, W):
     x, w, b, hw = _problem(B, H, W, seed=B * 1000 + H * 10 + W)
     got = native.conv3x3_head_taps(x, w, b, hw)

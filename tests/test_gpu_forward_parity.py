@@ -93,12 +93,20 @@ def _random_problem(rng, B, H, W, p_obst, learned, unreachable_ok=True):
     return cost, start, goal, obst
 
 
-SHAPES = [(32, 32), (12, 12), (1, 1), (1, 32), (32, 1), (5, 7), (31, 29), (16, 32), (32, 16), (3, 3), (20, 12), (12, 20)]
+SHAPES = [(32, 32), (12, 12), (1, 1), (1, 32), (32, 1), (5, 7), (31, 29), (16, 32), (32, 16), (3, 3), (20, 12), (12, 20),
+          # engine 4 (nastar_warp64.cuh): up to 64x64, not both sides <= 32
+          (33, 33), (1, 64), (64, 1), (2, 64), (64, 2), (32, 33), (33, 32), (40, 20), (63, 64), (47, 61),
+          # generic engine: state in shared memory up to (131, 131), in the HBM workspace from (131, 132) on
+          (65, 40), (1, 65), (70, 3), (97, 131), (131, 131), (131, 132), (144, 136)]
 
 
 @pytest.mark.parametrize("learned", [False, True])
 @pytest.mark.parametrize("H,W", SHAPES)
 def test_random_vs_oracle(native, oracle, H, W, learned):
+    """Every engine a shape selects (tests/test_abi_cpu.py pins the table).  Above 64x64 both cost kinds run on the
+    generic engine: learned costs always do, and binary aliased planes do too because a trace is requested (engine 5
+    records none).  When H > W the loop bound T = W*W is below N = H*W, so (64, 2) and (144, 136) also reach the step
+    cap and the T-1 hop backtrack of unsolved maps."""
     rng = np.random.RandomState(1000 * H + 10 * W + int(learned))
     B = 24
     for p_obst, g_ratio in ((0.0, 0.5), (0.25, 0.5), (0.45, 0.5), (0.2, 0.8), (0.2, 0.3)):
@@ -173,9 +181,11 @@ def test_low_g_ratio_batch_coupled_module_matches_reference(name):
     np.testing.assert_array_equal(sel.cpu().numpy(), g.z["trace"])
 
 
-@pytest.mark.parametrize("H,W", [(32, 32), (12, 12), (64, 64), (20, 40)])
+@pytest.mark.parametrize("H,W", [(32, 32), (12, 12), (64, 64), (20, 40), (65, 40), (144, 136)])
 def test_no_early_exit_kernel_vs_oracle(native, oracle, H, W):
-    """NASTAR_FWD_NO_EARLY_EXIT: exactly T steps per map, bit-exact trace vs the SPEC oracle in the same mode."""
+    """NASTAR_FWD_NO_EARLY_EXIT: exactly T steps per map, bit-exact trace vs the SPEC oracle in the same mode.  The
+    batch-coupled path (g_ratio < 0.5) runs this mode on every engine, including the generic one ((65, 40) keeps its
+    state in shared memory, (144, 136) in the HBM workspace)."""
     rng = np.random.RandomState(H + 3 * W)
     cost, start, goal, obst = _random_problem(rng, 12, H, W, 0.15, True)
     for g_ratio, T in ((0.0, 150), (0.3, 300), (0.5, 200)):
