@@ -52,6 +52,13 @@ enum {
                                       cost = obst (astar.py:93-94).  Every output array then holds 2B entries.
                                       Engine-1 shapes (H,W <= 32) run both halves in one kernel launch; other
                                       shapes issue the two halves back to back inside this call */
+#define NASTAR_FWD_NEWS 4          /* 4-connected search of the generator's NorthEastWestSouth mechanism
+                                      (mechanism.py:113-131): a selected cell opens and relaxes only its N, E, W and S
+                                      neighbours, and h = manhattan + 0.001 * euclid to the goal instead of chebyshev
+                                      + 0.001 * euclid.  Everything else (selection, cost charged at the selected cell,
+                                      early exit, backtrack, t_solve codes) is unchanged.  Without it the search is
+                                      Moore (8-connected).  Applies to both halves of NASTAR_FWD_PAIR.  Engines 1, 4,
+                                      2 and 3; engine 5 is never used for it */
 
 /* nastar_fwd_params.cost_kind: what `cost` points to (SURVEY.md 8(f)-3, encoder -> search hand-off) */
 #define NASTAR_COST_PLANE 0  /* finished cost maps, fp32 [B][H*W] (differentiable_astar.py:150-157) */
@@ -142,8 +149,14 @@ size_t nastar_b200_backward_workspace_bytes(int32_t B, int32_t H, int32_t W);
  * Asynchronous on `stream` (a cudaStream_t passed as void*). Returns NASTAR_*. */
 int nastar_b200_forward(const nastar_fwd_params *p, void *stream);
 
-/* Replaces autograd through the loop (closed form, SURVEY.md App. B): writes dL/dcost. */
+/* Replaces autograd through the loop (closed form, SURVEY.md App. B): writes dL/dcost.  Moore searches; it is
+ * nastar_b200_backward_mech(p, NASTAR_MECH_MOORE, stream). */
 int nastar_b200_backward(const nastar_bwd_params *p, void *stream);
+
+/* nastar_b200_backward for the search of either mechanism: NASTAR_MECH_MOORE, or NASTAR_MECH_NEWS to differentiate a
+ * forward that ran with NASTAR_FWD_NEWS (the replay then expands 4-connected with the Manhattan heuristic; the
+ * closed form itself does not depend on the stencil).  Any other mechanism is NASTAR_EINVAL, before any launch. */
+int nastar_b200_backward_mech(const nastar_bwd_params *p, int32_t mechanism, void *stream);
 
 /* T_batch[0] = min(T, 1 + max_b n_steps-style stop) computed on the device from the forward's
  * t_solve/n_steps arrays (replaces the host-synchronising torch.all(...) of :251). */
@@ -155,7 +168,8 @@ int nastar_b200_batch_steps(const int32_t *t_solve, const int32_t *n_steps, int3
  * 0 = unsupported.  Engine-2/3 shapes whose cost
  * plane IS the obstacle plane (same pointer and stride: VanillaAstar, astar.py:93-94) are first offered to
  * engine 5, the CTA-per-map binary-cost engine (csrc/nastar_bin16.cuh); maps it cannot take (a cost value
- * outside {0,1}) are re-run by engine 2/3 inside the same call. */
+ * outside {0,1}) are re-run by engine 2/3 inside the same call.  Engine 5 is Moore-only: a NASTAR_FWD_NEWS search
+ * of such a shape skips it and runs on engine 2/3 alone, in one launch. */
 int nastar_b200_engine_for(int32_t H, int32_t W);
 
 /* 1 if engine 5 (binary-cost, whole map in one CTA's shared memory) can hold this shape. */

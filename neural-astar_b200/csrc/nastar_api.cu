@@ -76,9 +76,9 @@ auto with_flags(F&& f, bool flag, Rest... rest) {
     return with_flags([&](auto... t) { return f(std::false_type{}, t...); }, rest...);
 }
 
-// one-time fill of the kSide x kSide heuristic table (g_heur32 / g_heur64) on the current device, stream-ordered
-// before first use; each table has its own per-device done mask
-template <int kSide>
+// one-time fill of the kSide x kSide heuristic table (g_heur32 / g_heur64, or their NEWS twins) on the current device,
+// stream-ordered before first use; each table has its own per-device done mask
+template <int kSide, bool kNews = false>
 cudaError_t ensure_heur(cudaStream_t stream) {
     static std::atomic<uint64_t> done_mask{0};
     int dev = 0;
@@ -86,7 +86,7 @@ cudaError_t ensure_heur(cudaStream_t stream) {
     if (e != cudaSuccess) return e;
     const uint64_t bit = uint64_t(1) << (dev & 63);
     if (done_mask.load(std::memory_order_acquire) & bit) return cudaSuccess;
-    auto* const init = kSide == 32 ? nastar::heur32_init_kernel : nastar::heur64_init_kernel;
+    auto* const init = kSide == 32 ? nastar::heur32_init_kernel<kNews> : nastar::heur64_init_kernel<kNews>;
     init<<<kSide * kSide / 256, 256, 0, stream>>>();
     g_launches.fetch_add(1, std::memory_order_relaxed);
     e = cudaGetLastError();
@@ -250,25 +250,26 @@ int nastar_b200_forward(const nastar_fwd_params* p, void* stream_v) {
     const bool trace = p->trace != nullptr;
     const bool noexit = (p->flags & NASTAR_FWD_NO_EARLY_EXIT) != 0;
     const bool fused = p->cost_kind != NASTAR_COST_PLANE;
+    const bool news = (p->flags & NASTAR_FWD_NEWS) != 0;
     if (engine == 1) {
-        const cudaError_t e = ensure_heur<32>(stream);
+        const cudaError_t e = news ? ensure_heur<32, true>(stream) : ensure_heur<32>(stream);
         if (e != cudaSuccess) return cuda_fail(e);
         nastar::W32Args a{};
         a.f = *p;
-        with_flags([&](auto kTrace, auto kNoExit, auto kFused) {
-            nastar::astar_warp32_kernel<kTrace, false, kNoExit, kFused><<<nmaps, 32, 0, stream>>>(a);
-        }, trace, noexit, fused);
+        with_flags([&](auto kTrace, auto kNoExit, auto kFused, auto kNews) {
+            nastar::astar_warp32_kernel<kTrace, false, kNoExit, kFused, kNews><<<nmaps, 32, 0, stream>>>(a);
+        }, trace, noexit, fused, news);
         return launched();
     }
     if (engine == 4) {
-        cudaError_t e = ensure_heur<64>(stream);
+        cudaError_t e = news ? ensure_heur<64, true>(stream) : ensure_heur<64>(stream);
         if (e != cudaSuccess) return cuda_fail(e);
         nastar::W64Args wa{};
         wa.f = *p;
-        e = with_flags([&](auto kTrace, auto kNoExit, auto kFused) {
-            return launch_smem(nastar::astar_warp64_kernel<kTrace, kNoExit, false, kFused>, p->B, 32,
+        e = with_flags([&](auto kTrace, auto kNoExit, auto kFused, auto kNews) {
+            return launch_smem(nastar::astar_warp64_kernel<kTrace, kNoExit, false, kFused, kNews>, p->B, 32,
                                sizeof(nastar::W64Smem), stream, wa);
-        }, trace, noexit, fused);
+        }, trace, noexit, fused, news);
         if (e != cudaSuccess) return cuda_fail(e);
         return launched();
     }
@@ -281,10 +282,11 @@ int nastar_b200_forward(const nastar_fwd_params* p, void* stream_v) {
     nastar::GenArgs ga{};
     ga.f = *p;
     // engine 5 first when the cost plane IS the binary obstacle plane (VanillaAstar / Config 5): whole map on
-    // chip, one CTA per SM pulling maps from a queue; maps it flags are re-run below by the generic engine
+    // chip, one CTA per SM pulling maps from a queue; maps it flags are re-run below by the generic engine.
+    // Engine 5 is Moore-only: NEWS searches go straight to the generic engine.
     const bool aliased = (p->obst == p->cost) && (p->obst_stride == p->cost_stride);
     const size_t aux = bin16_aux_bytes(p->B);
-    if (bin16_enabled() && aliased && !p->trace && p->flags == 0 && bin16_shape_ok(p->H, p->W) && p->workspace &&
+    if (bin16_enabled() && aliased && !news && !p->trace && p->flags == 0 && bin16_shape_ok(p->H, p->W) && p->workspace &&
         p->workspace_bytes >= aux + slots_bytes) {
         unsigned char* ws = static_cast<unsigned char*>(p->workspace);
         nastar::Bin16Args ba{};
@@ -312,18 +314,25 @@ int nastar_b200_forward(const nastar_fwd_params* p, void* stream_v) {
         ga.f.workspace = ws + aux;
         ga.f.workspace_bytes = p->workspace_bytes - aux;
     }
-    const cudaError_t e = with_flags([&](auto kGlobal, auto kTrace, auto kNoExit) {
-        return launch_smem(nastar::astar_generic_kernel<kGlobal, kTrace, false, kNoExit>, grid, 32, smem, stream, ga);
-    }, global, trace, noexit);
+    const cudaError_t e = with_flags([&](auto kGlobal, auto kTrace, auto kNoExit, auto kNews) {
+        return launch_smem(nastar::astar_generic_kernel<kGlobal, kTrace, false, kNoExit, kNews>, grid, 32, smem, stream,
+                           ga);
+    }, global, trace, noexit, news);
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();
 }
 
 int nastar_b200_backward(const nastar_bwd_params* p, void* stream_v) {
+    return nastar_b200_backward_mech(p, NASTAR_MECH_MOORE, stream_v);
+}
+
+int nastar_b200_backward_mech(const nastar_bwd_params* p, int32_t mechanism, void* stream_v) {
     if (!p || !p->cost || !p->start || !p->goal || !p->obst || !p->grad_histories || !p->grad_cost || !p->T_batch ||
         !p->t_solve)
         return NASTAR_EINVAL;
     if (p->B <= 0 || p->H <= 0 || p->W <= 0) return NASTAR_EINVAL;
+    if (mechanism != NASTAR_MECH_MOORE && mechanism != NASTAR_MECH_NEWS) return NASTAR_EINVAL;
+    const bool news = mechanism == NASTAR_MECH_NEWS;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
     const int engine = nastar_b200_engine_for(p->H, p->W);
     if (engine == 0) return NASTAR_EUNSUPPORTED;
@@ -331,16 +340,21 @@ int nastar_b200_backward(const nastar_bwd_params* p, void* stream_v) {
     if (engine == 1) {
         // dynamic shared memory = the per-cell interval state of the event-based closed form (W32Bwd, 32 KB); with the
         // 17.4 KB of static planes that is above the 48 KB default, hence the opt-in
-        e = ensure_heur<32>(stream);
+        e = news ? ensure_heur<32, true>(stream) : ensure_heur<32>(stream);
         if (e == cudaSuccess)
-            e = launch_smem(nastar::astar_warp32_kernel<false, true>, p->B, 32, sizeof(nastar::W32Bwd), stream,
-                            bwd_kernel_args<nastar::W32Args>(p));
+            e = with_flags([&](auto kNews) {
+                return launch_smem(nastar::astar_warp32_kernel<false, true, false, false, kNews>, p->B, 32,
+                                   sizeof(nastar::W32Bwd), stream, bwd_kernel_args<nastar::W32Args>(p));
+            }, news);
     } else if (engine == 4) {
         // warp-resident 64-wide engine: event-based closed form next to the forward state in shared memory
-        e = ensure_heur<64>(stream);
+        e = news ? ensure_heur<64, true>(stream) : ensure_heur<64>(stream);
         if (e == cudaSuccess)
-            e = launch_smem(nastar::astar_warp64_kernel<false, false, true>, p->B, 32,
-                            sizeof(nastar::W64Smem) + sizeof(nastar::W64Bwd), stream, bwd_kernel_args<nastar::W64Args>(p));
+            e = with_flags([&](auto kNews) {
+                return launch_smem(nastar::astar_warp64_kernel<false, false, true, false, kNews>, p->B, 32,
+                                   sizeof(nastar::W64Smem) + sizeof(nastar::W64Bwd), stream,
+                                   bwd_kernel_args<nastar::W64Args>(p));
+            }, news);
     } else {
         const nastar::GenericLayout L(p->H, p->W);
         const bool global = (engine == 3);
@@ -348,9 +362,10 @@ int nastar_b200_backward(const nastar_bwd_params* p, void* stream_v) {
         if (!p->workspace || p->workspace_bytes < size_t(grid) * L.slot_total(global, true)) return NASTAR_EWORKSPACE;
         const size_t smem = L.smem_common() + (global ? 0 : L.smem_planes());
         const nastar::GenArgs ga = bwd_kernel_args<nastar::GenArgs>(p);
-        e = with_flags([&](auto kGlobal) {
-            return launch_smem(nastar::astar_generic_kernel<kGlobal, false, true>, grid, 32, smem, stream, ga);
-        }, global);
+        e = with_flags([&](auto kGlobal, auto kNews) {
+            return launch_smem(nastar::astar_generic_kernel<kGlobal, false, true, false, kNews>, grid, 32, smem, stream,
+                               ga);
+        }, global, news);
     }
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();

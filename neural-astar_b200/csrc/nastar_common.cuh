@@ -32,6 +32,22 @@ __device__ __forceinline__ float heuristic(int y, int x, int gy, int gx) {
     return __fadd_rn(cheb, __fmul_rn(0.001f, euc));
 }
 
+// The generator's NorthEastWestSouth.get_heuristic (planning_datasets_utils/mechanism.py:124-131): manhattan +
+// 0.001 * euclid, all in fp32.  The manhattan term is an exact integer, like the Chebyshev one above.
+__device__ __forceinline__ float heuristic_news(int y, int x, int gy, int gx) {
+    int idy = y - gy, idx = x - gx;
+    int ady = idy < 0 ? -idy : idy, adx = idx < 0 ? -idx : idx;
+    float manh = static_cast<float>(ady + adx);                               // exact
+    float euc = __fsqrt_rn(static_cast<float>(ady * ady + adx * adx));       // exact int -> IEEE sqrt
+    return __fadd_rn(manh, __fmul_rn(0.001f, euc));
+}
+
+// heuristic of the search's mechanism: kNews = NASTAR_FWD_NEWS / NASTAR_MECH_NEWS (4-connected), else Moore
+template <bool kNews>
+__device__ __forceinline__ float heuristic_of(int y, int x, int gy, int gx) {
+    return kNews ? heuristic_news(y, x, gy, gx) : heuristic(y, x, gy, gx);
+}
+
 // encoder.py:32-34, cost = sigmoid(x) * const, with the operation sequence of ATen's CUDA sigmoid
 // (1 / (1 + exp(-x)), full-precision expf and IEEE division) followed by a separately rounded multiply.
 __device__ __forceinline__ float sigmoid_scaled(float x, float scale) {

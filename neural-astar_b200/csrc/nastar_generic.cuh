@@ -61,7 +61,9 @@ struct GenArgs {
 // maintained incrementally in fp64 from the <= 9 events of a step — O(1) work per step instead of a dense
 // O(N/32) softmax pass (round 1).  Per-cell state (v, A(t0), B(t0), acc) lives in the per-CTA workspace slot.
 // kNoExit (forward only): NASTAR_FWD_NO_EARLY_EXIT — keep stepping after the solve step, exactly T steps.
-template <bool kGlobal, bool kTrace, bool kBwd, bool kNoExit = false>
+// kNews: NASTAR_FWD_NEWS / NASTAR_MECH_NEWS — only lanes 1, 3, 5, 7 (N, W, E, S) take a neighbour, and h is the
+// Manhattan heuristic.
+template <bool kGlobal, bool kTrace, bool kBwd, bool kNoExit = false, bool kNews = false>
 __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
     constexpr bool kContinue = kBwd || kNoExit;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -234,7 +236,7 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
         auto gh_at = [&](int i) -> float { return (blocked && i == goal_idx) ? 0.f : __ldg(gG + i); };
         if (start_idx >= 0 && lane == 0) {
             const int sy = start_idx / W, sx = start_idx - sy * W;
-            const float h0 = __fadd_rn(heuristic(sy, sx, gy, gx), cost_at(start_idx));
+            const float h0 = __fadd_rn(heuristic_of<kNews>(sy, sx, gy, gx), cost_at(start_idx));
             const float f0 = f_value(gr, omg, 0.f, h0);
             G[start_idx] = 0.f;
             F[start_idx] = f0;
@@ -297,11 +299,12 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
                     if (k < rs_key) { rs_key = k; rs_col = x; }
                 }
             }
-            // neighbour cell of this lane (lanes 0..8, centre excluded)
+            // neighbour cell of this lane (lanes 0..8, centre excluded; NEWS: the odd lanes, no diagonals)
             const int k9 = lane;
             const int dr = k9 / 3 - 1, dc = k9 - (k9 / 3) * 3 - 1;
             const int y = r + dr, x = c + dc;
-            const bool valid = (lane < 9) && (lane != 4) && (unsigned(y) < unsigned(H)) && (unsigned(x) < unsigned(W));
+            const bool valid = (lane < 9) && (kNews ? (lane & 1) != 0 : lane != 4) && (unsigned(y) < unsigned(H)) &&
+                               (unsigned(x) < unsigned(W));
             const int n = y * W + x;
             bool passable = false, isopen = false, isclosed = false;
             float gn = 0.f;
@@ -319,7 +322,7 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
             uint32_t key = kKeyInf;
             double dS = 0.0, dD = 0.0;   // backward: this lane's change of S and D
             if (upd) {
-                const float hn = __fadd_rn(heuristic(y, x, gy, gx), cost_at(n));
+                const float hn = __fadd_rn(heuristic_of<kNews>(y, x, gy, gx), cost_at(n));
                 const float fn = f_value(gr, omg, g2, hn);
                 G[n] = g2;
                 F[n] = fn;

@@ -43,11 +43,14 @@ constexpr int kCells = 1024;  // padded 32 x 32
 // heuristic(|dy|, |dx|) for every offset on a 32x32 grid, filled once per device by
 // heur32_init_kernel with the very same device function the generic engine evaluates inline —
 // the per-map h pass becomes one cached load + one add per cell instead of an IEEE sqrt chain.
-__device__ float g_heur32[kCells];
+// The second half, g_heur32[kCells + i], is a second table holding the NEWS heuristic (heuristic_news) the same way;
+// it shares the array so that every kernel keeps its global address table.
+__device__ float g_heur32[2 * kCells];
 
+template <bool kNews>
 __global__ void heur32_init_kernel() {
     const int i = threadIdx.x + blockIdx.x * blockDim.x;
-    if (i < kCells) g_heur32[i] = heuristic(i >> 5, i & 31, 0, 0);
+    if (i < kCells) g_heur32[(kNews ? kCells : 0) + i] = heuristic_of<kNews>(i >> 5, i & 31, 0, 0);
 }
 
 // backward-only planes (dynamic shared memory), event-based closed form (see nastar_generic.cuh / DESIGN.md):
@@ -74,7 +77,8 @@ struct __align__(16) W32Smem {
 // kNoExit (forward only): NASTAR_FWD_NO_EARLY_EXIT — keep stepping after the solve step, exactly T steps.
 // kFused (forward only): the prologue may have to finish the encoder (NASTAR_COST_LOGIT / NASTAR_COST_TAPS); kept out
 // of the plain instantiation so that its cold instruction footprint stays small.
-template <bool kTrace, bool kBwd, bool kNoExit = false, bool kFused = false>
+// kNews: NASTAR_FWD_NEWS / NASTAR_MECH_NEWS — 4-connected expansion (N, E, W, S) and the Manhattan heuristic.
+template <bool kTrace, bool kBwd, bool kNoExit = false, bool kFused = false, bool kNews = false>
 __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
     constexpr bool kContinue = kBwd || kNoExit;   // the loop does not stop at the solve step
     __shared__ W32Smem S;
@@ -180,7 +184,7 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
         for (int y = 0; y < H; ++y) {
             const int i = (y << 5) + lane;
             const int ady = (y > gy) ? (y - gy) : (gy - y);
-            sGH[i] = make_float2(0.f, __fadd_rn(__ldg(&g_heur32[(ady << 5) | adx]), S.cost[i]));
+            sGH[i] = make_float2(0.f, __fadd_rn(__ldg(&g_heur32[(kNews ? kCells : 0) + ((ady << 5) | adx)]), S.cost[i]));
         }
     }
     __syncwarp();
@@ -287,7 +291,8 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
         }
         // -- expansion (:228-249) as mask algebra on this lane's row ---------------------------
         //    idx = ((1-open)(1-hist) + open*(g > g2)) * neighbours * obstacles   (:235-236)
-        const uint32_t win = isr ? (m0 | m2) : (m0 | m1 | m2);
+        //    NEWS: the own row's left/right neighbours, and only column c of the rows above and below
+        const uint32_t win = isr ? (m0 | m2) : (kNews ? m1 : (m0 | m1 | m2));
         const uint32_t cand = near ? (win & pass) : 0u;
         const uint32_t gt = ((n0.x > g2) ? m0 : 0u) | ((n1.x > g2) ? m1 : 0u) | ((n2.x > g2) ? m2 : 0u);
         const uint32_t upd = cand & ((open & gt) | ~(open | closed));

@@ -23,12 +23,13 @@ namespace nastar {
 
 constexpr int kCells64 = 4096;  // padded 64 x 64
 
-// heuristic(|dy|, |dx|) for every offset on a 64x64 grid (see g_heur32)
-__device__ float g_heur64[kCells64];
+// heuristic(|dy|, |dx|) for every offset on a 64x64 grid, then the NEWS table (see g_heur32)
+__device__ float g_heur64[2 * kCells64];
 
+template <bool kNews>
 __global__ void heur64_init_kernel() {
     const int i = threadIdx.x + blockIdx.x * blockDim.x;
-    if (i < kCells64) g_heur64[i] = heuristic(i >> 6, i & 63, 0, 0);
+    if (i < kCells64) g_heur64[(kNews ? kCells64 : 0) + i] = heuristic_of<kNews>(i >> 6, i & 63, 0, 0);
 }
 
 struct __align__(16) W64Smem {
@@ -64,7 +65,8 @@ struct W64Args {
 
 // kFused (forward only): the prologue may have to finish the encoder (NASTAR_COST_LOGIT / NASTAR_COST_TAPS), as in the
 // 32-wide engine; kept out of the plain instantiations.
-template <bool kTrace, bool kNoExit, bool kBwd = false, bool kFused = false>
+// kNews: 4-connected expansion and the Manhattan heuristic, as in the 32-wide engine.
+template <bool kTrace, bool kNoExit, bool kBwd = false, bool kFused = false, bool kNews = false>
 __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
     constexpr bool kContinue = kBwd || kNoExit;
     const nastar_fwd_params& p = a.f;
@@ -176,8 +178,9 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
         for (int y = 0; y < H; ++y) {
             const int i = (y << 6) + lane;
             const int ady = (y > gy) ? (y - gy) : (gy - y);
-            sGH[i] = make_float2(0.f, __fadd_rn(__ldg(&g_heur64[(ady << 6) | adx0]), S.cost[i]));
-            sGH[i + 32] = make_float2(0.f, __fadd_rn(__ldg(&g_heur64[(ady << 6) | adx1]), S.cost[i + 32]));
+            const float* heur = g_heur64 + (kNews ? kCells64 : 0);
+            sGH[i] = make_float2(0.f, __fadd_rn(__ldg(&heur[(ady << 6) | adx0]), S.cost[i]));
+            sGH[i + 32] = make_float2(0.f, __fadd_rn(__ldg(&heur[(ady << 6) | adx1]), S.cost[i + 32]));
         }
     }
     __syncwarp();
@@ -287,7 +290,7 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
             if (!solved) myopen &= ~m1;
             mykey = kKeyInf;
         }
-        const u64 win = isr ? (m0 | m2) : (m0 | m1 | m2);
+        const u64 win = isr ? (m0 | m2) : (kNews ? m1 : (m0 | m1 | m2));   // NEWS: no diagonal neighbours
         const u64 cand = near ? (win & mypass) : 0ull;
         const u64 gt = ((n0.x > g2) ? m0 : 0ull) | ((n1.x > g2) ? m1 : 0ull) | ((n2.x > g2) ? m2 : 0ull);
         const u64 upd = cand & ((myopen & gt) | ~(myopen | myclosed));

@@ -68,6 +68,7 @@ _SIGNATURES = {
     "nastar_b200_backward_workspace_bytes": (ctypes.c_size_t, [_i32] * 3),
     "nastar_b200_forward": (_int, [ctypes.POINTER(FwdParams), _p]),
     "nastar_b200_backward": (_int, [ctypes.POINTER(BwdParams), _p]),
+    "nastar_b200_backward_mech": (_int, [ctypes.POINTER(BwdParams), _i32, _p]),
     "nastar_b200_batch_steps": (_int, [_p, _p, _i32, _i32, _p, _p]),
     "nastar_b200_engine_for": (_int, [_i32, _i32]),
     "nastar_b200_bin16_supported": (_int, [_i32, _i32]),
@@ -182,7 +183,19 @@ def launch_count() -> int:
 
 FWD_NO_EARLY_EXIT = 1
 FWD_PAIR = 2
+FWD_NEWS = 4
 COST_PLANE, COST_LOGIT, COST_TAPS = 0, 1, 2
+
+
+# NASTAR_MECH_*: the planning-datasets generator's --mechanism values
+MECHANISMS = {"moore": 0, "news": 1}
+
+
+def mechanism_code(mechanism: str) -> int:
+    """NASTAR_MECH_* of a mechanism name; anything but "moore" and "news" is a ValueError."""
+    if mechanism not in MECHANISMS:
+        raise ValueError(f"mechanism must be one of {sorted(MECHANISMS)} (got {mechanism!r})")
+    return MECHANISMS[mechanism]
 
 
 class SearchCounts(tuple):
@@ -192,7 +205,7 @@ class SearchCounts(tuple):
 def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: torch.Tensor,
             g_ratio: float, T: int, want_trace: bool = False, no_early_exit: bool = False, *,
             pair: bool = False, cost_kind: int = COST_PLANE, cost_scale: float = 1.0, cost_bias: float = 0.0,
-            want_counts: bool = False):
+            want_counts: bool = False, mechanism: str = "moore"):
     """Run the search for a batch of [B,C,H,W] fp32 CUDA planes (channel 0 is used).
 
     Returns (histories [B',1,H,W] f32, paths [B',1,H,W] i64, t_solve [B'] i32, n_steps [B'] i32,
@@ -201,7 +214,10 @@ def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: t
     (NASTAR_FWD_PAIR: second half = the same problems with cost = obstacles), else B.
     `cost_kind` = COST_LOGIT / COST_TAPS: `cost` holds the encoder's raw output [B,1,H,W] / the 9-tap partial
     products [B,H,W,9] and the kernel prologue finishes encoder.py:32-34 itself (H, W <= 64 only).
+    `mechanism` = "moore" (8-connected, Chebyshev heuristic) or "news" (NASTAR_FWD_NEWS: 4-connected, Manhattan
+    heuristic; both halves of a `pair`).
     """
+    news = mechanism_code(mechanism) == MECHANISMS["news"]
     L = lib()
     if not cost.is_cuda:
         raise RuntimeError("neural_astar (H100): the search runs on CUDA tensors only (no CPU fallback); "
@@ -229,7 +245,7 @@ def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: t
     p.B, p.H, p.W = B, H, W
     p.g_ratio, p.one_minus_g_ratio = gr, omg
     p.T = int(T)
-    p.flags = (FWD_NO_EARLY_EXIT if no_early_exit else 0) | (FWD_PAIR if pair else 0)
+    p.flags = (FWD_NO_EARLY_EXIT if no_early_exit else 0) | (FWD_PAIR if pair else 0) | (FWD_NEWS if news else 0)
     p.cost_kind, p.cost_scale, p.cost_bias = int(cost_kind), float(cost_scale), float(cost_bias)
     Bo = 2 * B if pair else B
     ws_bytes = _ws_cache.get((B, H, W))
@@ -383,8 +399,6 @@ def batch_steps(t_solve: torch.Tensor, n_steps: torch.Tensor, T: int) -> torch.T
 
 
 LABELS_MAX_SIDE = 512
-# NASTAR_MECH_*: the planning-datasets generator's --mechanism values
-MECHANISMS = {"moore": 0, "news": 1}
 
 
 def opt_labels(maps: torch.Tensor, goal_idx: torch.Tensor, mechanism: str = "moore"):
@@ -637,8 +651,10 @@ def draw_policies(act_mask: torch.Tensor, draws: torch.Tensor) -> torch.Tensor:
 
 
 def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Tensor, t_solve: torch.Tensor,
-             g_ratio: float) -> torch.Tensor:
-    """dL/dcost [B,1,H,W] from dL/dhistories (closed form of the reference's autograd, SURVEY App. B)."""
+             g_ratio: float, mechanism: str = "moore") -> torch.Tensor:
+    """dL/dcost [B,1,H,W] from dL/dhistories (closed form of the reference's autograd, SURVEY App. B), for a forward
+    that ran with the same `mechanism`."""
+    mech = mechanism_code(mechanism)
     L = lib()
     dev = cost.device
     B, _, H, W = cost.shape
@@ -657,6 +673,6 @@ def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Te
         p.grad_cost = grad_cost.data_ptr()
         p.workspace = ws.data_ptr() if ws is not None else None
         p.workspace_bytes = ws_bytes
-        _check(L.nastar_b200_backward(ctypes.byref(p), stream), "nastar_b200_backward")
+        _check(L.nastar_b200_backward_mech(ctypes.byref(p), mech, stream), "nastar_b200_backward_mech")
     del keep
     return grad_cost

@@ -23,12 +23,15 @@ import torch.nn.functional as F
 
 from .. import _native
 from . import encoder as _encoders
-from .differentiable_astar import AstarOutput, DifferentiableAstar
+from .differentiable_astar import AstarOutput, DifferentiableAstar, TakesMechanism, _mech_kw
 from .pq_astar import pq_astar  # noqa: F401  re-exported, like the reference module does
 
 
-class VanillaAstar(nn.Module):
+class VanillaAstar(nn.Module, metaclass=TakesMechanism):
     """A* on the given map: cost == obstacles == map design (reference :93-94).
+
+    Keyword-only `mechanism` = "moore" (default, 8-connected) or "news" (4-connected with the Manhattan heuristic, for
+    the planning-datasets generator's NEWS datasets); see DifferentiableAstar.
 
     >>> out = VanillaAstar()(map_designs, start_maps, goal_maps)   # out.histories, out.paths
     """
@@ -41,6 +44,11 @@ class VanillaAstar(nn.Module):
         self.astar = DifferentiableAstar(g_ratio=g_ratio, Tmax=Tmax)
         self.g_ratio = g_ratio
         self.use_differentiable_astar = use_differentiable_astar
+
+    def _select_mechanism(self, mechanism: str) -> None:
+        if not self.use_differentiable_astar:
+            raise NotImplementedError("pq_astar (use_differentiable_astar=False) searches Moore neighbourhoods only")
+        self.astar._select_mechanism(mechanism)
 
     def perform_astar(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
                       obstacles_maps: torch.Tensor, store_intermediate_results: bool = False) -> AstarOutput:
@@ -68,6 +76,8 @@ class NeuralAstar(VanillaAstar):
         learn_obstacles: hide the obstacle map from the search (all cells passable).
         const: learnable multiplier on the predicted cost (None = 1).
         use_differentiable_astar: kept for compatibility, see module docstring.
+        mechanism (keyword-only): "moore" (default) or "news": the search's neighbourhood and heuristic, see
+            DifferentiableAstar.
     """
 
     def __init__(self, g_ratio: float = 0.5, Tmax: float = 1.0, encoder_input: str = "m+", encoder_arch: str = "CNN",
@@ -125,7 +135,8 @@ class NeuralAstar(VanillaAstar):
     def forward_pair(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
                      vanilla_g_ratio: float = 0.5):
         """Validation pair (reference utils/training.py:63-87) in one search launch: returns
-        (outputs of this planner, outputs of VanillaAstar on the same batch, (n_closed [2B], path_len [2B]))
+        (outputs of this planner, outputs of VanillaAstar on the same batch with this planner's mechanism,
+        (n_closed [2B], path_len [2B]))
         or None when the single-launch form does not apply (autograd on, CPU tensors, learn_obstacles, different
         g_ratio for the baseline, g_ratio < 0.5 batches, pq_astar).  Inference only."""
         B = start_maps.shape[0]
@@ -136,13 +147,13 @@ class NeuralAstar(VanillaAstar):
             return None
         H, W = start_maps.shape[-2], start_maps.shape[-1]
         T = self.astar.num_steps(W)
-        kw = {}
+        kw = _mech_kw(self.astar.mechanism)
         cost = None
         if H <= 64 and W <= 64 and self.encoder.fast_path_ok(map_designs):
             head = self._head_taps(map_designs, start_maps, goal_maps)
             if head is not None:
                 cost, bias, scale = head
-                kw = dict(cost_kind=_native.COST_TAPS, cost_bias=bias, cost_scale=scale)
+                kw.update(cost_kind=_native.COST_TAPS, cost_bias=bias, cost_scale=scale)
         if cost is None:
             cost = self.encode(map_designs, start_maps, goal_maps)
         hist, paths, _, _, _, counts = _native.forward(cost, start_maps, goal_maps, map_designs, float(self.g_ratio), T,

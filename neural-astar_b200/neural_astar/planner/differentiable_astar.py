@@ -44,17 +44,77 @@ def get_heuristic(goal_maps: torch.Tensor, tb_factor: float = 0.001) -> torch.Te
     return (cheb + tb_factor * euc).reshape_as(goal_maps)
 
 
+def get_news_heuristic(goal_maps: torch.Tensor, tb_factor: float = 0.001) -> torch.Tensor:
+    """Manhattan distance + tb_factor * Euclidean distance to the goal: the planning-datasets generator's
+    NorthEastWestSouth.get_heuristic (planning_datasets_utils/mechanism.py:124-131), for any H x W.
+
+    `DifferentiableAstar(mechanism="news").get_heuristic`; the engine evaluates the same expression on-chip
+    (csrc/nastar_common.cuh: heuristic_news()).
+    """
+    B, H, W = goal_maps.shape[0], goal_maps.shape[-2], goal_maps.shape[-1]
+    flat = goal_maps.reshape(B, -1)
+    ys = torch.arange(H, device=goal_maps.device, dtype=goal_maps.dtype).repeat_interleave(W)
+    xs = torch.arange(W, device=goal_maps.device, dtype=goal_maps.dtype).repeat(H)
+    gy = (flat * ys).sum(-1, keepdim=True)
+    gx = (flat * xs).sum(-1, keepdim=True)
+    dy, dx = (ys - gy).abs(), (xs - gx).abs()
+    euc = torch.sqrt(dy * dy + dx * dx)
+    return ((dy + dx) + tb_factor * euc).reshape_as(goal_maps)
+
+
+def neighbor_filter_of(mechanism: str) -> torch.Tensor:
+    """The 3x3 neighbour filter [1,1,3,3] of a mechanism: Moore = all but the centre (reference :139-143), NEWS = N,
+    W, E, S (NorthEastWestSouth.get_neighbor_filter, mechanism.py:113-121)."""
+    _check_mechanism(mechanism)
+    if mechanism == "news":
+        f = torch.zeros(1, 1, 3, 3)
+        f[0, 0, 0, 1] = f[0, 0, 1, 0] = f[0, 0, 1, 2] = f[0, 0, 2, 1] = 1
+    else:
+        f = torch.ones(1, 1, 3, 3)
+        f[0, 0, 1, 1] = 0
+    return f
+
+
+MECHANISMS = ("moore", "news")   # the planning-datasets generator's --mechanism values
+
+
+def _check_mechanism(mechanism: str) -> None:
+    if mechanism not in MECHANISMS:
+        raise ValueError(f"mechanism must be one of {list(MECHANISMS)} (got {mechanism!r})")
+
+
+def _mech_kw(mechanism: str) -> dict:
+    """Keyword arguments of the _native search calls for a mechanism: none for Moore, the engine's default."""
+    return {} if mechanism == "moore" else {"mechanism": mechanism}
+
+
+class TakesMechanism(type):
+    """Metaclass of the planners: `Planner(*args, mechanism="news", **kwargs)` runs __init__ with the other arguments,
+    then `planner._select_mechanism(mechanism)`.  So the keyword-only `mechanism` ("moore", the default, or "news")
+    exists while every __init__ keeps the reference's signature, which positional callers and checkpoint tooling rely
+    on.  Any other value is a ValueError, raised before anything is built."""
+
+    def __call__(cls, *args, mechanism: str = "moore", **kwargs):
+        _check_mechanism(mechanism)
+        planner = super().__call__(*args, **kwargs)
+        if mechanism != "moore":
+            planner._select_mechanism(mechanism)
+        return planner
+
+
 class _AstarSearch(torch.autograd.Function):
     """forward: libnastar_b200 search; backward: closed-form dL/dcost kernel."""
 
     @staticmethod
-    def forward(ctx, cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped=None):
+    def forward(ctx, cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped=None,
+                mechanism="moore"):
         # goal_clamped is given only on the batch-coupled path (g_ratio < 0.5, see _coupled_steps): the search then
         # runs exactly T steps per map and the backward is told which goals were selected more than once
         no_early_exit = goal_clamped is not None
         hist, paths, t_solve, n_steps, trace = _native.forward(
-            cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, no_early_exit)
+            cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, no_early_exit, **_mech_kw(mechanism))
         ctx.g_ratio = g_ratio
+        ctx.mechanism = mechanism
         ctx.T = T
         ctx.no_early_exit = no_early_exit
         if no_early_exit:
@@ -77,15 +137,16 @@ class _AstarSearch(torch.autograd.Function):
                 T_batch = torch.full((1,), ctx.T, dtype=torch.int32, device=cost.device)
             else:
                 T_batch = _native.batch_steps(t_solve, n_steps, ctx.T)
-            grad_cost = _native.backward(cost, start, goal, obst, grad_hist.contiguous(), T_batch, t_solve, ctx.g_ratio)
+            grad_cost = _native.backward(cost, start, goal, obst, grad_hist.contiguous(), T_batch, t_solve, ctx.g_ratio,
+                                         **_mech_kw(ctx.mechanism))
             if grad_cost.shape != cost.shape:  # cost had extra channels: only channel 0 is searched (:177)
                 full = torch.zeros_like(cost)
                 full[:, :1] = grad_cost
                 grad_cost = full
-        return grad_cost, None, None, None, None, None, None, None
+        return grad_cost, None, None, None, None, None, None, None, None
 
 
-class DifferentiableAstar(nn.Module):
+class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
     def __init__(self, g_ratio: float = 0.5, Tmax: float = 1.0):
         """
         Differentiable A* module (reference :129-148).
@@ -93,17 +154,27 @@ class DifferentiableAstar(nn.Module):
         Args:
             g_ratio: ratio between g(v) + h(v). Set 0 to perform as best-first search.
             Tmax: how much of the map the planner explores during training.
+        Keyword-only (TakesMechanism):
+            mechanism: "moore" (8-connected, Chebyshev heuristic, the reference's search) or "news" (4-connected,
+                Manhattan heuristic: the planning-datasets generator's NorthEastWestSouth, for its *_news_* datasets).
+                This keyword alone decides the search; `neighbor_filter` and `get_heuristic` are set to match it but
+                are never read by the engine.
         """
         super().__init__()
-        # kept so that reference checkpoints load with "All keys matched" (state-dict key
-        # `astar.neighbor_filter`); the 3x3 Moore stencil itself is hard-wired in the kernel.
-        neighbor_filter = torch.ones(1, 1, 3, 3)
-        neighbor_filter[0, 0, 1, 1] = 0
-        self.neighbor_filter = nn.Parameter(neighbor_filter, requires_grad=False)
+        self.mechanism = "moore"
+        # kept so that reference checkpoints load with "All keys matched" (state-dict key `astar.neighbor_filter`) and
+        # a NEWS planner's state dict looks like a reference model given the generator's NEWS filter; the stencil
+        # itself is compiled into the kernel and chosen by `mechanism`.
+        self.neighbor_filter = nn.Parameter(neighbor_filter_of("moore"), requires_grad=False)
         self.get_heuristic = get_heuristic
         self.g_ratio = g_ratio
         assert (Tmax > 0) & (Tmax <= 1), "Tmax must be within (0, 1]"
         self.Tmax = Tmax
+
+    def _select_mechanism(self, mechanism: str) -> None:
+        self.mechanism = mechanism
+        self.neighbor_filter.data = neighbor_filter_of(mechanism)
+        self.get_heuristic = get_news_heuristic if mechanism == "news" else get_heuristic
 
     def num_steps(self, width: int) -> int:
         """Loop bound of the reference (:200-202): int(Tmax_eff * W * W), W = last dim."""
@@ -135,9 +206,11 @@ class DifferentiableAstar(nn.Module):
             # Reproduce it: step every map without early exit, find the first step at which ALL maps select
             # their goal, and take the state after exactly that many steps.  (One host sync; the reference
             # synchronises every step.)
-            T, goal_clamped = _coupled_steps(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T)
+            T, goal_clamped = _coupled_steps(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T,
+                                             self.mechanism)
         hist, paths, t_solve, n_steps, trace = _AstarSearch.apply(
-            cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, bool(store_intermediate_results), goal_clamped)
+            cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, bool(store_intermediate_results), goal_clamped,
+            self.mechanism)
 
         intermediate_results: List[dict] = []
         if store_intermediate_results:
@@ -156,20 +229,20 @@ class DifferentiableAstar(nn.Module):
         T = self.num_steps(W)
         hist, paths, t_solve, n_steps, trace = _native.forward(
             taps, start_maps, goal_maps, obstacles_maps, float(self.g_ratio), T, bool(store_intermediate_results),
-            cost_kind=_native.COST_TAPS, cost_scale=scale, cost_bias=bias)
+            cost_kind=_native.COST_TAPS, cost_scale=scale, cost_bias=bias, **_mech_kw(self.mechanism))
         frames: List[dict] = []
         if store_intermediate_results:
             frames = _materialise_frames(hist, paths, goal_maps, t_solve, n_steps, trace, T)
         return AstarOutput(hist, paths, frames)
 
 
-def _coupled_steps(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio: float, T: int):
+def _coupled_steps(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio: float, T: int, mechanism: str = "moore"):
     """(T_batch, goal_clamped[B]) for g_ratio < 0.5: the number of iterations the reference's loop executes when
     solved maps keep evolving, and per map whether its goal is selected more than once within them — then
     clamp(hist + sel) saw 2 at the goal and blocks its gradient (differentiable_astar.py:222-223)."""
     with torch.no_grad():
         _, _, _, _, trace = _native.forward(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T,
-                                            want_trace=True, no_early_exit=True)
+                                            want_trace=True, no_early_exit=True, **_mech_kw(mechanism))
         B = goal_maps.shape[0]
         goal_idx = goal_maps[:, 0].reshape(B, -1).argmax(-1).to(trace.dtype)
         at_goal = trace == goal_idx[:, None]

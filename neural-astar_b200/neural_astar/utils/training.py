@@ -167,7 +167,9 @@ class PlannerModule(_ModuleBase):
     def __init__(self, planner, config):
         super().__init__()
         self.planner = planner
-        self.vanilla_astar = VanillaAstar()
+        # the validation baseline searches the planner's neighbourhood (forward_pair's vanilla half does too)
+        astar = getattr(planner, "astar", None)
+        self.vanilla_astar = VanillaAstar(mechanism=getattr(astar, "mechanism", "moore"))
         self.config = config
 
     # -- Lightning hooks (same names as the reference) ---------------------------------------------
