@@ -237,7 +237,7 @@ int nastar_b200_selftest_sqrt(int32_t n, int32_t *mismatches, void *stream);
 int nastar_b200_opt_labels(const float *maps, int64_t map_stride, const int32_t *goal_idx, int32_t B, int32_t H,
                            int32_t W, float *dists, uint8_t *act_mask, int8_t *action, void *stream);
 
-/* mechanism of nastar_b200_opt_labels_mech: the planning-datasets generator's --mechanism (mechanism.py:267-277) */
+/* mechanism of nastar_b200_opt_labels_mech and nastar_b200_weighted_labels_mech: the planning-datasets generator's --mechanism (mechanism.py:267-277) */
 #define NASTAR_MECH_MOORE 0   /* 8 actions: N, E, W, S, NE, NW, SE, SW (the labels of nastar_b200_opt_labels) */
 #define NASTAR_MECH_NEWS  1   /* 4 actions: N, E, W, S (NorthEastWestSouth, mechanism.py:52-131) */
 
@@ -278,6 +278,18 @@ int nastar_b200_weighted_labels(const float *cost, int64_t cost_stride, const fl
                                 const int32_t *goal_idx, const int32_t *start_idx, int32_t B, int32_t H, int32_t W,
                                 float *dists, int32_t *hops, uint8_t *act_mask, int8_t *action, float *path_maps,
                                 float *path_costs, int32_t *status, void *stream);
+
+/* nastar_b200_weighted_labels for either mechanism.  NASTAR_MECH_MOORE gives exactly nastar_b200_weighted_labels'
+ * output.  NASTAR_MECH_NEWS: moves are actions 0..3 = N, E, W, S only (into an in-grid 4-neighbour that is passable or
+ * is the goal); D, hops, the policy, the roll-out, path_costs and status follow the same rules over those 4 moves, and
+ * act_mask uses bits 0..3 only.  Every argument is checked before the launch: a mechanism other than these two is
+ * NASTAR_EINVAL.  One kernel launch, one CTA per map.  H, W <= 128, else NASTAR_EUNSUPPORTED.  Asynchronous on
+ * `stream`.  Returns NASTAR_*. */
+int nastar_b200_weighted_labels_mech(const float *cost, int64_t cost_stride, const float *passable,
+                                     int64_t passable_stride, const int32_t *goal_idx, const int32_t *start_idx,
+                                     int32_t B, int32_t H, int32_t W, int32_t mechanism, float *dists, int32_t *hops,
+                                     uint8_t *act_mask, int8_t *action, float *path_maps, float *path_costs,
+                                     int32_t *status, void *stream);
 
 /* Training-batch sampler, preparation (MazeDataset._prepared's per-map work, once per dataset, one kernel launch).
  * dists fp32 [B][H*W] (opt_dists), policies fp32 [B][8][H*W] (opt_policies; the first maximal action of each cell

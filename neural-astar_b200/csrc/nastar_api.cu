@@ -473,23 +473,36 @@ int nastar_b200_opt_labels(const float* maps, int64_t map_stride, const int32_t*
                                        stream_v);
 }
 
-int nastar_b200_weighted_labels(const float* cost, int64_t cost_stride, const float* passable, int64_t passable_stride,
-                                const int32_t* goal_idx, const int32_t* start_idx, int32_t B, int32_t H, int32_t W,
-                                float* dists, int32_t* hops, uint8_t* act_mask, int8_t* action, float* path_maps,
-                                float* path_costs, int32_t* status, void* stream_v) {
+int nastar_b200_weighted_labels_mech(const float* cost, int64_t cost_stride, const float* passable,
+                                     int64_t passable_stride, const int32_t* goal_idx, const int32_t* start_idx,
+                                     int32_t B, int32_t H, int32_t W, int32_t mechanism, float* dists, int32_t* hops,
+                                     uint8_t* act_mask, int8_t* action, float* path_maps, float* path_costs,
+                                     int32_t* status, void* stream_v) {
     if (!cost || !goal_idx || !dists || !hops || !act_mask || !action || !status || B <= 0 || H <= 0 || W <= 0)
         return NASTAR_EINVAL;
     if (cost_stride < int64_t(H) * W || (passable && passable_stride < int64_t(H) * W)) return NASTAR_EINVAL;
     // paths need a start per map, and a start needs somewhere to put its path
     if (bool(start_idx) != bool(path_maps) || bool(start_idx) != bool(path_costs)) return NASTAR_EINVAL;
+    if (mechanism != NASTAR_MECH_MOORE && mechanism != NASTAR_MECH_NEWS) return NASTAR_EINVAL;
     if (H > nastar::kWLabelsMaxSide || W > nastar::kWLabelsMaxSide || int64_t(H) * W > nastar::kWLabelsMaxCells)
         return NASTAR_EUNSUPPORTED;
     const nastar::WLabelsArgs a{cost,   cost_stride, passable,  passable_stride, goal_idx,   start_idx, B,     H, W,
                                 dists,  hops,        act_mask,  action,          path_maps,  path_costs, status};
-    const cudaError_t e = launch_smem(nastar::weighted_labels_kernel, B, nastar::wlabels_threads(H, W),
-                                      nastar::wlabels_smem_bytes(H, W), static_cast<cudaStream_t>(stream_v), a);
+    auto* const kernel = mechanism == NASTAR_MECH_NEWS ? nastar::weighted_labels_kernel<true>
+                                                       : nastar::weighted_labels_kernel<false>;
+    const cudaError_t e = launch_smem(kernel, B, nastar::wlabels_threads(H, W), nastar::wlabels_smem_bytes(H, W),
+                                      static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();
+}
+
+int nastar_b200_weighted_labels(const float* cost, int64_t cost_stride, const float* passable, int64_t passable_stride,
+                                const int32_t* goal_idx, const int32_t* start_idx, int32_t B, int32_t H, int32_t W,
+                                float* dists, int32_t* hops, uint8_t* act_mask, int8_t* action, float* path_maps,
+                                float* path_costs, int32_t* status, void* stream_v) {
+    return nastar_b200_weighted_labels_mech(cost, cost_stride, passable, passable_stride, goal_idx, start_idx, B, H, W,
+                                            NASTAR_MECH_MOORE, dists, hops, act_mask, action, path_maps, path_costs,
+                                            status, stream_v);
 }
 
 int nastar_b200_sampler_prepare(const float* dists, const float* policies, const float* goal_maps, int32_t B, int32_t H,

@@ -5,7 +5,8 @@
 //   inputs   cost c fp32 [H,W]; passable (value != 0; no plane = every cell passable); a goal; optionally a start.
 //   moves    actions 0..7 = N, E, W, S, NE, NW, SE, SW (the Moore mechanism of nastar_labels.cuh); a diagonal move
 //            does not check the orthogonal cells; a move leaves a passable cell and enters an in-grid cell that is
-//            passable or is the goal (the goal is always enterable and is the source).
+//            passable or is the goal (the goal is always enterable and is the source).  kNews: actions 0..3 = N, E,
+//            W, S only (the NEWS mechanism), everything below with "4 moves" for "8 moves".
 //   D        cost-to-go: D[goal] = +0, D[v] = min over moves v->t of fl(D[t] + c[t]) (one __fadd_rn per move, no
 //            contraction), +inf where the goal cannot be reached.  For c >= 0, x -> fl(x + c) is monotone and never
 //            decreases x, so D is the minimum over all paths of the fp32 left fold from the goal: it does not depend
@@ -26,9 +27,10 @@
 //
 // One CTA per map, one launch.  Everything lives in shared memory: D and c (fp32), hop (u16, exact since
 // hop < H*W <= 16384), the passable bit plane and three rotating "changed" bit planes (u32 row words).
-//   1. D: frontier Bellman-Ford.  A cell is re-evaluated only in the round after one of its 8 neighbours changed;
-//      a cell that lowers its D marks its neighbours in the next plane.  Updates are in place (D only decreases and
-//      every value read is the fold of a real path, so a stale read is only a later re-evaluation).  The loop ends
+//   1. D: frontier Bellman-Ford.  A cell is re-evaluated only in the round after one of its 8 (kNews: 4) neighbours
+//      changed; a cell that lowers its D marks itself and those neighbours in the next plane.  Updates are in place
+//      (D only decreases and every value read is the fold of a real path, so a stale read is only a later
+//      re-evaluation).  The loop ends
 //      when a round changes nothing (__syncthreads_or); it is capped at H*W + 1 rounds (Bellman-Ford needs at most
 //      H*W - 1), so input that skipped validation cannot hang the GPU.
 //   2. hop: BFS wavefronts over the optimal-move relation, frontier-driven the same way, capped the same way.
@@ -90,6 +92,7 @@ struct WLMap {
         return t == goal || ((pas[ty * nw + (tx >> 5)] >> (tx & 31)) & 1u);
     }
     // bit a set iff action a is an optimal move from v = (y, x) into a cell one hop closer to the goal
+    template <bool kNews>
     __device__ uint32_t policy_mask(int y, int x) const {
         const int v = y * W + x;
         const int hv = hop[v];
@@ -99,7 +102,7 @@ struct WLMap {
         constexpr int dxs[8] = {0, +1, -1, 0, +1, -1, +1, -1};
         uint32_t m = 0;
 #pragma unroll
-        for (int a = 0; a < 8; ++a) {
+        for (int a = 0; a < (kNews ? 4 : 8); ++a) {
             const int ty = y + dys[a], tx = x + dxs[a];
             if (ty < 0 || ty >= H || tx < 0 || tx >= W || !enterable(ty, tx)) continue;
             const int t = ty * W + tx;
@@ -109,14 +112,17 @@ struct WLMap {
     }
 };
 
-// mark the 3x3 block around (y, x) in a row-word bit plane
+// mark the 3x3 block around (y, x) in a row-word bit plane; kNews: (y, x) and its 4 neighbours only
+template <bool kNews>
 __device__ __forceinline__ void wl_mark(uint32_t* plane, int nw, int H, int W, int y, int x) {
     const int lo = x > 0 ? x - 1 : 0, hi = x + 1 < W ? x + 1 : W - 1;
     const int wl = lo >> 5, wh = hi >> 5;
     for (int yy = y - 1; yy <= y + 1; ++yy) {
         if (yy < 0 || yy >= H) continue;
         uint32_t* row = plane + yy * nw;
-        if (wl == wh) {
+        if (kNews && yy != y) {
+            atomicOr(row + (x >> 5), 1u << (x & 31));
+        } else if (wl == wh) {
             atomicOr(row + wl, ((2u << (hi - lo)) - 1u) << (lo & 31));
         } else {
             atomicOr(row + wl, ~0u << (lo & 31));
@@ -125,6 +131,7 @@ __device__ __forceinline__ void wl_mark(uint32_t* plane, int nw, int H, int W, i
     }
 }
 
+template <bool kNews>
 __global__ void __launch_bounds__(kWLabelsMaxThreads) weighted_labels_kernel(WLabelsArgs a) {
     extern __shared__ __align__(16) unsigned char wl_smem[];
     const int H = a.H, W = a.W, N = H * W, nw = (W + 31) >> 5, nwords = H * nw, nseg = 2 * nwords;
@@ -175,13 +182,14 @@ __global__ void __launch_bounds__(kWLabelsMaxThreads) weighted_labels_kernel(WLa
     const WLMap m{D, C, hop, pas, H, W, nw, goal};
     constexpr int dys[8] = {-1, 0, 0, +1, -1, -1, +1, +1};
     constexpr int dxs[8] = {0, +1, -1, 0, +1, -1, +1, -1};
+    constexpr int kMoves = kNews ? 4 : 8;   // the first 4 actions are N, E, W, S
     const int gy = ok ? goal / W : 0, gx = ok ? goal - gy * W : 0;
 
     if (ok) {
         if (tid == 0) {
             D[goal] = 0.0f;
             hop[goal] = 0;
-            wl_mark(P0, nw, H, W, gy, gx);
+            wl_mark<kNews>(P0, nw, H, W, gy, gx);
         }
         __syncthreads();
         // 1. cost-to-go
@@ -202,7 +210,7 @@ __global__ void __launch_bounds__(kWLabelsMaxThreads) weighted_labels_kernel(WLa
                     const float dv = D[v];
                     float best = dv;
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) {
+                    for (int k = 0; k < kMoves; ++k) {
                         const int ty = y + dys[k], tx = x + dxs[k];
                         if (ty < 0 || ty >= H || tx < 0 || tx >= W || !m.enterable(ty, tx)) continue;
                         const int t = ty * W + tx;
@@ -211,7 +219,7 @@ __global__ void __launch_bounds__(kWLabelsMaxThreads) weighted_labels_kernel(WLa
                     }
                     if (best < dv) {
                         D[v] = best;
-                        wl_mark(nxt, nw, H, W, y, x);
+                        wl_mark<kNews>(nxt, nw, H, W, y, x);
                         any = 1;
                     }
                 }
@@ -229,7 +237,7 @@ __global__ void __launch_bounds__(kWLabelsMaxThreads) weighted_labels_kernel(WLa
             P2[i] = 0u;
         }
         __syncthreads();
-        if (tid == 0) wl_mark(P0, nw, H, W, gy, gx);
+        if (tid == 0) wl_mark<kNews>(P0, nw, H, W, gy, gx);
         __syncthreads();
         cur = P0;
         nxt = P1;
@@ -250,7 +258,7 @@ __global__ void __launch_bounds__(kWLabelsMaxThreads) weighted_labels_kernel(WLa
                     if (hop[v] != kHopUnset || dv == kInf) continue;   // the goal has hop 0
                     bool hit = false;
 #pragma unroll
-                    for (int q = 0; q < 8; ++q) {
+                    for (int q = 0; q < kMoves; ++q) {
                         const int ty = y + dys[q], tx = x + dxs[q];
                         if (ty < 0 || ty >= H || tx < 0 || tx >= W || !m.enterable(ty, tx)) continue;
                         const int t = ty * W + tx;
@@ -258,7 +266,7 @@ __global__ void __launch_bounds__(kWLabelsMaxThreads) weighted_labels_kernel(WLa
                     }
                     if (hit) {
                         hop[v] = uint16_t(k);
-                        wl_mark(nxt, nw, H, W, y, x);
+                        wl_mark<kNews>(nxt, nw, H, W, y, x);
                         any = 1;
                     }
                 }
@@ -275,7 +283,7 @@ __global__ void __launch_bounds__(kWLabelsMaxThreads) weighted_labels_kernel(WLa
     const int64_t base = int64_t(b) * N;
     for (int c = tid; c < N; c += nthr) {
         const int y = c / W, x = c - y * W;
-        const uint32_t mk = ok ? m.policy_mask(y, x) : 0u;
+        const uint32_t mk = ok ? m.policy_mask<kNews>(y, x) : 0u;
         const int h = hop[c];
         a.dists[base + c] = __fsub_rn(0.0f, D[c]);
         a.hops[base + c] = h == kHopUnset ? -1 : h;
@@ -297,7 +305,7 @@ __global__ void __launch_bounds__(kWLabelsMaxThreads) weighted_labels_kernel(WLa
             int v = s, y = s / W, x = s - y * W;
             P0[y * nw + (x >> 5)] |= 1u << (x & 31);
             for (int step = 0; step < N && v != goal; ++step) {
-                const uint32_t mk = m.policy_mask(y, x);
+                const uint32_t mk = m.policy_mask<kNews>(y, x);
                 if (!mk) break;
                 const int q = __ffs(mk) - 1;
                 y += int((kWLMoveDy >> (2 * q)) & 3u) - 1;

@@ -81,6 +81,7 @@ _SIGNATURES = {
     "nastar_b200_opt_labels": (_int, [_p, _i64, _p, _i32, _i32, _i32, _p, _p, _p, _p]),
     "nastar_b200_opt_labels_mech": (_int, [_p, _i64, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _p]),
     "nastar_b200_weighted_labels": (_int, [_p, _i64, _p, _i64] + [_p] * 2 + [_i32] * 3 + [_p] * 8),
+    "nastar_b200_weighted_labels_mech": (_int, [_p, _i64, _p, _i64] + [_p] * 2 + [_i32] * 4 + [_p] * 8),
     "nastar_b200_sampler_prepare": (_int, [_p] * 3 + [_i32] * 3 + [ctypes.c_double] * 4 + [_p] * 7),
     "nastar_b200_sampler_sample": (_int, [_p] * 2 + [_i32] * 3 + [_p] * 6 + [_i32] * 2 + [_p] * 5),
     "nastar_b200_sample_goals": (_int, [_p, _i64] + [_i32] * 4 + [_p] * 5),
@@ -439,13 +440,16 @@ class WeightedLabels(tuple):
 
 
 def weighted_labels(cost: torch.Tensor, goal_idx: torch.Tensor, passable: Optional[torch.Tensor] = None,
-                    start_idx: Optional[torch.Tensor] = None) -> WeightedLabels:
+                    start_idx: Optional[torch.Tensor] = None, mechanism: str = "moore") -> WeightedLabels:
     """Exact vertex-weighted shortest paths of B cost maps in one kernel (include/nastar_b200.h,
-    nastar_b200_weighted_labels).
+    nastar_b200_weighted_labels_mech).
 
     cost: fp32 CUDA [B,H,W] or [B,1,H,W]; passable: the same shape (a cell is passable iff != 0) or None (every cell);
-    goal_idx / start_idx: int32 CUDA [B] flat indices (start_idx None: no paths).  H, W <= 128.  Asynchronous on the
-    current stream; the per-map status is not read back here."""
+    goal_idx / start_idx: int32 CUDA [B] flat indices (start_idx None: no paths); mechanism: "moore" (8 moves) or
+    "news" (4 moves N, E, W, S; act_mask bits 0..3 only).  H, W <= 128.  Asynchronous on the current stream; the
+    per-map status is not read back here."""
+    if mechanism not in MECHANISMS:
+        raise ValueError(f"weighted_labels: mechanism must be one of {sorted(MECHANISMS)} (got {mechanism!r})")
     L = lib()
 
     def plane(x, name):
@@ -473,12 +477,13 @@ def weighted_labels(cost: torch.Tensor, goal_idx: torch.Tensor, passable: Option
         paths = None if si is None else torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
         pcost = None if si is None else torch.empty((B,), dtype=torch.float32, device=dev)
         status = torch.empty((B,), dtype=torch.int32, device=dev)
-        _check(L.nastar_b200_weighted_labels(cptr, cstride, pptr, pstride, gi.data_ptr(),
-                                             None if si is None else si.data_ptr(), B, H, W, dists.data_ptr(),
-                                             hops.data_ptr(), mask.data_ptr(), action.data_ptr(),
-                                             None if paths is None else paths.data_ptr(),
-                                             None if pcost is None else pcost.data_ptr(), status.data_ptr(),
-                                             stream), "nastar_b200_weighted_labels")
+        _check(L.nastar_b200_weighted_labels_mech(cptr, cstride, pptr, pstride, gi.data_ptr(),
+                                                  None if si is None else si.data_ptr(), B, H, W,
+                                                  MECHANISMS[mechanism], dists.data_ptr(), hops.data_ptr(),
+                                                  mask.data_ptr(), action.data_ptr(),
+                                                  None if paths is None else paths.data_ptr(),
+                                                  None if pcost is None else pcost.data_ptr(), status.data_ptr(),
+                                                  stream), "nastar_b200_weighted_labels_mech")
     del c, p, gi, si
     return WeightedLabels((dists, hops, mask, action, paths, pcost, status))
 

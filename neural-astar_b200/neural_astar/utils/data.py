@@ -361,16 +361,19 @@ def _raise_on_bad_costs(status: torch.Tensor, what: str) -> None:
         raise ValueError(f"{what}: the goal or a passable cell has a negative, NaN or infinite cost in maps {bad}")
 
 
-def compute_weighted_opt_labels(cost_maps: torch.Tensor, goal_maps: torch.Tensor, passable: torch.Tensor = None):
+def compute_weighted_opt_labels(cost_maps: torch.Tensor, goal_maps: torch.Tensor, passable: torch.Tensor = None,
+                                mechanism: str = "moore"):
     """Exact vertex-weighted shortest-path labels of cost maps, computed on the GPU in one kernel launch
-    (DESIGN.md §11).  A move (8-connected, no corner check) leaves a passable cell, enters an in-grid cell that is
-    passable or is the goal, and costs the cost of the cell it enters; every sum is the fp32 fold from the goal.
+    (DESIGN.md §11).  A move (8-connected, no corner check; 4-connected with mechanism="news") leaves a passable cell,
+    enters an in-grid cell that is passable or is the goal, and costs the cost of the cell it enters; every sum is the
+    fp32 fold from the goal.
 
     cost_maps: CUDA [B,H,W] or [B,1,H,W], every cost that can be charged finite and >= 0; goal_maps: CUDA [B,1,H,W] or
     [B,H,W] with one 1 per map (the first maximum is taken); passable: CUDA maps of the same shape (a cell is passable
-    iff != 0), None = every cell.  H, W <= 128.
-    Returns, on the maps' device:
-      opt_policies [B,8,1,H,W] float32 one-hot of the first optimal action that leads one hop closer to the goal,
+    iff != 0), None = every cell.  H, W <= 128.  mechanism: "moore" (8 actions N, E, W, S, NE, NW, SE, SW) or "news"
+    (4 actions N, E, W, S: 4-connected moves, the optimum a 4-connected planner can reach).
+    Returns, on the maps' device, with A = 8 (moore) or 4 (news):
+      opt_policies [B,A,1,H,W] float32 one-hot of the first optimal action that leads one hop closer to the goal,
                    all zero at the goal and where the goal is unreachable;
       opt_dists    [B,1,H,W] float32: minus the cost-to-go (0 at the goal, -inf where the goal is unreachable);
       act_mask     [B,1,H,W] uint8: bit a set iff action a is optimal and leads one hop closer;
@@ -379,17 +382,20 @@ def compute_weighted_opt_labels(cost_maps: torch.Tensor, goal_maps: torch.Tensor
     reads the per-map status back to the host)."""
     cost, pas, goal_idx = _weighted_inputs(cost_maps, goal_maps, passable, "compute_weighted_opt_labels")
     B, H, W = cost.shape
-    dists, hops, act_mask, action, _, _, status = _native.weighted_labels(cost, goal_idx, pas)
+    dists, hops, act_mask, action, _, _, status = _native.weighted_labels(cost, goal_idx, pas, mechanism=mechanism)
     _raise_on_bad_costs(status, "compute_weighted_opt_labels")
-    policies = torch.zeros((B, 9, 1, H, W), dtype=torch.float32, device=cost.device)
-    policies.scatter_(1, (action.long() % 9).view(B, 1, 1, H, W), 1.0)    # action -1 lands in the dropped slot 8
-    return policies[:, :8].contiguous(), dists, act_mask, hops
+    A = 4 if mechanism == "news" else 8
+    policies = torch.zeros((B, A + 1, 1, H, W), dtype=torch.float32, device=cost.device)
+    policies.scatter_(1, (action.long() % (A + 1)).view(B, 1, 1, H, W), 1.0)   # action -1 lands in the dropped slot A
+    return policies[:, :A].contiguous(), dists, act_mask, hops
 
 
 def shortest_path_maps(cost_maps: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
-                       passable: torch.Tensor = None):
-    """Minimum-cost paths from the start to the goal of every map, in one kernel launch (the inputs and moves of
-    compute_weighted_opt_labels; start_maps [B,1,H,W] or [B,H,W] with one 1 per map).
+                       passable: torch.Tensor = None, mechanism: str = "moore"):
+    """Minimum-cost paths from the start to the goal of every map, in one kernel launch (the inputs, moves and
+    `mechanism` of compute_weighted_opt_labels; start_maps [B,1,H,W] or [B,H,W] with one 1 per map).  Judge a
+    planner against the optimum of its own mechanism: a 4-connected path never costs less than the "news" optimum,
+    which can be strictly dearer than the "moore" one.
 
     Returns (path_maps [B,1,H,W] float32: the cells of the path, start and goal included -- the layout of WarCraft's
     shortest_paths and of DifferentiableAstar's paths; path_costs [B] float32: the sum of the costs of every cell of
@@ -398,7 +404,7 @@ def shortest_path_maps(cost_maps: torch.Tensor, start_maps: torch.Tensor, goal_m
     cost, pas, goal_idx = _weighted_inputs(cost_maps, goal_maps, passable, "shortest_path_maps")
     B, H, W = cost.shape
     start_idx = start_maps.detach().reshape(B, H * W).argmax(1).to(torch.int32)
-    out = _native.weighted_labels(cost, goal_idx, pas, start_idx)
+    out = _native.weighted_labels(cost, goal_idx, pas, start_idx, mechanism)
     _raise_on_bad_costs(out[6], "shortest_path_maps")
     return out[4], out[5]
 

@@ -9,9 +9,13 @@ Workloads (inputs device-resident, one start and one goal per map):
   mazes_032_all1000      the 1000 mazes_032 problems, costs from the shipped checkpoint's encoder, map passability;
   all_064_test400        the 400 all_064 test problems, unit costs on their passable cells;
   random_128x128_b1024   1024 random 128x128 maps, 20 % obstacles, costs uniform in [0.1, 10), random start and goal.
-Timing: CUDA events around 10 back-to-back calls, median of 3 trials.  Prints one JSON object; --out also writes it.
+Timing: CUDA events around 10 back-to-back calls, median of 3 trials.  --mechanism takes moore (default, 8 moves)
+and/or news (4 moves N, E, W, S); with both, every timing alternates them trial by trial on the same inputs, the
+first mechanism's row stays at the top level of each workload and the other is nested under its name.  Prints one JSON
+object; --out also writes it.
 
     python tools/wlabels_bench.py [--out profiles/h100_wlabels_bench.json]
+    python tools/wlabels_bench.py --mechanism news moore [--out profiles/h100_wlabels_bench_news.json]
 """
 import argparse
 import json
@@ -27,12 +31,32 @@ for _p in (ROOT, os.path.join(ROOT, "neural-astar_b200"), os.path.join(ROOT, "te
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from labels_bench import timed  # noqa: E402
 
 _MOVES = ((-1, 0), (0, 1), (0, -1), (1, 0), (-1, 1), (-1, -1), (1, 1), (1, -1))
+NUM_MOVES = {"moore": 8, "news": 4}     # NEWS moves are the first four Moore actions
 
 
-def scipy_graph(cost, passable, goal):
+def timed_alternating(fns, reps=10):
+    """labels_bench.timed for several callables at once: each warmed up, then 3 trials in which every callable is
+    timed in turn (CUDA events around `reps` back-to-back calls), so they share the same stretch of time.  Returns
+    (median ms, trials) per callable."""
+    for fn in fns:
+        for _ in range(3):
+            fn()
+    trials = [[] for _ in fns]
+    for _ in range(3):
+        for i, fn in enumerate(fns):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            for _ in range(reps):
+                fn()
+            b.record()
+            torch.cuda.synchronize()
+            trials[i].append(a.elapsed_time(b) / reps)
+    return [(sorted(t)[1], t) for t in trials]
+
+
+def scipy_graph(cost, passable, goal, moves=_MOVES):
     """the reversed move graph: an edge t -> v of weight c[t] for every move v -> t"""
     from scipy.sparse import csr_matrix
 
@@ -43,7 +67,7 @@ def scipy_graph(cost, passable, goal):
     enter_ok = passable.ravel() != 0
     enter_ok[goal] = True
     rows, cols, w = [], [], []
-    for dy, dx in _MOVES:
+    for dy, dx in moves:
         ty, tx = ys + dy, xs + dx
         inside = (ty >= 0) & (ty < H) & (tx >= 0) & (tx < W)
         v, t = (ys * W + xs)[inside], (ty * W + tx)[inside]
@@ -54,14 +78,14 @@ def scipy_graph(cost, passable, goal):
     return csr_matrix((np.concatenate(w), (np.concatenate(rows), np.concatenate(cols))), shape=(H * W, H * W))
 
 
-def scipy_arm(cost, passable, goal_idx, n):
+def scipy_arm(cost, passable, goal_idx, n, moves=_MOVES):
     from scipy.sparse.csgraph import dijkstra
 
     n = min(n, len(cost))
     build = solve = 0.0
     for i in range(n):
         t0 = time.perf_counter()
-        g = scipy_graph(cost[i], passable[i], int(goal_idx[i]))
+        g = scipy_graph(cost[i], passable[i], int(goal_idx[i]), moves)
         t1 = time.perf_counter()
         dijkstra(g, directed=True, indices=int(goal_idx[i]))
         t2 = time.perf_counter()
@@ -122,7 +146,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--scipy-maps", type=int, default=50, help="maps per workload for the scipy arm")
+    ap.add_argument("--mechanism", nargs="+", choices=sorted(NUM_MOVES), default=["moore"],
+                    help="moore (8 moves) and/or news (4 moves); several are timed alternately")
     args = ap.parse_args()
+    mechs = list(dict.fromkeys(args.mechanism))
     from neural_astar import _native
     from neural_astar.utils.data import compute_weighted_opt_labels, shortest_path_maps
 
@@ -130,7 +157,9 @@ def main():
     dev = torch.device("cuda:0")
     out = {"kernel": "nastar::weighted_labels_kernel (frontier Bellman-Ford + hop wavefronts + policy + roll-out, "
                      "one CTA per map, all state in shared memory)",
-           "timing": "CUDA events around 10 back-to-back calls, median of 3 trials; inputs device-resident",
+           "timing": "CUDA events around 10 back-to-back calls, median of 3 trials; inputs device-resident" +
+                     ("; mechanisms alternated trial by trial" if len(mechs) > 1 else ""),
+           "mechanism": mechs,
            "device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(0),
            "scipy_arm": "scipy.sparse.csgraph.dijkstra per map on one host core, float64, distances only (graph "
                         "construction included in ms_per_map); a point of comparison, not an oracle"}
@@ -141,18 +170,28 @@ def main():
         gi = torch.from_numpy(np.asarray(goal_np, np.int32)).to(dev)
         sm = torch.zeros_like(cost).view(B, -1).scatter_(1, si.long()[:, None], 1.0).view_as(cost)
         gm = torch.zeros_like(cost).view(B, -1).scatter_(1, gi.long()[:, None], 1.0).view_as(cost)
-        k_ms, k_trials = timed(lambda: _native.weighted_labels(cost, gi, pas, si))
-        kl_ms, _ = timed(lambda: _native.weighted_labels(cost, gi, pas))
-        a_ms, _ = timed(lambda: compute_weighted_opt_labels(cost, gm, passable=pas))
-        p_ms, _ = timed(lambda: shortest_path_maps(cost, sm, gm, passable=pas))
-        r = _native.weighted_labels(cost, gi, pas, si)
-        hops, status = r[1].view(B, -1), r[6]
-        out[name] = {"maps": B, "grid": f"{H}x{W}", "kernel_ms": k_ms, "kernel_ms_trials": k_trials,
-                     "maps_per_s": B / (k_ms * 1e-3), "kernel_without_paths_ms": kl_ms,
-                     "compute_weighted_opt_labels_ms": a_ms, "shortest_path_maps_ms": p_ms,
-                     "shortest_path_maps_maps_per_s": B / (p_ms * 1e-3),
-                     "start_unreachable_maps": int(((status & 4) != 0).sum()), "max_hops": int(hops.max()),
-                     "scipy": scipy_arm(cost_np[:, 0], pas_np[:, 0], goal_np, args.scipy_maps)}
+        k = timed_alternating([lambda m=m: _native.weighted_labels(cost, gi, pas, si, m) for m in mechs])
+        kl = timed_alternating([lambda m=m: _native.weighted_labels(cost, gi, pas, mechanism=m) for m in mechs])
+        a = timed_alternating([lambda m=m: compute_weighted_opt_labels(cost, gm, passable=pas, mechanism=m)
+                               for m in mechs])
+        p = timed_alternating([lambda m=m: shortest_path_maps(cost, sm, gm, passable=pas, mechanism=m)
+                               for m in mechs])
+        rows = {}
+        for i, m in enumerate(mechs):
+            (k_ms, k_trials), (kl_ms, _), (a_ms, _), (p_ms, _) = k[i], kl[i], a[i], p[i]
+            r = _native.weighted_labels(cost, gi, pas, si, m)
+            hops, status, pcost = r[1].view(B, -1), r[6], r[5]
+            reached = (status & 4) == 0
+            rows[m] = {"kernel_ms": k_ms, "kernel_ms_trials": k_trials, "maps_per_s": B / (k_ms * 1e-3),
+                       "kernel_without_paths_ms": kl_ms, "compute_weighted_opt_labels_ms": a_ms,
+                       "shortest_path_maps_ms": p_ms, "shortest_path_maps_maps_per_s": B / (p_ms * 1e-3),
+                       "start_unreachable_maps": int((~reached).sum()), "max_hops": int(hops.max()),
+                       "mean_path_cells": float((hops.gather(1, si.long()[:, None])[:, 0][reached] + 1).double()
+                                                .mean()),
+                       "mean_path_cost": float(pcost[reached].double().mean()),
+                       "scipy": scipy_arm(cost_np[:, 0], pas_np[:, 0], goal_np, args.scipy_maps,
+                                          _MOVES[:NUM_MOVES[m]])}
+        out[name] = {"maps": B, "grid": f"{H}x{W}", **rows[mechs[0]], **{m: rows[m] for m in mechs[1:]}}
     line = json.dumps(out)
     print(line)
     if args.out:
