@@ -233,6 +233,7 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
         // backward running sums (replicated in every lane): S = sum of v over the open set, D = <Gh, v>,
         // A / B = prefix sums of 1/S and D/S^2 over the steps executed so far
         double Ssum = 0.0, Slo = 0.0, Dsum = 0.0, Dlo = 0.0, Acum = 0.0, Bcum = 0.0;   // (Ssum,Slo), (Dsum,Dlo): double-double
+        double Smax = 0.0;   // largest S since the last resum (bwd_track)
         auto gh_at = [&](int i) -> float { return (blocked && i == goal_idx) ? 0.f : __ldg(gG + i); };
         if (start_idx >= 0 && lane == 0) {
             const int sy = start_idx / W, sx = start_idx - sy * W;
@@ -266,6 +267,7 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
             if (m == kKeyInf) { t_solve = NASTAR_TS_EXHAUSTED; break; }
             double A1 = 0.0, B1 = 0.0;   // prefix sums INCLUDING step t (events of step t take effect from t+1 on)
             if (kBwd) {
+                bwd_track(lane, N, [&](int i) { return V[i]; }, gh_at, Ssum, Slo, Dsum, Dlo, Smax);
                 const double inv = 1.0 / (Ssum + Slo);
                 const double a_t = inv, b_t = (Dsum + Dlo) * inv * inv;
                 const bool last = stationary_ok && (ts_in >= 0) && (t == ts_in + 1);

@@ -203,6 +203,7 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
     S.open_row[lane + 32] = open[1];
     // backward state: running sums replicated in every lane
     double Ssum = 0.0, Slo = 0.0, Dsum = 0.0, Dlo = 0.0, Acum = 0.0, Bcum = 0.0;   // (Ssum,Slo), (Dsum,Dlo): double-double
+    double Smax = 0.0;   // largest S since the last resum (bwd_track)
     int Tb = 0, ts_in = NASTAR_TS_CAPPED;
     if (kBwd) {
         Tb = *a.T_batch;
@@ -243,6 +244,8 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
         if (m == kKeyInf) { t_solve = NASTAR_TS_EXHAUSTED; break; }
         double A1 = 0.0, B1 = 0.0;   // prefix sums INCLUDING step t (the events of step t act from t+1 on)
         if (kBwd) {
+            bwd_track(lane, kCells64, [&](int i) { return Bw.v[i]; }, [&](int i) { return Bw.gh[i]; }, Ssum, Slo, Dsum,
+                      Dlo, Smax);
             const double inv = 1.0 / (Ssum + Slo);
             const double a_t = inv, b_t = (Dsum + Dlo) * inv * inv;
             if (stationary_ok && (ts_in >= 0) && (t == ts_in + 1)) {

@@ -17,6 +17,14 @@ IndexError).  Files, under tests/golden/news/ (all square: the generator's heuri
   news_mazes032_lowg      16 of them at g_ratio = 0.2 (batch-coupled) with learned costs and a gradient
   news_all064_vanilla     40 all_064 test maps, 64x64, VanillaAstar: engine 4
   news_large128_learned   2 random 128x128 maps with random learned costs: engine 2
+  news_all064_learned     8 more all_064 test maps with random learned costs (eval), then one training-mode batch
+                          (Tmax 0.25) with the autograd gradient of sum(histories * rand_G): engine 4
+  news_all064_lowg        4 of them at g_ratio = 0.3 (batch-coupled) with a gradient
+  news_large144_learned   2 random 144x144 maps with random learned costs: engine 3
+  news_mazes032_gr08      mazes_032 test maps 84..99, new starts and random learned costs, g_ratio = 0.8, with a
+                          gradient: engine 1
+
+    python tests/golden/make_golden_news.py --more   # only the last four
 """
 import importlib.util
 import os
@@ -156,7 +164,66 @@ def main():
     res = run_news(cost, starts, goals, maps)
     mg.save("news_large128_learned", dict(desc="2 random 128x128 maps, random costs, NEWS", g_ratio=0.5,
                                           mechanism="news"), **mg.common_arrays(maps, starts, goals, res, cost=cost))
+    more()
+
+
+def more():
+    """Learned costs above 32x32, a batch-coupled 64x64 batch, a generic-engine workspace map and g_ratio 0.8.  Host
+    memory: the reference keeps ~10 [B,H,W] fp32 tensors per step of a differentiated loop, so B x steps is kept to
+    about 1 GB (all064 training: 8 maps x 1024 steps) to 3 GB (all064 lowg: 4 maps x at most 4096 steps)."""
+    # --- all_064 maps 40..47 with random learned costs: eval, then a training batch with a gradient ------------------
+    maps, goals = load_split("all_064_moore_c16.npz", 48)
+    maps, goals = maps[40:], goals[40:]
+    starts = news_starts(maps.numpy(), mg.onehot_idx(goals), 4)
+    rng = np.random.RandomState(21)
+    cost = torch.from_numpy(rng.rand(8, 1, 64, 64).astype(np.float32))
+    res = run_news(cost, starts, goals, maps)
+    arrays = mg.common_arrays(maps, starts, goals, res, cost=cost)
+    rand_G = torch.from_numpy(rng.randn(8, 1, 64, 64).astype(np.float32))
+    tr = run_news(cost, starts, goals, maps, Tmax=0.25, training=True, grad_hist=rand_G)
+    arrays.update(train_hist_bits=mg.pack(tr["hist"][:, 0]), train_path_bits=mg.pack(tr["paths"][:, 0]),
+                  train_T_batch=np.int32(tr["T_batch"]), train_trace=tr["trace"].numpy(),
+                  rand_G=rand_G[:, 0].numpy(), train_grad_cost=tr["grad_cost"][:, 0].numpy())
+    mg.save("news_all064_learned", dict(desc="8 all_064 test maps, random costs, NEWS; train Tmax 0.25 + grad",
+                                        g_ratio=0.5, Tmax_train=0.25, mechanism="news"), **arrays)
+
+    # --- 4 of them at g_ratio 0.3: batch-coupled, eval length, with a gradient --------------------------------------
+    sl = slice(0, 4)
+    res = run_news(cost[sl], starts[sl], goals[sl], maps[sl], g_ratio=0.3, grad_hist=rand_G[sl])
+    arrays = mg.common_arrays(maps[sl], starts[sl], goals[sl], res, cost=cost[sl])
+    arrays.update(rand_G=rand_G[sl, 0].numpy(), rand_grad_cost=res["grad_cost"][:, 0].numpy())
+    mg.save("news_all064_lowg", dict(desc="4 all_064 test maps, random costs, NEWS, g_ratio 0.3 + grad", g_ratio=0.3,
+                                     mechanism="news"), **arrays)
+
+    # --- 144x144: the generic engine's HBM workspace -----------------------------------------------------------------
+    rng = np.random.RandomState(12)
+    maps = torch.from_numpy((rng.rand(2, 1, 144, 144) > 0.25).astype(np.float32))
+    goals = torch.zeros_like(maps)
+    goals[0, 0, 130, 20] = goals[1, 0, 71, 140] = 1
+    maps[goals > 0] = 1
+    starts = news_starts(maps.numpy(), mg.onehot_idx(goals), 5)
+    cost = torch.from_numpy(rng.rand(2, 1, 144, 144).astype(np.float32))
+    with torch.no_grad():
+        res = run_news(cost, starts, goals, maps)
+    mg.save("news_large144_learned", dict(desc="2 random 144x144 maps, random costs, NEWS", g_ratio=0.5,
+                                          mechanism="news"), **mg.common_arrays(maps, starts, goals, res, cost=cost))
+
+    # --- mazes_032 at g_ratio 0.8, random costs, eval with a gradient ------------------------------------------------
+    maps, goals = load_split("mazes_032_moore_c8.npz", 100)
+    maps, goals = maps[84:], goals[84:]
+    starts = news_starts(maps.numpy(), mg.onehot_idx(goals), 6)
+    rng = np.random.RandomState(23)
+    cost = torch.from_numpy(rng.rand(16, 1, 32, 32).astype(np.float32))
+    rand_G = torch.from_numpy(rng.randn(16, 1, 32, 32).astype(np.float32))
+    res = run_news(cost, starts, goals, maps, g_ratio=0.8, grad_hist=rand_G)
+    arrays = mg.common_arrays(maps, starts, goals, res, cost=cost)
+    arrays.update(rand_G=rand_G[:, 0].numpy(), rand_grad_cost=res["grad_cost"][:, 0].numpy())
+    mg.save("news_mazes032_gr08", dict(desc="16 mazes_032 test maps, random costs, NEWS, g_ratio 0.8 + grad",
+                                       g_ratio=0.8, mechanism="news"), **arrays)
 
 
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["--more"]:   # only the files added after the first five
+        more()
+    else:
+        main()

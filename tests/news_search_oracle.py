@@ -190,15 +190,16 @@ def _literal(c, goalmap, o, si, gi, B, H, W, g_ratio, T, want_trace) -> Output:
     return Output(hist.reshape(B, 1, H, W), paths.reshape(B, 1, H, W), ts, np.full(B, tb, np.int32), tb, trace)
 
 
-def backward(cost, start, goal, obst, grad_hist, T_batch: int, g_ratio=0.5) -> np.ndarray:
-    """dL/dcost [B,1,H,W] float32 for dL/dhistories = grad_hist, replaying spec for T_batch steps per map:
+def backward(cost, start, goal, obst, grad_hist, T_batch: int, g_ratio=0.5, dtype=F32) -> np.ndarray:
+    """dL/dcost [B,1,H,W] (float32, or `dtype`: float64 keeps the fp64 sums unrounded) for dL/dhistories = grad_hist,
+    replaying spec for T_batch steps per map:
     sum_t -(1-g_ratio)/sqrt(W) * y_t * (G - <G, y_t>), y_t the softmax of -f/sqrt(W) over the open set, with G zeroed at
     the goal when the goal is selected twice (clamp(hist + sel) blocks it there)."""
     c, H, W = _planes(cost)
     s, g, o, G = _planes(start)[0], _planes(goal)[0], _planes(obst)[0], _planes(grad_hist)[0].astype(np.float64)
     B, N = c.shape
     gr, omg, sqw = _scalars(g_ratio, W)
-    out = np.zeros((B, N), F32)
+    out = np.zeros((B, N), dtype)
     for b in range(B):
         gi = int(g[b].argmax())
         m = _Spec(c[b], o[b], H, W, int(s[b].argmax()), gi)
