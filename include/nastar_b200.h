@@ -44,8 +44,10 @@ enum {
 #define NASTAR_FWD_NO_EARLY_EXIT 1 /* run exactly T steps per map: a solved map keeps stepping (re-selecting its
                                       goal, or other nodes when g_ratio < 0.5) like the reference's batch-synchronous
                                       loop does until the slowest map is solved (differentiable_astar.py:251-252).
-                                      Per-map early exit is exact for g_ratio >= 0.5 (SURVEY App. A.4); the host
-                                      side uses this flag to reproduce the batch coupling for g_ratio < 0.5 */
+                                      Per-map early exit is exact for g_ratio >= 0.5 (SURVEY App. A.4).  For
+                                      g_ratio < 0.5 the batch coupling is either decided on the host from a
+                                      NO_EARLY_EXIT trace (a full-length search, then a second one of T_batch steps)
+                                      or on the device by nastar_b200_forward_coupled() */
 #define NASTAR_FWD_PAIR 2          /* validation pair in ONE launch (utils/training.py:63-87 runs the learned-cost
                                       search and VanillaAstar on the same batch): maps 0..B-1 are searched on
                                       `cost` (any cost_kind), maps B..2B-1 are the same problems searched with
@@ -128,7 +130,8 @@ typedef struct nastar_bwd_params {
                                  then selected again and clamp(hist+sel) saw 2, differentiable_astar.py:222-223).
                                  For g_ratio < 0.5 a solved map need not re-select its goal: pass 0 for maps
                                  whose goal is selected at least twice within T_batch steps and T_batch otherwise
-                                 (the Python module derives this from a NO_EARLY_EXIT trace) */
+                                 (the Python module derives this from a NO_EARLY_EXIT trace, or takes the goal_clamp
+                                 of nastar_b200_forward_coupled) */
     const float *grad_histories; int64_t grad_stride; /* dL/d histories, [B][H*W] */
     float *grad_cost;                                  /* dL/d cost_maps, [B][H*W], overwritten */
     void  *workspace;
@@ -157,6 +160,27 @@ int nastar_b200_backward(const nastar_bwd_params *p, void *stream);
  * forward that ran with NASTAR_FWD_NEWS (the replay then expands 4-connected with the Manhattan heuristic; the
  * closed form itself does not depend on the stencil).  Any other mechanism is NASTAR_EINVAL, before any launch. */
 int nastar_b200_backward_mech(const nastar_bwd_params *p, int32_t mechanism, void *stream);
+
+/* Batch-coupled forward for g_ratio < 0.5 (differentiable_astar.py:203-252) with T_batch decided on the device: the
+ * reference steps every map until one step has every map selecting its goal, so a map solved early keeps evolving
+ * (it need not re-select its goal when g_ratio < 0.5, SURVEY App. A.4).  Writes the outputs of exactly
+ *   T_batch = 1 + min{k < T : every map selects its goal at step k}   (T if there is no such k)
+ * steps per map, bit-equal to nastar_b200_forward with p->T = T_batch and NASTAR_FWD_NO_EARLY_EXIT (histories, paths,
+ * t_solve, n_steps, n_closed, path_len), plus
+ *   T_batch[0]     (device int32) that step count, ready for nastar_bwd_params.T_batch;
+ *   goal_clamp[b]  (device int32) 0 if map b selects its goal at least twice within T_batch steps, else T_batch: the
+ *                  nastar_bwd_params.t_solve encoding of the goal clamp for this case.
+ * Three launches on `stream`, no host round trip (CUDA-graph capturable): pass 1 searches without the solve-step exit
+ * and stops a map at its fixed point (its goal, already closed, is selected again and nothing is opened or relaxed: every
+ * later step repeats that one), when its open set is exhausted, or at T, recording the at-goal bit of every step; a
+ * one-CTA reduction computes T_batch and goal_clamp from those bits; pass 2 re-runs, for exactly T_batch steps, only the
+ * maps pass 1 stopped later than T_batch.
+ * p->T is the cap; p->flags may hold only NASTAR_FWD_NEWS (NO_EARLY_EXIT or PAIR: NASTAR_EINVAL); p->trace must be
+ * NULL; any cost_kind (LOGIT / TAPS on engines 1 and 4).  p->workspace must hold
+ * nastar_b200_forward_coupled_workspace_bytes(B, H, W, T) bytes, else NASTAR_EWORKSPACE.  Every check precedes the
+ * first launch.  Engines 1, 4, 2 and 3; engine 5 is not used. */
+size_t nastar_b200_forward_coupled_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t T);
+int nastar_b200_forward_coupled(const nastar_fwd_params *p, int32_t *T_batch, int32_t *goal_clamp, void *stream);
 
 /* T_batch[0] = min(T, 1 + max_b n_steps-style stop) computed on the device from the forward's
  * t_solve/n_steps arrays (replaces the host-synchronising torch.all(...) of :251). */

@@ -176,6 +176,81 @@ __global__ void batch_steps_kernel(const int32_t* __restrict__ t_solve, const in
     }
 }
 
+// ---- batch-coupled forward (nastar_b200_forward_coupled) ------------------------------------------------
+inline size_t round256(size_t n) { return (n + 255) & ~size_t(255); }
+
+// head of the coupled forward's workspace: stop / end / first [B] int32 each, then the at-goal bitmaps [B][ceil(T/32)];
+// the generic engine's slots (engine 3) follow
+size_t coupled_aux_bytes(int32_t B, int32_t T) {
+    const size_t words = (size_t(T) + 31) / 32;
+    return 3 * round256(size_t(B) * 4) + round256(size_t(B) * words * 4);
+}
+
+nastar::CoupledWs coupled_ws(void* workspace, int32_t B, int32_t T) {
+    unsigned char* w = static_cast<unsigned char*>(workspace);
+    const size_t per_map = round256(size_t(B) * 4);
+    nastar::CoupledWs cw;
+    cw.stop = reinterpret_cast<int32_t*>(w);
+    cw.end = reinterpret_cast<int32_t*>(w + per_map);
+    cw.first = reinterpret_cast<int32_t*>(w + 2 * per_map);
+    cw.bits = reinterpret_cast<uint32_t*>(w + 3 * per_map);
+    cw.words = (T + 31) / 32;
+    return cw;
+}
+
+constexpr int kCoupledThreads = 512;
+
+template <class Op>
+__device__ int block_reduce(int v, Op op, int* red) {
+    for (int o = 16; o; o >>= 1) v = op(v, __shfl_xor_sync(0xFFFFFFFFu, v, o));
+    __syncthreads();   // red[] may still be read by the previous reduction
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    v = red[0];
+    for (int i = 1; i < int(blockDim.x >> 5); ++i) v = op(v, red[i]);
+    return v;
+}
+
+// T_batch = 1 + min{k < T : every map selects its goal at step k}, or T (differentiable_astar.py:251-252), from the
+// at-goal bitmaps of pass 1; then goal_clamp[b] = 0 if map b selects its goal at least twice within T_batch steps,
+// else T_batch (the t_solve encoding of nastar_bwd_params).  Integer AND / min / popcount only: deterministic.
+__global__ void __launch_bounds__(kCoupledThreads) coupled_reduce_kernel(const nastar::CoupledWs cw, int B, int T,
+                                                                         int32_t* __restrict__ T_batch,
+                                                                         int32_t* __restrict__ goal_clamp) {
+    __shared__ int red[kCoupledThreads / 32];
+    auto imax = [](int x, int y) { return max(x, y); };
+    auto iand = [](int x, int y) { return x & y; };
+    // no step before the last map's first goal selection can have every map at its goal; a map that never selects
+    // its goal keeps T_batch at T
+    int lo = 0;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        const int f = cw.first[b];
+        lo = max(lo, f < 0 ? T : f);
+    }
+    lo = block_reduce(lo, imax, red);
+    int Tb = T;
+    for (int w = lo >> 5; w < cw.words; ++w) {
+        uint32_t all = 0xFFFFFFFFu;
+        for (int b = threadIdx.x; b < B; b += blockDim.x) all &= nastar::coupled_word(cw, b, w);
+        all = uint32_t(block_reduce(int(all), iand, red));
+        if (w == cw.words - 1 && (T & 31)) all &= (1u << (T & 31)) - 1u;
+        if (all) { Tb = (w << 5) + __ffs(all); break; }   // block-uniform
+    }
+    if (threadIdx.x == 0) T_batch[0] = Tb;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        const int f = cw.first[b];
+        int n = 0;
+        if (f >= 0) {
+            for (int w = f >> 5; (w << 5) < Tb && n < 2; ++w) {
+                uint32_t v = nastar::coupled_word(cw, b, w);
+                if (Tb - (w << 5) < 32) v &= (1u << (Tb - (w << 5))) - 1u;
+                n += __popc(v);
+            }
+        }
+        goal_clamp[b] = (n >= 2) ? 0 : Tb;
+    }
+}
+
 template <int C>
 void launch_head(const float* x, int64_t P, const float* w_host, float* taps, cudaStream_t stream) {
     nastar::HeadWeights<C> hw;
@@ -320,6 +395,89 @@ int nastar_b200_forward(const nastar_fwd_params* p, void* stream_v) {
     }, global, trace, noexit, news);
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();
+}
+
+size_t nastar_b200_forward_coupled_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t T) {
+    if (B <= 0 || T < 1) return 0;
+    const int engine = nastar_b200_engine_for(H, W);
+    if (engine == 0) return 0;
+    const size_t slots = (engine == 3) ? size_t(generic_slots(B)) * nastar::GenericLayout(H, W).slot_bytes() : 0;
+    return coupled_aux_bytes(B, T) + slots;
+}
+
+int nastar_b200_forward_coupled(const nastar_fwd_params* p, int32_t* T_batch, int32_t* goal_clamp, void* stream_v) {
+    if (!p || !T_batch || !goal_clamp || !p->cost || !p->start || !p->goal || !p->obst || !p->histories || !p->paths)
+        return NASTAR_EINVAL;
+    if (p->B <= 0 || p->H <= 0 || p->W <= 0 || p->T < 1) return NASTAR_EINVAL;
+    if (p->cost_kind < NASTAR_COST_PLANE || p->cost_kind > NASTAR_COST_TAPS) return NASTAR_EINVAL;
+    if ((p->flags & ~NASTAR_FWD_NEWS) != 0 || p->trace) return NASTAR_EINVAL;
+    const int engine = nastar_b200_engine_for(p->H, p->W);
+    if (engine == 0) return NASTAR_EUNSUPPORTED;
+    if (p->cost_kind != NASTAR_COST_PLANE && engine != 1 && engine != 4) return NASTAR_EUNSUPPORTED;
+    const size_t need = nastar_b200_forward_coupled_workspace_bytes(p->B, p->H, p->W, p->T);
+    if (!p->workspace || p->workspace_bytes < need) return NASTAR_EWORKSPACE;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+    const bool fused = p->cost_kind != NASTAR_COST_PLANE;
+    const bool news = (p->flags & NASTAR_FWD_NEWS) != 0;
+    const nastar::CoupledWs cw = coupled_ws(p->workspace, p->B, p->T);
+    // pass 1 (kExitCoupled1), the reduction, pass 2 (kExitCoupled2): three launches, no host round trip
+    auto both_passes = [&](auto launch_pass) -> int {
+        cudaError_t e = launch_pass(std::integral_constant<int, nastar::kExitCoupled1>{});
+        if (e != cudaSuccess) return cuda_fail(e);
+        int st = launched();
+        if (st != NASTAR_OK) return st;
+        coupled_reduce_kernel<<<1, kCoupledThreads, 0, stream>>>(cw, p->B, p->T, T_batch, goal_clamp);
+        st = launched();
+        if (st != NASTAR_OK) return st;
+        e = launch_pass(std::integral_constant<int, nastar::kExitCoupled2>{});
+        if (e != cudaSuccess) return cuda_fail(e);
+        return launched();
+    };
+    if (engine == 1) {
+        const cudaError_t e = news ? ensure_heur<32, true>(stream) : ensure_heur<32>(stream);
+        if (e != cudaSuccess) return cuda_fail(e);
+        nastar::W32Args a{};
+        a.f = *p;
+        a.T_batch = T_batch;
+        a.cw = cw;
+        return both_passes([&](auto kExit) {
+            with_flags([&](auto kFused, auto kNews) {
+                nastar::astar_warp32_kernel<false, false, kExit, kFused, kNews><<<p->B, 32, 0, stream>>>(a);
+            }, fused, news);
+            return cudaSuccess;
+        });
+    }
+    if (engine == 4) {
+        const cudaError_t e = news ? ensure_heur<64, true>(stream) : ensure_heur<64>(stream);
+        if (e != cudaSuccess) return cuda_fail(e);
+        nastar::W64Args wa{};
+        wa.f = *p;
+        wa.T_batch = T_batch;
+        wa.cw = cw;
+        return both_passes([&](auto kExit) {
+            return with_flags([&](auto kFused, auto kNews) {
+                return launch_smem(nastar::astar_warp64_kernel<false, kExit, false, kFused, kNews>, p->B, 32,
+                                   sizeof(nastar::W64Smem), stream, wa);
+            }, fused, news);
+        });
+    }
+    const nastar::GenericLayout L(p->H, p->W);
+    const bool global = (engine == 3);
+    const size_t smem = L.smem_common() + (global ? 0 : L.smem_planes());
+    const int grid = global ? generic_slots(p->B) : p->B;
+    const size_t aux = coupled_aux_bytes(p->B, p->T);
+    nastar::GenArgs ga{};
+    ga.f = *p;
+    ga.f.workspace = static_cast<unsigned char*>(p->workspace) + aux;   // engine 3's slots follow the records
+    ga.f.workspace_bytes = p->workspace_bytes - aux;
+    ga.T_batch = T_batch;
+    ga.cw = cw;
+    return both_passes([&](auto kExit) {
+        return with_flags([&](auto kGlobal, auto kNews) {
+            return launch_smem(nastar::astar_generic_kernel<kGlobal, false, false, kExit, kNews>, grid, 32, smem,
+                               stream, ga);
+        }, global, news);
+    });
 }
 
 int nastar_b200_backward(const nastar_bwd_params* p, void* stream_v) {

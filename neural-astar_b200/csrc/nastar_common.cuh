@@ -12,6 +12,51 @@ namespace nastar {
 constexpr unsigned kFull = 0xFFFFFFFFu;
 constexpr uint32_t kKeyInf = 0xFFFFFFFFu;  // "no open cell" sentinel, above every float key
 
+// Exit mode of a forward search kernel (template parameter kExit):
+//   kExitEarly    the map stops at its solve step (per-map early exit, differentiable_astar.py:251-252);
+//   kExitNone     NASTAR_FWD_NO_EARLY_EXIT: exactly T steps per map;
+//   kExitCoupled1 pass 1 of nastar_b200_forward_coupled: no solve-step exit, but the map stops at its fixed point
+//                 (the goal is re-selected and the step changes nothing), and every executed step's at-goal bit
+//                 goes to a per-map bitmap (CoupledWs);
+//   kExitCoupled2 pass 2: maps that pass 1 stopped after more than *T_batch steps run again for exactly *T_batch
+//                 steps; every other map only finishes its counters.
+constexpr int kExitEarly = 0, kExitNone = 1, kExitCoupled1 = 2, kExitCoupled2 = 3;
+
+// how pass 1 of the coupled forward ended for a map (CoupledWs::end)
+constexpr int kEndCapped = 0;      // T steps executed
+constexpr int kEndExhausted = 1;   // the open set ran empty: "at goal" is false from then on
+constexpr int kEndFixed = 2;       // fixed point: the goal is selected at every later step
+
+// per-map records of the coupled forward, in the caller's workspace (nastar_b200_forward_coupled)
+struct CoupledWs {
+    int32_t* stop;    // [B] steps pass 1 executed
+    int32_t* end;     // [B] kEnd*
+    int32_t* first;   // [B] first step that selected the goal, or NASTAR_TS_* (pass 1's t_solve)
+    uint32_t* bits;   // [B][words] bit t of word t/32: step t selected the goal; only bits < stop[b] are valid
+    int32_t words;    // ceil(T / 32)
+};
+
+// the at-goal bits of map b for steps 32w .. 32w+31: the recorded bits below stop, the constant tail above
+__device__ __forceinline__ uint32_t coupled_word(const CoupledWs& cw, int b, int w) {
+    const int stop = cw.stop[b];
+    const uint32_t tail = (cw.end[b] == kEndFixed) ? 0xFFFFFFFFu : 0u;
+    const int lo = w << 5;
+    if (lo >= stop) return tail;
+    const uint32_t v = cw.bits[int64_t(b) * cw.words + w];
+    if (stop - lo >= 32) return v;
+    const uint32_t m = (1u << (stop - lo)) - 1u;
+    return (v & m) | (tail & ~m);
+}
+
+// pass 2 for a map that pass 1 already finished (stop <= T_batch): its masks stand; the counters become those of a
+// NO_EARLY_EXIT search of T_batch steps.  A map at its fixed point executes all of them; a map whose open set ran
+// empty exactly at step T_batch reaches the cap before it can notice.
+__device__ __forceinline__ void coupled_keep(const CoupledWs& cw, int b, int Tb, int32_t* t_solve, int32_t* n_steps) {
+    const int end = cw.end[b];
+    if (end == kEndFixed && n_steps) n_steps[b] = Tb;
+    if (end == kEndExhausted && cw.stop[b] == Tb && t_solve) t_solve[b] = -1;   // NASTAR_TS_CAPPED
+}
+
 // Order-preserving map float -> uint32 (a < b  <=>  key(a) < key(b) for non-NaN a, b).
 __device__ __forceinline__ uint32_t fkey(float f) {
     uint32_t b = __float_as_uint(f);

@@ -51,6 +51,7 @@ struct GenArgs {
     // forward only, nullable: per-map flags written by the bin16 engine (nastar_bin16.cuh); when given, only
     // maps with redo[b] != 0 are processed here (the others were already finished on-chip)
     const int32_t* redo;
+    CoupledWs cw;   // coupled forward only (see W32Args)
 };
 
 // kBwd = true replays the search for *T_batch steps and accumulates the closed-form gradient (SURVEY App. B)
@@ -60,12 +61,13 @@ struct GenArgs {
 // prefix sums A(t) = sum_{tau<t} 1/S_tau, B(t) = sum_{tau<t} D_tau/S_tau^2, D_t = <Gh, v_t>.  S and D are
 // maintained incrementally in fp64 from the <= 9 events of a step — O(1) work per step instead of a dense
 // O(N/32) softmax pass (round 1).  Per-cell state (v, A(t0), B(t0), acc) lives in the per-CTA workspace slot.
-// kNoExit (forward only): NASTAR_FWD_NO_EARLY_EXIT — keep stepping after the solve step, exactly T steps.
+// kExit (forward only): kExitEarly, kExitNone (NASTAR_FWD_NO_EARLY_EXIT — keep stepping after the solve step, exactly
+// T steps) or a pass of the coupled forward, kExitCoupled1 / kExitCoupled2 (nastar_common.cuh).
 // kNews: NASTAR_FWD_NEWS / NASTAR_MECH_NEWS — only lanes 1, 3, 5, 7 (N, W, E, S) take a neighbour, and h is the
 // Manhattan heuristic.
-template <bool kGlobal, bool kTrace, bool kBwd, bool kNoExit = false, bool kNews = false>
+template <bool kGlobal, bool kTrace, bool kBwd, int kExit = kExitEarly, bool kNews = false>
 __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
-    constexpr bool kContinue = kBwd || kNoExit;
+    constexpr bool kContinue = kBwd || (kExit != kExitEarly);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const nastar_fwd_params& p = a.f;
     const int lane = threadIdx.x;
@@ -111,8 +113,8 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
     uint64_t* bar = reinterpret_cast<uint64_t*>((reinterpret_cast<uintptr_t>(sp) + 7) & ~uintptr_t(7));
 
     const float gr = p.g_ratio, omg = p.one_minus_g_ratio;
-    const int Tb = kBwd ? *a.T_batch : 0;
-    const int T = kBwd ? Tb : p.T;
+    const int Tb = (kBwd || (kExit == kExitCoupled2)) ? *a.T_batch : 0;
+    const int T = (kBwd || (kExit == kExitCoupled2)) ? Tb : p.T;
     const bool stationary_ok = (gr >= 0.5f);
     uint32_t bar_parity = 0;
     if (!kGlobal) {
@@ -122,6 +124,12 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
 
     for (int b = blockIdx.x; b < p.B; b += gridDim.x) {
         if (!kBwd && a.redo != nullptr && a.redo[b] == 0) continue;
+        if constexpr (kExit == kExitCoupled2) {
+            if (a.cw.stop[b] <= Tb) {   // pass 1's outputs stand
+                if (lane == 0) coupled_keep(a.cw, b, Tb, p.t_solve, p.n_steps);
+                continue;
+            }
+        }
         const float* gCost = p.cost + int64_t(b) * p.cost_stride;
         const float* gStart = p.start + int64_t(b) * p.start_stride;
         const float* gGoal = p.goal + int64_t(b) * p.goal_stride;
@@ -262,9 +270,11 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
         int t_solve = NASTAR_TS_CAPPED;
         int steps = 0;
         int32_t* trace = kTrace ? (p.trace + int64_t(b) * T) : nullptr;
+        uint32_t gbits = 0u;          // pass 1: at-goal bits of the current 32-step word
+        int end = kEndCapped;         // pass 1: how the loop ended
         for (int t = 0; t < T; ++t) {
             const uint32_t m = __reduce_min_sync(kFull, bk);
-            if (m == kKeyInf) { t_solve = NASTAR_TS_EXHAUSTED; break; }
+            if (m == kKeyInf) { t_solve = NASTAR_TS_EXHAUSTED; end = kEndExhausted; break; }
             double A1 = 0.0, B1 = 0.0;   // prefix sums INCLUDING step t (events of step t take effect from t+1 on)
             if (kBwd) {
                 bwd_track(lane, N, [&](int i) { return V[i]; }, gh_at, Ssum, Slo, Dsum, Dlo, Smax);
@@ -287,6 +297,13 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
             steps = t + 1;
             if (kTrace && lane == 0) trace[t] = ind;
             const bool solved = (ind == goal_idx);
+            if constexpr (kExit == kExitCoupled1) {
+                gbits |= uint32_t(solved) << (t & 31);
+                if ((t & 31) == 31) {
+                    if (lane == 0) a.cw.bits[int64_t(b) * a.cw.words + (t >> 5)] = gbits;
+                    gbits = 0u;
+                }
+            }
             if (lane == 0) {
                 sClosed[r * Wd + (c >> 5)] |= 1u << (c & 31);
                 if (!solved) sOpen[r * Wd + (c >> 5)] &= ~(1u << (c & 31));
@@ -367,6 +384,11 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
             }
             if (solved && t_solve < 0) t_solve = t;
             if (!kContinue && solved) break;
+            if constexpr (kExit == kExitCoupled1) {
+                // fixed point: the goal, closed at an earlier step, is selected again and no lane opens or relaxes a
+                // neighbour (see the 32-wide engine)
+                if (solved && t_solve < t && !__any_sync(kFull, upd)) { end = kEndFixed; break; }
+            }
             // per-row minimum of the freshly written keys: lanes {0,1,2} {3,4,5} {6,7,8}
             const uint32_t k1 = __shfl_down_sync(kFull, key, 1), k2 = __shfl_down_sync(kFull, key, 2);
             const int x1 = __shfl_down_sync(kFull, x, 1), x2 = __shfl_down_sync(kFull, x, 2);
@@ -398,6 +420,12 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
             }
         }
         __syncwarp();
+        if constexpr (kExit == kExitCoupled1) if (lane == 0) {
+            if (steps & 31) a.cw.bits[int64_t(b) * a.cw.words + (steps >> 5)] = gbits;   // the last, partial word
+            a.cw.stop[b] = steps;
+            a.cw.end[b] = end;
+            a.cw.first[b] = t_solve;
+        }
 
         if (kBwd) {
             // close the intervals of the cells still open at the end, then scale

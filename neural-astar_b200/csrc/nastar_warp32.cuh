@@ -36,6 +36,8 @@ struct W32Args {
     const float* grad_hist;
     int64_t grad_stride;
     float* grad_cost;
+    // coupled forward only (kExitCoupled1 / kExitCoupled2; pass 2 also reads *T_batch)
+    CoupledWs cw;
 };
 
 constexpr int kCells = 1024;  // padded 32 x 32
@@ -74,13 +76,14 @@ struct __align__(16) W32Smem {
     unsigned long long bar;    // mbarrier for the TMA prologue
 };
 
-// kNoExit (forward only): NASTAR_FWD_NO_EARLY_EXIT — keep stepping after the solve step, exactly T steps.
+// kExit (forward only): kExitEarly, kExitNone (NASTAR_FWD_NO_EARLY_EXIT — keep stepping after the solve step, exactly
+// T steps) or a pass of the coupled forward, kExitCoupled1 / kExitCoupled2 (nastar_common.cuh).
 // kFused (forward only): the prologue may have to finish the encoder (NASTAR_COST_LOGIT / NASTAR_COST_TAPS); kept out
 // of the plain instantiation so that its cold instruction footprint stays small.
 // kNews: NASTAR_FWD_NEWS / NASTAR_MECH_NEWS — 4-connected expansion (N, E, W, S) and the Manhattan heuristic.
-template <bool kTrace, bool kBwd, bool kNoExit = false, bool kFused = false, bool kNews = false>
+template <bool kTrace, bool kBwd, int kExit = kExitEarly, bool kFused = false, bool kNews = false>
 __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
-    constexpr bool kContinue = kBwd || kNoExit;   // the loop does not stop at the solve step
+    constexpr bool kContinue = kBwd || (kExit != kExitEarly);   // the loop does not stop at the solve step
     __shared__ W32Smem S;
     extern __shared__ __align__(16) unsigned char bwd_raw[];  // backward only: W32Bwd
     W32Bwd& Bw = *reinterpret_cast<W32Bwd*>(bwd_raw);
@@ -100,6 +103,13 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
     const int cost_kind = (!kFused || kBwd || vanilla_half) ? NASTAR_COST_PLANE : p.cost_kind;
     const bool cost_plane = (cost_kind == NASTAR_COST_PLANE);
     const bool obst_is_cost = cost_plane && (gObst == gCost);
+    if constexpr (kExit == kExitCoupled2) {
+        const int Tc = *a.T_batch;
+        if (a.cw.stop[b] <= Tc) {   // pass 1's outputs stand
+            if (lane == 0) coupled_keep(a.cw, b, Tc, p.t_solve, p.n_steps);
+            return;
+        }
+    }
 
     // ---------------- prologue: stage planes, build row masks ------------------------------
     uint32_t pass = 0u;
@@ -214,6 +224,7 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
         }
         __syncwarp();
     }
+    if constexpr (kExit == kExitCoupled2) Tb = *a.T_batch;   // pass 2 runs T_batch steps
     if (lane == 0) S.par[goal_rc] = 0;  // parents are initialised to the goal (:195-198): a self link at the goal
     if (start_rc >= 0) {
         const float f0 = f_value(gr, omg, 0.f, sGH[start_rc].y);
@@ -235,13 +246,14 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
     }
 
     // ---------------- the search loop (differentiable_astar.py:203-252) --------------------
-    const int T = kBwd ? Tb : p.T;
+    const int T = (kBwd || kExit == kExitCoupled2) ? Tb : p.T;
     // post-solve steps are stationary when g_ratio >= 0.5 (the goal keeps being re-selected and
     // nothing changes, SURVEY App. A.4): the backward then adds them in one go
     const bool stationary_ok = (gr >= 0.5f);
     int t_solve = NASTAR_TS_CAPPED;
     int32_t* trace = kTrace ? (p.trace + int64_t(b) * p.T) : nullptr;
     const float2* ghrow = sGH + (lane << 5);      // this lane's row of {g,h}
+    uint32_t gbits = 0u;          // pass 1: at-goal bits of the current 32-step word
     int t = 0;
     for (; t < T; ++t) {
         // -- select: lexicographic arg-min of (f key, row, col) with two REDUX.MINs -----------
@@ -266,6 +278,13 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
         const int r = int(ind >> 5), c = int(ind & 31u);
         if (kTrace && lane == 0) trace[t] = r * W + c;
         const bool solved = (int(ind) == goal_rc);          // :219-220
+        if constexpr (kExit == kExitCoupled1) {
+            gbits |= uint32_t(solved) << (t & 31);
+            if ((t & 31) == 31) {
+                if (lane == 0) a.cw.bits[int64_t(b) * a.cw.words + (t >> 5)] = gbits;
+                gbits = 0u;
+            }
+        }
         const uint32_t m1 = 1u << c;                        // column masks of the 3-wide window;
         const uint32_t m0 = m1 >> 1, m2 = m1 << 1;          // they fall off the row at c == 0 / 31
         // -- rescan inputs for row r (pre-expansion open cells minus the selected one); stale f
@@ -347,6 +366,11 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
         if ((bk < rm_key) | ((bk == rm_key) & (bc < rm_col))) { rm_key = bk; rm_col = bc; }
         if (solved && t_solve < 0) t_solve = t;             // first step at which the goal was selected
         if (!kContinue && solved) break;                    // :251-252 (per-map early exit, App. A.4)
+        if constexpr (kExit == kExitCoupled1) {
+            // the goal, closed at an earlier step, is selected again and nothing is opened or relaxed: the state after
+            // this step is the state before it, so every later step repeats it (fixed point)
+            if (solved && t_solve < t && !__any_sync(kFull, upd != 0u)) { ++t; break; }
+        }
         if (near) S.open_row[lane] = open;
         // -- fold the rescan into lane r's cached minimum -------------------------------------
         const bool take = isr & ((mr < rm_key) | ((mr == rm_key) & (int(mc) < rm_col)));
@@ -357,6 +381,14 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
     __syncwarp();
     // selection steps executed: t on exhaustion / cap, t+1 when the loop left through the solve step
     const int steps = (!kContinue && t_solve >= 0) ? (t + 1) : t;
+    if constexpr (kExit == kExitCoupled1) if (lane == 0) {
+        if (t & 31) a.cw.bits[int64_t(b) * a.cw.words + (t >> 5)] = gbits;   // the last, partial word
+        a.cw.stop[b] = t;
+        // left before the cap with the goal selected: the fixed point (a fixed point at step T-1 looks capped, which
+        // is the same record: no step past the cap is ever read)
+        a.cw.end[b] = (t_solve == NASTAR_TS_EXHAUSTED) ? kEndExhausted : ((t < T) ? kEndFixed : kEndCapped);
+        a.cw.first[b] = t_solve;
+    }
 
     if (kBwd) {
         // close the intervals of the cells still open; dL/dcost = -(1-g_ratio)/sqrt(W) * acc
@@ -382,7 +414,7 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
         // the start's parent is the goal in the reference (the initial value); the walk stops at the start
         // before following it, which marks the same cells (App. A.3)
         int loc = goal_rc - S.par[goal_rc];
-        const int hops = (t_solve >= 0) ? N : (p.T - 1);
+        const int hops = (t_solve >= 0) ? N : ((kExit == kExitCoupled2 ? T : p.T) - 1);
         for (int k = 0; k < hops; ++k) {
             if (lane == (loc >> 5)) path |= 1u << (loc & 31);
             if (loc == start_rc || loc == goal_rc) break;   // reached the start (or the goal's self link)

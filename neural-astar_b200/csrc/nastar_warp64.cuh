@@ -61,14 +61,16 @@ struct W64Args {
     const float* grad_hist;
     int64_t grad_stride;
     float* grad_cost;
+    CoupledWs cw;   // coupled forward only (see W32Args)
 };
 
 // kFused (forward only): the prologue may have to finish the encoder (NASTAR_COST_LOGIT / NASTAR_COST_TAPS), as in the
 // 32-wide engine; kept out of the plain instantiations.
 // kNews: 4-connected expansion and the Manhattan heuristic, as in the 32-wide engine.
-template <bool kTrace, bool kNoExit, bool kBwd = false, bool kFused = false, bool kNews = false>
+// kExit: exit mode of the forward (kExitEarly, kExitNone, or a pass of the coupled forward), as in the 32-wide engine.
+template <bool kTrace, int kExit, bool kBwd = false, bool kFused = false, bool kNews = false>
 __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
-    constexpr bool kContinue = kBwd || kNoExit;
+    constexpr bool kContinue = kBwd || (kExit != kExitEarly);
     const nastar_fwd_params& p = a.f;
     extern __shared__ __align__(16) unsigned char smem64_raw[];
     W64Smem& S = *reinterpret_cast<W64Smem*>(smem64_raw);
@@ -86,6 +88,13 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
     const int cost_kind = (kFused && !kBwd) ? p.cost_kind : NASTAR_COST_PLANE;
     const bool cost_plane = (cost_kind == NASTAR_COST_PLANE);
     const bool obst_is_cost = cost_plane && (gObst == gCost);
+    if constexpr (kExit == kExitCoupled2) {
+        const int Tc = *a.T_batch;
+        if (a.cw.stop[b] <= Tc) {   // pass 1's outputs stand
+            if (lane == 0) coupled_keep(a.cw, b, Tc, p.t_solve, p.n_steps);
+            return;
+        }
+    }
 
     // ---------------- prologue ----------------------------------------------------------------
     u64 pass[2] = {0ull, 0ull};
@@ -227,13 +236,15 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
             Dsum = double(Bw.gh[start_rc]) * Ssum;
         }
     }
+    if constexpr (kExit == kExitCoupled2) Tb = *a.T_batch;   // pass 2 runs T_batch steps
     __syncwarp();
 
     // ---------------- search loop --------------------------------------------------------------
-    const int T = kBwd ? Tb : p.T;
+    const int T = (kBwd || kExit == kExitCoupled2) ? Tb : p.T;
     const bool stationary_ok = (gr >= 0.5f);   // post-solve steps are stationary (SURVEY App. A.4)
     int t_solve = NASTAR_TS_CAPPED;
     int32_t* trace = kTrace ? (p.trace + int64_t(b) * T) : nullptr;
+    uint32_t gbits = 0u;          // pass 1: at-goal bits of the current 32-step word
     int t = 0;
     for (; t < T; ++t) {
         // local best of the lane's two rows (strict <: the lower row wins ties)
@@ -261,6 +272,13 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
         const int r = int(ind >> 6), c = int(ind & 63u);
         if (kTrace && lane == 0) trace[t] = r * W + c;
         const bool solved = (int(ind) == goal_rc);
+        if constexpr (kExit == kExitCoupled1) {
+            gbits |= uint32_t(solved) << (t & 31);
+            if ((t & 31) == 31) {
+                if (lane == 0) a.cw.bits[int64_t(b) * a.cw.words + (t >> 5)] = gbits;
+                gbits = 0u;
+            }
+        }
         const u64 m1 = 1ull << c, m0 = m1 >> 1, m2 = m1 << 1;
         // rescan inputs: columns lane and lane+32 of row r
         const u64 open_r = (kContinue && solved) ? S.open_row[r] : (S.open_row[r] & ~m1);
@@ -345,6 +363,11 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
         }
         if (solved && t_solve < 0) t_solve = t;
         if (!kContinue && solved) break;
+        if constexpr (kExit == kExitCoupled1) {
+            // fixed point: the goal, closed at an earlier step, is selected again and nothing is opened or relaxed
+            // (see the 32-wide engine)
+            if (solved && t_solve < t && !__any_sync(kFull, upd != 0ull)) { ++t; break; }
+        }
         // fold the rescan into the cached minimum of row r (lane r&31, slot r>>5)
         // (kept AFTER the expansion: hoisting these two reductions above it, as the warp32 engine does, lands them inside
         // the divergent region of the `near` lanes here and REDUX then takes its slow divergent path — 3.6x slower)
@@ -361,6 +384,14 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
     }
     __syncwarp();
     const int steps = (!kContinue && t_solve >= 0) ? (t + 1) : t;
+    if constexpr (kExit == kExitCoupled1) if (lane == 0) {
+        if (t & 31) a.cw.bits[int64_t(b) * a.cw.words + (t >> 5)] = gbits;   // the last, partial word
+        a.cw.stop[b] = t;
+        // left before the cap with the goal selected: the fixed point (a fixed point at step T-1 looks capped, which
+        // is the same record: no step past the cap is ever read)
+        a.cw.end[b] = (t_solve == NASTAR_TS_EXHAUSTED) ? kEndExhausted : ((t < T) ? kEndFixed : kEndCapped);
+        a.cw.first[b] = t_solve;
+    }
 
     if (kBwd) {
         // close the intervals of the cells still open, scale: dL/dcost = -(1-g_ratio)/sqrt(W) * acc

@@ -67,6 +67,8 @@ _SIGNATURES = {
     "nastar_b200_forward_workspace_bytes": (ctypes.c_size_t, [_i32] * 3),
     "nastar_b200_backward_workspace_bytes": (ctypes.c_size_t, [_i32] * 3),
     "nastar_b200_forward": (_int, [ctypes.POINTER(FwdParams), _p]),
+    "nastar_b200_forward_coupled_workspace_bytes": (ctypes.c_size_t, [_i32] * 4),
+    "nastar_b200_forward_coupled": (_int, [ctypes.POINTER(FwdParams), _p, _p, _p]),
     "nastar_b200_backward": (_int, [ctypes.POINTER(BwdParams), _p]),
     "nastar_b200_backward_mech": (_int, [ctypes.POINTER(BwdParams), _i32, _p]),
     "nastar_b200_batch_steps": (_int, [_p, _p, _i32, _i32, _p, _p]),
@@ -95,6 +97,7 @@ EXPORTS = tuple(_SIGNATURES)
 
 _lib = None
 _ws_cache = {}
+_coupled_ws_cache = {}
 
 
 class NativeLibraryMissing(ImportError):
@@ -271,6 +274,74 @@ def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: t
     if want_counts:
         return hist, paths, t_solve, n_steps, trace, SearchCounts((counters[2], counters[3]))
     return hist, paths, t_solve, n_steps, trace
+
+
+def forward_coupled(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: torch.Tensor,
+                    g_ratio: float, T: int, *, cost_kind: int = COST_PLANE, cost_scale: float = 1.0,
+                    cost_bias: float = 0.0, mechanism: str = "moore", want_counts: bool = False):
+    """The reference's batch-synchronous search for g_ratio < 0.5 with T_batch decided on the device
+    (include/nastar_b200.h, nastar_b200_forward_coupled): every map's outputs after exactly
+    T_batch = 1 + min{k < T : every map selects its goal at step k} steps (T if there is none), in three launches on the
+    current stream and without a host synchronisation, so the call can be captured in a CUDA graph.
+
+    Inputs as in `forward` (no trace, no pair).  Returns (histories [B,1,H,W] f32, paths [B,1,H,W] i64, t_solve [B] i32,
+    n_steps [B] i32, T_batch [1] i32, goal_clamp [B] i32), all on the inputs' device; with `want_counts` a seventh
+    element (n_closed [B], path_len [B]) is appended.  The first five equal `forward(..., T=T_batch,
+    no_early_exit=True)`; goal_clamp is 0 where the goal is selected at least twice within T_batch steps and T_batch
+    elsewhere, the `t_solve` that `backward` takes for such a forward."""
+    news = mechanism_code(mechanism) == MECHANISMS["news"]
+    L = lib()
+    if not cost.is_cuda:
+        raise RuntimeError("neural_astar (H100): the search runs on CUDA tensors only (no CPU fallback); "
+                           "move the planner inputs to the GPU")
+    dev = cost.device
+    for t_ in (start, goal, obst):
+        if t_.device != dev:
+            raise RuntimeError("all planes must live on the same CUDA device")
+    if start.ndim != 4:
+        raise ValueError("planes are [B,C,H,W]")
+    B, _, H, W = start.shape
+    planes = [("start", start), ("goal", goal), ("obst", obst)]
+    p = FwdParams()
+    if cost_kind == COST_TAPS:
+        if cost.dtype != torch.float32 or tuple(cost.shape) != (B, H, W, 9) or not cost.is_contiguous():
+            raise ValueError("COST_TAPS expects a contiguous fp32 [B,H,W,9] tensor")
+        p.cost, p.cost_stride = cost.data_ptr(), 9 * H * W
+    else:
+        planes.insert(0, ("cost", cost))
+    for _, t_ in planes:
+        if t_.shape[0] != B or t_.shape[-2:] != (H, W):
+            raise ValueError("plane shapes differ")
+    keep = _set_planes(p, planes)
+    gr, omg, _ = host_scalars(g_ratio, W)
+    p.B, p.H, p.W = B, H, W
+    p.g_ratio, p.one_minus_g_ratio = gr, omg
+    p.T = int(T)
+    p.flags = FWD_NEWS if news else 0
+    p.cost_kind, p.cost_scale, p.cost_bias = int(cost_kind), float(cost_scale), float(cost_bias)
+    key = (B, H, W, int(T))
+    ws_bytes = _coupled_ws_cache.get(key)
+    if ws_bytes is None:
+        ws_bytes = _coupled_ws_cache[key] = int(L.nastar_b200_forward_coupled_workspace_bytes(B, H, W, int(T)))
+    with _on_device(dev) as stream:
+        hist = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
+        paths = torch.empty((B, 1, H, W), dtype=torch.int64, device=dev)
+        counters = torch.empty((5 if want_counts else 3, B), dtype=torch.int32, device=dev)  # [t_solve | n_steps | clamp | ...]
+        t_solve, n_steps, goal_clamp = counters[0], counters[1], counters[2]
+        T_batch = torch.empty((1,), dtype=torch.int32, device=dev)
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        p.histories, p.paths = hist.data_ptr(), paths.data_ptr()
+        p.t_solve, p.n_steps = t_solve.data_ptr(), n_steps.data_ptr()
+        if want_counts:
+            p.n_closed, p.path_len = counters[3].data_ptr(), counters[4].data_ptr()
+        p.trace = None
+        p.workspace, p.workspace_bytes = ws.data_ptr(), ws_bytes
+        _check(L.nastar_b200_forward_coupled(ctypes.byref(p), T_batch.data_ptr(), goal_clamp.data_ptr(), stream),
+               "nastar_b200_forward_coupled")
+    del keep
+    if want_counts:
+        return hist, paths, t_solve, n_steps, T_batch, goal_clamp, SearchCounts((counters[3], counters[4]))
+    return hist, paths, t_solve, n_steps, T_batch, goal_clamp
 
 
 def pack_inputs(map_designs: torch.Tensor, start: torch.Tensor, goal: torch.Tensor) -> torch.Tensor:

@@ -164,10 +164,13 @@ class NeuralAstar(VanillaAstar):
         """Inference fast path: the search kernel consumes the encoder's 9-tap partial products directly
         (NASTAR_COST_TAPS), so no cost plane, sigmoid, bias add or layout conversion is launched.  Returns None
         when it does not apply (training / autograd, CPU tensors, planning grids above 64x64, encoders without a
-        single-output-channel conv head, g_ratio < 0.5 batches, pq_astar)."""
+        single-output-channel conv head, pq_astar, and g_ratio < 0.5 batches outside CUDA-graph capture: those keep
+        the host procedure of DifferentiableAstar.forward, while under capture search_from_taps couples the batch on
+        the device)."""
         H, W = start_maps.shape[-2], start_maps.shape[-1]
+        coupled = float(self.g_ratio) < 0.5 and start_maps.shape[0] > 1
         if (not self.use_differentiable_astar or not self.encoder.fast_path_ok(map_designs) or H > 64 or W > 64
-                or not start_maps.is_cuda or (float(self.g_ratio) < 0.5 and start_maps.shape[0] > 1)
+                or not start_maps.is_cuda or (coupled and not torch.cuda.is_current_stream_capturing())
                 or start_maps.dtype != torch.float32 or passable.dtype != torch.float32):
             return None
         head = self._head_taps(map_designs, start_maps, goal_maps)

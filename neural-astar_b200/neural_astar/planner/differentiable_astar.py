@@ -107,17 +107,29 @@ class _AstarSearch(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped=None,
-                mechanism="moore"):
+                mechanism="moore", device_coupled=False):
         # goal_clamped is given only on the batch-coupled path (g_ratio < 0.5, see _coupled_steps): the search then
-        # runs exactly T steps per map and the backward is told which goals were selected more than once
-        no_early_exit = goal_clamped is not None
-        hist, paths, t_solve, n_steps, trace = _native.forward(
-            cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, no_early_exit, **_mech_kw(mechanism))
+        # runs exactly T steps per map and the backward is told which goals were selected more than once.
+        # device_coupled: the same batch coupling decided on the device (_native.forward_coupled, T is the cap), which
+        # hands T_batch and the goal clamp to the backward as device tensors
+        ctx.device_T_batch = None
+        if device_coupled:
+            hist, paths, t_solve, n_steps, T_batch, goal_clamp = _native.forward_coupled(
+                cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, **_mech_kw(mechanism))
+            trace = None
+            ctx.device_T_batch = T_batch
+        else:
+            no_early_exit = goal_clamped is not None
+            hist, paths, t_solve, n_steps, trace = _native.forward(
+                cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, no_early_exit,
+                **_mech_kw(mechanism))
         ctx.g_ratio = g_ratio
         ctx.mechanism = mechanism
         ctx.T = T
-        ctx.no_early_exit = no_early_exit
-        if no_early_exit:
+        ctx.no_early_exit = no_early_exit = goal_clamped is not None
+        if device_coupled:
+            t_for_bwd = goal_clamp   # already the backward's encoding (include/nastar_b200.h, nastar_bwd_params)
+        elif no_early_exit:
             # encoding understood by nastar_b200_backward: t_solve < T_batch-1  <=>  gradient blocked at the goal
             t_for_bwd = torch.where(goal_clamped, torch.zeros_like(t_solve), torch.full_like(t_solve, T))
         else:
@@ -133,7 +145,9 @@ class _AstarSearch(torch.autograd.Function):
         cost, start, goal, obst, t_solve, n_steps = ctx.saved_tensors
         grad_cost = None
         if ctx.needs_input_grad[0]:
-            if ctx.no_early_exit:   # the forward already ran exactly the reference's T_batch steps
+            if ctx.device_T_batch is not None:
+                T_batch = ctx.device_T_batch
+            elif ctx.no_early_exit:   # the forward already ran exactly the reference's T_batch steps
                 T_batch = torch.full((1,), ctx.T, dtype=torch.int32, device=cost.device)
             else:
                 T_batch = _native.batch_steps(t_solve, n_steps, ctx.T)
@@ -143,7 +157,7 @@ class _AstarSearch(torch.autograd.Function):
                 full = torch.zeros_like(cost)
                 full[:, :1] = grad_cost
                 grad_cost = full
-        return grad_cost, None, None, None, None, None, None, None, None
+        return grad_cost, None, None, None, None, None, None, None, None, None
 
 
 class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
@@ -200,6 +214,14 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
         g_ratio = float(self.g_ratio)
         coupled = g_ratio < 0.5 and cost_maps.shape[0] > 1
         goal_clamped = None
+        if coupled and cost_maps.is_cuda and torch.cuda.is_current_stream_capturing():
+            # under CUDA-graph capture the host decision below cannot happen: decide T_batch on the device instead
+            # (_native.forward_coupled, the same outputs and gradient); frames need the host procedure's trace
+            if store_intermediate_results:
+                raise ValueError("store_intermediate_results needs a host sync and cannot be captured")
+            hist, paths, _, _, _ = _AstarSearch.apply(
+                cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, False, None, self.mechanism, True)
+            return AstarOutput(hist, paths, [])
         if coupled:
             # For g_ratio < 0.5 a solved map does not necessarily keep re-selecting its goal (SURVEY App. A.4),
             # so the reference's batch-synchronous loop (:251-252) changes the outputs of already-solved maps.
@@ -224,9 +246,19 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
                          store_intermediate_results: bool = False) -> AstarOutput:
         """Inference-only entry of the fused encoder hand-off (SURVEY.md 8(f)-3): `taps` [B,H,W,9] are the
         partial products of the encoder's last 3x3 conv; the kernel prologue computes
-        cost = sigmoid(bias + gather(taps)) * scale (encoder.py:32-34) and searches on it.  No autograd."""
+        cost = sigmoid(bias + gather(taps)) * scale (encoder.py:32-34) and searches on it.  No autograd.
+        A batch of more than one map with g_ratio < 0.5 is searched batch-coupled like `forward` (the reference's
+        loop, :251-252), with T_batch decided on the device (_native.forward_coupled); it has no frames."""
         W = start_maps.shape[-1]
         T = self.num_steps(W)
+        if float(self.g_ratio) < 0.5 and start_maps.shape[0] > 1:
+            if store_intermediate_results:
+                raise ValueError("store_intermediate_results is not available for a batch-coupled search from taps "
+                                 "(g_ratio < 0.5, more than one map): use forward() on the cost maps")
+            hist, paths = _native.forward_coupled(
+                taps, start_maps, goal_maps, obstacles_maps, float(self.g_ratio), T, cost_kind=_native.COST_TAPS,
+                cost_scale=scale, cost_bias=bias, **_mech_kw(self.mechanism))[:2]
+            return AstarOutput(hist, paths, [])
         hist, paths, t_solve, n_steps, trace = _native.forward(
             taps, start_maps, goal_maps, obstacles_maps, float(self.g_ratio), T, bool(store_intermediate_results),
             cost_kind=_native.COST_TAPS, cost_scale=scale, cost_bias=bias, **_mech_kw(self.mechanism))

@@ -18,7 +18,9 @@ the step is close to CPU-launch bound and slows down further when several ranks 
     handles = [over.submit(*batch) for batch in batches]
     outs = [h.result() for h in handles]               # each result() orders the current stream after that batch
 
-Inference only (eval mode, no autograd, `store_intermediate_results=False`, `g_ratio >= 0.5` or batch 1).
+Inference only (eval mode, no autograd, `store_intermediate_results=False`).  Batches of more than one map with
+`g_ratio < 0.5` are searched batch-coupled, as the eager call does; inside the graphs T_batch is decided on the device
+(`_native.forward_coupled`) instead of by the eager call's host round trip, with the same outputs.
 """
 from __future__ import annotations
 
@@ -32,8 +34,6 @@ from ..planner.differentiable_astar import AstarOutput
 def _check_planner(planner, map_designs):
     if planner.training:
         raise ValueError("graph capture covers the inference forward: call planner.eval() first")
-    if getattr(planner, "g_ratio", 0.5) < 0.5 and map_designs.shape[0] > 1:
-        raise ValueError("g_ratio < 0.5 needs a host decision per batch (batch-coupled stop) and cannot be captured")
     dev = next((p.device for p in planner.parameters()), torch.device("cuda", torch.cuda.current_device()))
     if dev.type != "cuda":
         raise ValueError("the planner must live on a CUDA device")

@@ -96,8 +96,9 @@ class GraphedTrainStep:
 
     An eager step issues ~150 small launches from Python (train-mode convs + BatchNorms, their backward, the two
     search kernels, the optimiser's foreach kernels) and is CPU-launch bound at b=100 / 32x32; the replay is one
-    launch.  Same arithmetic as the eager step (same kernels, same order).  Fixed batch shape; `g_ratio >= 0.5` or
-    batch 1 (the batch-coupled procedure below 0.5 needs a host decision per batch).
+    launch.  Same arithmetic as the eager step (same kernels, same order).  Fixed batch shape.  Below `g_ratio` 0.5 the
+    captured search couples the batch with T_batch decided on the device (`_native.forward_coupled`) where the eager
+    step decides it on the host; outputs and gradients are the same.
 
         step = GraphedTrainStep(module, example_batch)        # module: PlannerModule, in train() mode, on CUDA
         for batch in loader:
@@ -108,8 +109,6 @@ class GraphedTrainStep:
         planner = module.planner
         if not module.training:
             raise ValueError("GraphedTrainStep captures the training step: call module.train() first")
-        if float(getattr(planner, "g_ratio", 0.5)) < 0.5 and example_batch[0].shape[0] > 1:
-            raise ValueError("g_ratio < 0.5 needs a host decision per batch and cannot be captured")
         self.module = module
         dev = next(planner.parameters()).device
         self.optimizer = torch.optim.RMSprop(planner.parameters(), module.config.params.lr, capturable=True)
