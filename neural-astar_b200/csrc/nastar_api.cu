@@ -65,7 +65,8 @@ cudaError_t launch_smem(void (*kernel)(P...), int grid, int block, size_t smem, 
     return e;
 }
 
-// f(std::bool_constant<flags>...): turns runtime flags into template arguments, one instantiation per combination
+// f(std::bool_constant<flags>...): turns runtime flags into template arguments, one instantiation per combination; a
+// flag passed as std::false_type has no `true` instantiation
 template <class F>
 auto with_flags(F&& f) {
     return f();
@@ -75,10 +76,21 @@ auto with_flags(F&& f, bool flag, Rest... rest) {
     if (flag) return with_flags([&](auto... t) { return f(std::true_type{}, t...); }, rest...);
     return with_flags([&](auto... t) { return f(std::false_type{}, t...); }, rest...);
 }
+template <class F, class... Rest>
+auto with_flags(F&& f, std::false_type, Rest... rest) {
+    return with_flags([&](auto... t) { return f(std::false_type{}, t...); }, rest...);
+}
+
+// `flag` where the kernel has a variant for it (kHas), else std::false_type
+template <bool kHas>
+auto flag_if(bool flag) {
+    if constexpr (kHas) return flag;
+    else return std::false_type{};
+}
 
 // one-time fill of the kSide x kSide heuristic table (g_heur32 / g_heur64, or their NEWS twins) on the current device,
 // stream-ordered before first use; each table has its own per-device done mask
-template <int kSide, bool kNews = false>
+template <int kSide, bool kNews>
 cudaError_t ensure_heur(cudaStream_t stream) {
     static std::atomic<uint64_t> done_mask{0};
     int dev = 0;
@@ -86,8 +98,7 @@ cudaError_t ensure_heur(cudaStream_t stream) {
     if (e != cudaSuccess) return e;
     const uint64_t bit = uint64_t(1) << (dev & 63);
     if (done_mask.load(std::memory_order_acquire) & bit) return cudaSuccess;
-    auto* const init = kSide == 32 ? nastar::heur32_init_kernel<kNews> : nastar::heur64_init_kernel<kNews>;
-    init<<<kSide * kSide / 256, 256, 0, stream>>>();
+    nastar::heur_init_kernel<kSide, kNews><<<kSide * kSide / 256, 256, 0, stream>>>();
     g_launches.fetch_add(1, std::memory_order_relaxed);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
@@ -98,10 +109,10 @@ cudaError_t ensure_heur(cudaStream_t stream) {
     return cudaSuccess;
 }
 
-// W32Args / W64Args / GenArgs of a backward call: the search inputs in `f`, then the backward-only fields
-template <class A>
-A bwd_kernel_args(const nastar_bwd_params* p) {
-    A a{};
+// SearchArgs of a backward call: the search inputs in `f` (NASTAR_FWD_NEWS in f.flags for `news`), then the
+// backward-only fields
+nastar::SearchArgs bwd_kernel_args(const nastar_bwd_params* p, bool news) {
+    nastar::SearchArgs a{};
     a.f.cost = p->cost;   a.f.cost_stride = p->cost_stride;
     a.f.start = p->start; a.f.start_stride = p->start_stride;
     a.f.goal = p->goal;   a.f.goal_stride = p->goal_stride;
@@ -110,6 +121,7 @@ A bwd_kernel_args(const nastar_bwd_params* p) {
     a.f.g_ratio = p->g_ratio;
     a.f.one_minus_g_ratio = p->one_minus_g_ratio;
     a.f.T = 0;   // the loop bound comes from *T_batch on the device
+    a.f.flags = news ? NASTAR_FWD_NEWS : 0;
     a.f.workspace = p->workspace;
     a.f.workspace_bytes = p->workspace_bytes;
     a.sqrt_w = p->sqrt_w;
@@ -131,6 +143,54 @@ int generic_engine_for(int32_t H, int32_t W) {
 }
 
 int generic_slots(int B) { return capped_grid(B, kGlobalCtasPerSm); }
+
+// Launches the search kernel of `engine` (nastar_b200_engine_for) for the problems in a.f, with exit mode kExit, or the
+// backward replay (kBwd).  The variant follows a.f: a trace when a.f.trace is set, the fused prologue for cost_kind !=
+// NASTAR_COST_PLANE, 4-connected for NASTAR_FWD_NEWS; the 32-wide engine runs 2B CTAs under NASTAR_FWD_PAIR.  The
+// generic engine gets one CTA per map, or one per workspace slot when its state or the backward lives in the
+// workspace.  Fills the heuristic table first where the engine reads one; the launch is left for launched().
+template <int kExit, bool kBwd>
+cudaError_t launch_search(int engine, const nastar::SearchArgs& a, cudaStream_t stream) {
+    constexpr bool kMayTrace = !kBwd && (kExit == nastar::kExitEarly || kExit == nastar::kExitNone);
+    const auto trace = flag_if<kMayTrace>(a.f.trace != nullptr);
+    const auto fused = flag_if<!kBwd>(a.f.cost_kind != NASTAR_COST_PLANE);
+    const bool news = (a.f.flags & NASTAR_FWD_NEWS) != 0;
+    const int B = a.f.B;
+    if (engine == 1 || engine == 4) {
+        const cudaError_t e = (engine == 1) ? (news ? ensure_heur<32, true>(stream) : ensure_heur<32, false>(stream))
+                                            : (news ? ensure_heur<64, true>(stream) : ensure_heur<64, false>(stream));
+        if (e != cudaSuccess) return e;
+    }
+    if (engine == 1) {
+        const int grid = (a.f.flags & NASTAR_FWD_PAIR) ? 2 * B : B;   // output slots
+        return with_flags([&](auto kTrace, auto kFused, auto kNews) {
+            // the backward's dynamic shared memory is the per-cell interval state of the event-based closed form
+            // (W32Bwd, 32 KB); with the 17.4 KB of static planes that is above the 48 KB default, hence the opt-in
+            if constexpr (kBwd) {
+                return launch_smem(nastar::astar_warp32_kernel<kTrace, true, kExit, kFused, kNews>, grid, 32,
+                                   sizeof(nastar::W32Bwd), stream, a);
+            } else {
+                nastar::astar_warp32_kernel<kTrace, false, kExit, kFused, kNews><<<grid, 32, 0, stream>>>(a);
+                return cudaSuccess;
+            }
+        }, trace, fused, news);
+    }
+    if (engine == 4) {
+        // the backward's event-based closed form keeps its per-cell state next to the forward state in shared memory
+        const size_t smem = sizeof(nastar::W64Smem) + (kBwd ? sizeof(nastar::W64Bwd) : 0);
+        return with_flags([&](auto kTrace, auto kFused, auto kNews) {
+            return launch_smem(nastar::astar_warp64_kernel<kTrace, kExit, kBwd, kFused, kNews>, B, 32, smem, stream, a);
+        }, trace, fused, news);
+    }
+    const nastar::GenericLayout L(a.f.H, a.f.W);
+    const bool global = (engine == 3);
+    const size_t smem = L.smem_common() + (global ? 0 : L.smem_planes());
+    const int grid = (global || kBwd) ? generic_slots(B) : B;
+    return with_flags([&](auto kGlobal, auto kTrace, auto kNews) {
+        return launch_smem(nastar::astar_generic_kernel<kGlobal, kTrace, kBwd, kExit, kNews>, grid, 32, smem, stream,
+                           a);
+    }, global, trace, news);
+}
 
 // ---- engine 5 (nastar_bin16.cuh): binary-cost maps, one CTA per map --------------------------------------
 // NASTAR_B200_BIN16=0 in the environment disables it (A/B measurements against engines 2/3)
@@ -322,44 +382,24 @@ int nastar_b200_forward(const nastar_fwd_params* p, void* stream_v) {
         cudaError_t e = cudaMemsetAsync(p->trace, 0xFF, size_t(nmaps) * size_t(p->T) * sizeof(int32_t), stream);
         if (e != cudaSuccess) return cuda_fail(e);
     }
-    const bool trace = p->trace != nullptr;
+    nastar::SearchArgs a{};
+    a.f = *p;
     const bool noexit = (p->flags & NASTAR_FWD_NO_EARLY_EXIT) != 0;
-    const bool fused = p->cost_kind != NASTAR_COST_PLANE;
-    const bool news = (p->flags & NASTAR_FWD_NEWS) != 0;
-    if (engine == 1) {
-        const cudaError_t e = news ? ensure_heur<32, true>(stream) : ensure_heur<32>(stream);
-        if (e != cudaSuccess) return cuda_fail(e);
-        nastar::W32Args a{};
-        a.f = *p;
-        with_flags([&](auto kTrace, auto kNoExit, auto kFused, auto kNews) {
-            nastar::astar_warp32_kernel<kTrace, false, kNoExit, kFused, kNews><<<nmaps, 32, 0, stream>>>(a);
-        }, trace, noexit, fused, news);
-        return launched();
-    }
-    if (engine == 4) {
-        cudaError_t e = news ? ensure_heur<64, true>(stream) : ensure_heur<64>(stream);
-        if (e != cudaSuccess) return cuda_fail(e);
-        nastar::W64Args wa{};
-        wa.f = *p;
-        e = with_flags([&](auto kTrace, auto kNoExit, auto kFused, auto kNews) {
-            return launch_smem(nastar::astar_warp64_kernel<kTrace, kNoExit, false, kFused, kNews>, p->B, 32,
-                               sizeof(nastar::W64Smem), stream, wa);
-        }, trace, noexit, fused, news);
-        if (e != cudaSuccess) return cuda_fail(e);
-        return launched();
-    }
-    const nastar::GenericLayout L(p->H, p->W);
+    auto launch = [&]() {
+        const cudaError_t e = noexit ? launch_search<nastar::kExitNone, false>(engine, a, stream)
+                                     : launch_search<nastar::kExitEarly, false>(engine, a, stream);
+        return e == cudaSuccess ? launched() : cuda_fail(e);
+    };
+    if (engine == 1 || engine == 4) return launch();
     const bool global = (engine == 3);
-    const size_t smem = L.smem_common() + (global ? 0 : L.smem_planes());
-    const int grid = global ? generic_slots(p->B) : p->B;
-    const size_t slots_bytes = global ? size_t(grid) * L.slot_bytes() : 0;
+    const size_t slots_bytes =
+        global ? size_t(generic_slots(p->B)) * nastar::GenericLayout(p->H, p->W).slot_bytes() : 0;
     if (global && (!p->workspace || p->workspace_bytes < slots_bytes)) return NASTAR_EWORKSPACE;
-    nastar::GenArgs ga{};
-    ga.f = *p;
     // engine 5 first when the cost plane IS the binary obstacle plane (VanillaAstar / Config 5): whole map on
     // chip, one CTA per SM pulling maps from a queue; maps it flags are re-run below by the generic engine.
     // Engine 5 is Moore-only: NEWS searches go straight to the generic engine.
     const bool aliased = (p->obst == p->cost) && (p->obst_stride == p->cost_stride);
+    const bool news = (p->flags & NASTAR_FWD_NEWS) != 0;
     const size_t aux = bin16_aux_bytes(p->B);
     if (bin16_enabled() && aliased && !news && !p->trace && p->flags == 0 && bin16_shape_ok(p->H, p->W) && p->workspace &&
         p->workspace_bytes >= aux + slots_bytes) {
@@ -385,16 +425,11 @@ int nastar_b200_forward(const nastar_fwd_params* p, void* stream_v) {
         if (e != cudaSuccess) return cuda_fail(e);
         const int st = launched();
         if (st != NASTAR_OK) return st;
-        ga.redo = ba.redo;
-        ga.f.workspace = ws + aux;
-        ga.f.workspace_bytes = p->workspace_bytes - aux;
+        a.redo = ba.redo;
+        a.f.workspace = ws + aux;
+        a.f.workspace_bytes = p->workspace_bytes - aux;
     }
-    const cudaError_t e = with_flags([&](auto kGlobal, auto kTrace, auto kNoExit, auto kNews) {
-        return launch_smem(nastar::astar_generic_kernel<kGlobal, kTrace, false, kNoExit, kNews>, grid, 32, smem, stream,
-                           ga);
-    }, global, trace, noexit, news);
-    if (e != cudaSuccess) return cuda_fail(e);
-    return launched();
+    return launch();
 }
 
 size_t nastar_b200_forward_coupled_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t T) {
@@ -417,67 +452,26 @@ int nastar_b200_forward_coupled(const nastar_fwd_params* p, int32_t* T_batch, in
     const size_t need = nastar_b200_forward_coupled_workspace_bytes(p->B, p->H, p->W, p->T);
     if (!p->workspace || p->workspace_bytes < need) return NASTAR_EWORKSPACE;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-    const bool fused = p->cost_kind != NASTAR_COST_PLANE;
-    const bool news = (p->flags & NASTAR_FWD_NEWS) != 0;
-    const nastar::CoupledWs cw = coupled_ws(p->workspace, p->B, p->T);
+    nastar::SearchArgs a{};
+    a.f = *p;
+    a.T_batch = T_batch;
+    a.cw = coupled_ws(p->workspace, p->B, p->T);
+    if (engine == 2 || engine == 3) {
+        const size_t aux = coupled_aux_bytes(p->B, p->T);
+        a.f.workspace = static_cast<unsigned char*>(p->workspace) + aux;   // engine 3's slots follow the records
+        a.f.workspace_bytes = p->workspace_bytes - aux;
+    }
     // pass 1 (kExitCoupled1), the reduction, pass 2 (kExitCoupled2): three launches, no host round trip
-    auto both_passes = [&](auto launch_pass) -> int {
-        cudaError_t e = launch_pass(std::integral_constant<int, nastar::kExitCoupled1>{});
-        if (e != cudaSuccess) return cuda_fail(e);
-        int st = launched();
-        if (st != NASTAR_OK) return st;
-        coupled_reduce_kernel<<<1, kCoupledThreads, 0, stream>>>(cw, p->B, p->T, T_batch, goal_clamp);
-        st = launched();
-        if (st != NASTAR_OK) return st;
-        e = launch_pass(std::integral_constant<int, nastar::kExitCoupled2>{});
-        if (e != cudaSuccess) return cuda_fail(e);
-        return launched();
-    };
-    if (engine == 1) {
-        const cudaError_t e = news ? ensure_heur<32, true>(stream) : ensure_heur<32>(stream);
-        if (e != cudaSuccess) return cuda_fail(e);
-        nastar::W32Args a{};
-        a.f = *p;
-        a.T_batch = T_batch;
-        a.cw = cw;
-        return both_passes([&](auto kExit) {
-            with_flags([&](auto kFused, auto kNews) {
-                nastar::astar_warp32_kernel<false, false, kExit, kFused, kNews><<<p->B, 32, 0, stream>>>(a);
-            }, fused, news);
-            return cudaSuccess;
-        });
-    }
-    if (engine == 4) {
-        const cudaError_t e = news ? ensure_heur<64, true>(stream) : ensure_heur<64>(stream);
-        if (e != cudaSuccess) return cuda_fail(e);
-        nastar::W64Args wa{};
-        wa.f = *p;
-        wa.T_batch = T_batch;
-        wa.cw = cw;
-        return both_passes([&](auto kExit) {
-            return with_flags([&](auto kFused, auto kNews) {
-                return launch_smem(nastar::astar_warp64_kernel<false, kExit, false, kFused, kNews>, p->B, 32,
-                                   sizeof(nastar::W64Smem), stream, wa);
-            }, fused, news);
-        });
-    }
-    const nastar::GenericLayout L(p->H, p->W);
-    const bool global = (engine == 3);
-    const size_t smem = L.smem_common() + (global ? 0 : L.smem_planes());
-    const int grid = global ? generic_slots(p->B) : p->B;
-    const size_t aux = coupled_aux_bytes(p->B, p->T);
-    nastar::GenArgs ga{};
-    ga.f = *p;
-    ga.f.workspace = static_cast<unsigned char*>(p->workspace) + aux;   // engine 3's slots follow the records
-    ga.f.workspace_bytes = p->workspace_bytes - aux;
-    ga.T_batch = T_batch;
-    ga.cw = cw;
-    return both_passes([&](auto kExit) {
-        return with_flags([&](auto kGlobal, auto kNews) {
-            return launch_smem(nastar::astar_generic_kernel<kGlobal, false, false, kExit, kNews>, grid, 32, smem,
-                               stream, ga);
-        }, global, news);
-    });
+    cudaError_t e = launch_search<nastar::kExitCoupled1, false>(engine, a, stream);
+    if (e != cudaSuccess) return cuda_fail(e);
+    int st = launched();
+    if (st != NASTAR_OK) return st;
+    coupled_reduce_kernel<<<1, kCoupledThreads, 0, stream>>>(a.cw, p->B, p->T, T_batch, goal_clamp);
+    st = launched();
+    if (st != NASTAR_OK) return st;
+    e = launch_search<nastar::kExitCoupled2, false>(engine, a, stream);
+    if (e != cudaSuccess) return cuda_fail(e);
+    return launched();
 }
 
 int nastar_b200_backward(const nastar_bwd_params* p, void* stream_v) {
@@ -490,41 +484,16 @@ int nastar_b200_backward_mech(const nastar_bwd_params* p, int32_t mechanism, voi
         return NASTAR_EINVAL;
     if (p->B <= 0 || p->H <= 0 || p->W <= 0) return NASTAR_EINVAL;
     if (mechanism != NASTAR_MECH_MOORE && mechanism != NASTAR_MECH_NEWS) return NASTAR_EINVAL;
-    const bool news = mechanism == NASTAR_MECH_NEWS;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
     const int engine = nastar_b200_engine_for(p->H, p->W);
     if (engine == 0) return NASTAR_EUNSUPPORTED;
-    cudaError_t e;
-    if (engine == 1) {
-        // dynamic shared memory = the per-cell interval state of the event-based closed form (W32Bwd, 32 KB); with the
-        // 17.4 KB of static planes that is above the 48 KB default, hence the opt-in
-        e = news ? ensure_heur<32, true>(stream) : ensure_heur<32>(stream);
-        if (e == cudaSuccess)
-            e = with_flags([&](auto kNews) {
-                return launch_smem(nastar::astar_warp32_kernel<false, true, false, false, kNews>, p->B, 32,
-                                   sizeof(nastar::W32Bwd), stream, bwd_kernel_args<nastar::W32Args>(p));
-            }, news);
-    } else if (engine == 4) {
-        // warp-resident 64-wide engine: event-based closed form next to the forward state in shared memory
-        e = news ? ensure_heur<64, true>(stream) : ensure_heur<64>(stream);
-        if (e == cudaSuccess)
-            e = with_flags([&](auto kNews) {
-                return launch_smem(nastar::astar_warp64_kernel<false, false, true, false, kNews>, p->B, 32,
-                                   sizeof(nastar::W64Smem) + sizeof(nastar::W64Bwd), stream,
-                                   bwd_kernel_args<nastar::W64Args>(p));
-            }, news);
-    } else {
+    if (engine == 2 || engine == 3) {
         const nastar::GenericLayout L(p->H, p->W);
-        const bool global = (engine == 3);
-        const int grid = generic_slots(p->B);
-        if (!p->workspace || p->workspace_bytes < size_t(grid) * L.slot_total(global, true)) return NASTAR_EWORKSPACE;
-        const size_t smem = L.smem_common() + (global ? 0 : L.smem_planes());
-        const nastar::GenArgs ga = bwd_kernel_args<nastar::GenArgs>(p);
-        e = with_flags([&](auto kGlobal, auto kNews) {
-            return launch_smem(nastar::astar_generic_kernel<kGlobal, false, true, false, kNews>, grid, 32, smem, stream,
-                               ga);
-        }, global, news);
+        const size_t need = size_t(generic_slots(p->B)) * L.slot_total(engine == 3, true);
+        if (!p->workspace || p->workspace_bytes < need) return NASTAR_EWORKSPACE;
     }
+    const cudaError_t e =
+        launch_search<nastar::kExitEarly, true>(engine, bwd_kernel_args(p, mechanism == NASTAR_MECH_NEWS), stream);
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();
 }

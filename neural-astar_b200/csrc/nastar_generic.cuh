@@ -15,8 +15,7 @@
 //   kGlobal = true : g, f, parent live in a per-CTA slot of the HBM workspace (L2 resident),
 //                    cost is read through the read-only path; persistent CTAs loop over maps.
 #pragma once
-#include "../../include/nastar_b200.h"
-#include "nastar_common.cuh"
+#include "nastar_engine.cuh"
 
 namespace nastar {
 
@@ -39,21 +38,6 @@ struct GenericLayout {
     }
 };
 
-// forward parameters + the extra fields of nastar_bwd_params (same idea as W32Args)
-struct GenArgs {
-    nastar_fwd_params f;
-    float sqrt_w;
-    const int32_t* T_batch;
-    const int32_t* t_solve_in;
-    const float* grad_hist;
-    int64_t grad_stride;
-    float* grad_cost;
-    // forward only, nullable: per-map flags written by the bin16 engine (nastar_bin16.cuh); when given, only
-    // maps with redo[b] != 0 are processed here (the others were already finished on-chip)
-    const int32_t* redo;
-    CoupledWs cw;   // coupled forward only (see W32Args)
-};
-
 // kBwd = true replays the search for *T_batch steps and accumulates the closed-form gradient (SURVEY App. B)
 //   dL/dcost[p] = -(1-g_ratio)/sqrt(W) * sum_t y_t[p] * (Gh[p] - <Gh, y_t>),   y_t = v_t / S_t over the open set,
 // EVENT-BASED: v_t[p] = exp(-f_t[p]/sqrt(W)) only changes when p is opened, relaxed or closed, so a cell's
@@ -66,7 +50,7 @@ struct GenArgs {
 // kNews: NASTAR_FWD_NEWS / NASTAR_MECH_NEWS — only lanes 1, 3, 5, 7 (N, W, E, S) take a neighbour, and h is the
 // Manhattan heuristic.
 template <bool kGlobal, bool kTrace, bool kBwd, int kExit = kExitEarly, bool kNews = false>
-__global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
+__global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
     constexpr bool kContinue = kBwd || (kExit != kExitEarly);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const nastar_fwd_params& p = a.f;
@@ -474,11 +458,7 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const GenArgs a) {
                 const int wi = (seg << 2) + (lane >> 3);
                 const int q = (seg << 5) + lane;
                 if (q >= nq) continue;            // partial last segment
-                const uint32_t cb = sClosed[wi] >> sh, pb = sPath[wi] >> sh;
-                reinterpret_cast<float4*>(gHist)[q] = make_float4((cb & 1u) ? 1.f : 0.f, (cb & 2u) ? 1.f : 0.f,
-                                                                  (cb & 4u) ? 1.f : 0.f, (cb & 8u) ? 1.f : 0.f);
-                reinterpret_cast<longlong2*>(gPath)[2 * q] = make_longlong2((pb & 1u) ? 1ll : 0ll, (pb & 2u) ? 1ll : 0ll);
-                reinterpret_cast<longlong2*>(gPath)[2 * q + 1] = make_longlong2((pb & 4u) ? 1ll : 0ll, (pb & 8u) ? 1ll : 0ll);
+                store_cells4(gHist, gPath, q, sClosed[wi] >> sh, sPath[wi] >> sh);
             }
         } else {
             for (int y = 0; y < H; ++y) {

@@ -21,39 +21,9 @@
 //   accumulation is event-based (a cell's softmax weight only changes when it is opened, relaxed or
 //   closed: per-cell interval bookkeeping against fp64 prefix sums, O(1) per step).
 #pragma once
-#include "../../include/nastar_b200.h"
-#include "nastar_common.cuh"
+#include "nastar_engine.cuh"
 
 namespace nastar {
-
-// Kernel arguments: the forward parameters plus the extra fields of nastar_bwd_params.
-struct W32Args {
-    nastar_fwd_params f;
-    // backward only
-    float sqrt_w;
-    const int32_t* T_batch;     // device scalar: loop iterations the reference would execute
-    const int32_t* t_solve_in;  // forward's t_solve[] (goal clamp blocking, App. B)
-    const float* grad_hist;
-    int64_t grad_stride;
-    float* grad_cost;
-    // coupled forward only (kExitCoupled1 / kExitCoupled2; pass 2 also reads *T_batch)
-    CoupledWs cw;
-};
-
-constexpr int kCells = 1024;  // padded 32 x 32
-
-// heuristic(|dy|, |dx|) for every offset on a 32x32 grid, filled once per device by
-// heur32_init_kernel with the very same device function the generic engine evaluates inline —
-// the per-map h pass becomes one cached load + one add per cell instead of an IEEE sqrt chain.
-// The second half, g_heur32[kCells + i], is a second table holding the NEWS heuristic (heuristic_news) the same way;
-// it shares the array so that every kernel keeps its global address table.
-__device__ float g_heur32[2 * kCells];
-
-template <bool kNews>
-__global__ void heur32_init_kernel() {
-    const int i = threadIdx.x + blockIdx.x * blockDim.x;
-    if (i < kCells) g_heur32[(kNews ? kCells : 0) + i] = heuristic_of<kNews>(i >> 5, i & 31, 0, 0);
-}
 
 // backward-only planes (dynamic shared memory), event-based closed form (see nastar_generic.cuh / DESIGN.md):
 struct __align__(16) W32Bwd {
@@ -82,7 +52,7 @@ struct __align__(16) W32Smem {
 // of the plain instantiation so that its cold instruction footprint stays small.
 // kNews: NASTAR_FWD_NEWS / NASTAR_MECH_NEWS — 4-connected expansion (N, E, W, S) and the Manhattan heuristic.
 template <bool kTrace, bool kBwd, int kExit = kExitEarly, bool kFused = false, bool kNews = false>
-__global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
+__global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const SearchArgs a) {
     constexpr bool kContinue = kBwd || (kExit != kExitEarly);   // the loop does not stop at the solve step
     __shared__ W32Smem S;
     extern __shared__ __align__(16) unsigned char bwd_raw[];  // backward only: W32Bwd
@@ -435,11 +405,7 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const W32Args a) {
             const int y = (lane >> 3) + 4 * j;
             if (y < H) {
                 const int i4 = lane + 32 * j;
-                const uint32_t cb = S.bits_a[y] >> x, pb = S.bits_b[y] >> x;
-                reinterpret_cast<float4*>(gHist)[i4] = make_float4((cb & 1u) ? 1.f : 0.f, (cb & 2u) ? 1.f : 0.f,
-                                                                   (cb & 4u) ? 1.f : 0.f, (cb & 8u) ? 1.f : 0.f);
-                reinterpret_cast<longlong2*>(gPath)[2 * i4] = make_longlong2((pb & 1u) ? 1ll : 0ll, (pb & 2u) ? 1ll : 0ll);
-                reinterpret_cast<longlong2*>(gPath)[2 * i4 + 1] = make_longlong2((pb & 4u) ? 1ll : 0ll, (pb & 8u) ? 1ll : 0ll);
+                store_cells4(gHist, gPath, i4, S.bits_a[y] >> x, S.bits_b[y] >> x);
             }
         }
     } else {

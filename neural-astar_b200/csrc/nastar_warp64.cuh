@@ -16,21 +16,9 @@
 // set, D = <Gh, v>, both maintained in fp64 from the <= 10 events of a step).  Per-cell v / A(t0) / B(t0) / acc and
 // the upstream gradient live in shared memory next to the forward state (198 KB per map).
 #pragma once
-#include "../../include/nastar_b200.h"
-#include "nastar_common.cuh"
+#include "nastar_engine.cuh"
 
 namespace nastar {
-
-constexpr int kCells64 = 4096;  // padded 64 x 64
-
-// heuristic(|dy|, |dx|) for every offset on a 64x64 grid, then the NEWS table (see g_heur32)
-__device__ float g_heur64[2 * kCells64];
-
-template <bool kNews>
-__global__ void heur64_init_kernel() {
-    const int i = threadIdx.x + blockIdx.x * blockDim.x;
-    if (i < kCells64) g_heur64[(kNews ? kCells64 : 0) + i] = heuristic_of<kNews>(i >> 6, i & 63, 0, 0);
-}
 
 struct __align__(16) W64Smem {
     float cost[kCells64];
@@ -52,24 +40,12 @@ struct __align__(16) W64Bwd {
     float gh[kCells64];     // upstream gradient dL/dhistories (goal zeroed when the clamp blocks it)
 };
 
-// forward parameters + the extra fields of nastar_bwd_params (same idea as W32Args)
-struct W64Args {
-    nastar_fwd_params f;
-    float sqrt_w;
-    const int32_t* T_batch;
-    const int32_t* t_solve_in;
-    const float* grad_hist;
-    int64_t grad_stride;
-    float* grad_cost;
-    CoupledWs cw;   // coupled forward only (see W32Args)
-};
-
 // kFused (forward only): the prologue may have to finish the encoder (NASTAR_COST_LOGIT / NASTAR_COST_TAPS), as in the
 // 32-wide engine; kept out of the plain instantiations.
 // kNews: 4-connected expansion and the Manhattan heuristic, as in the 32-wide engine.
 // kExit: exit mode of the forward (kExitEarly, kExitNone, or a pass of the coupled forward), as in the 32-wide engine.
 template <bool kTrace, int kExit, bool kBwd = false, bool kFused = false, bool kNews = false>
-__global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
+__global__ void __launch_bounds__(32) astar_warp64_kernel(const SearchArgs a) {
     constexpr bool kContinue = kBwd || (kExit != kExitEarly);
     const nastar_fwd_params& p = a.f;
     extern __shared__ __align__(16) unsigned char smem64_raw[];
@@ -444,11 +420,7 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const W64Args a) {
         const int n4 = N >> 2;
         for (int i4 = lane; i4 < n4; i4 += 32) {
             const int y = i4 >> 4;
-            const uint32_t cb = uint32_t(S.bits_a[y] >> x), pb = uint32_t(S.bits_b[y] >> x);
-            reinterpret_cast<float4*>(gHist)[i4] = make_float4((cb & 1u) ? 1.f : 0.f, (cb & 2u) ? 1.f : 0.f,
-                                                               (cb & 4u) ? 1.f : 0.f, (cb & 8u) ? 1.f : 0.f);
-            reinterpret_cast<longlong2*>(gPath)[2 * i4] = make_longlong2((pb & 1u) ? 1ll : 0ll, (pb & 2u) ? 1ll : 0ll);
-            reinterpret_cast<longlong2*>(gPath)[2 * i4 + 1] = make_longlong2((pb & 4u) ? 1ll : 0ll, (pb & 8u) ? 1ll : 0ll);
+            store_cells4(gHist, gPath, i4, uint32_t(S.bits_a[y] >> x), uint32_t(S.bits_b[y] >> x));
         }
     } else {
         for (int y = 0; y < H; ++y) {

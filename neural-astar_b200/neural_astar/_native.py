@@ -206,23 +206,12 @@ class SearchCounts(tuple):
     """(n_closed [B'] i32, path_len [B'] i32): histories.sum() / paths.sum() per map, written by the kernel."""
 
 
-def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: torch.Tensor,
-            g_ratio: float, T: int, want_trace: bool = False, no_early_exit: bool = False, *,
-            pair: bool = False, cost_kind: int = COST_PLANE, cost_scale: float = 1.0, cost_bias: float = 0.0,
-            want_counts: bool = False, mechanism: str = "moore"):
-    """Run the search for a batch of [B,C,H,W] fp32 CUDA planes (channel 0 is used).
-
-    Returns (histories [B',1,H,W] f32, paths [B',1,H,W] i64, t_solve [B'] i32, n_steps [B'] i32,
-    trace [B',T] i32 or None), all on the inputs' device, asynchronously on the current stream; with
-    `want_counts` a sixth element (n_closed [B'], path_len [B']) is appended.  B' = 2B with `pair`
-    (NASTAR_FWD_PAIR: second half = the same problems with cost = obstacles), else B.
-    `cost_kind` = COST_LOGIT / COST_TAPS: `cost` holds the encoder's raw output [B,1,H,W] / the 9-tap partial
-    products [B,H,W,9] and the kernel prologue finishes encoder.py:32-34 itself (H, W <= 64 only).
-    `mechanism` = "moore" (8-connected, Chebyshev heuristic) or "news" (NASTAR_FWD_NEWS: 4-connected, Manhattan
-    heuristic; both halves of a `pair`).
-    """
+def _search_params(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: torch.Tensor, g_ratio: float,
+                   T: int, flags: int, cost_kind: int, cost_scale: float, cost_bias: float, mechanism: str):
+    """Check the inputs of `forward` / `forward_coupled` and fill their FwdParams up to the outputs.  `flags` gets
+    NASTAR_FWD_NEWS added for `mechanism` "news".  Returns (p, planes to keep alive, B, H, W, device)."""
     news = mechanism_code(mechanism) == MECHANISMS["news"]
-    L = lib()
+    lib()
     if not cost.is_cuda:
         raise RuntimeError("neural_astar (H100): the search runs on CUDA tensors only (no CPU fallback); "
                            "move the planner inputs to the GPU")
@@ -249,8 +238,30 @@ def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: t
     p.B, p.H, p.W = B, H, W
     p.g_ratio, p.one_minus_g_ratio = gr, omg
     p.T = int(T)
-    p.flags = (FWD_NO_EARLY_EXIT if no_early_exit else 0) | (FWD_PAIR if pair else 0) | (FWD_NEWS if news else 0)
+    p.flags = flags | (FWD_NEWS if news else 0)
     p.cost_kind, p.cost_scale, p.cost_bias = int(cost_kind), float(cost_scale), float(cost_bias)
+    return p, keep, B, H, W, dev
+
+
+def forward(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: torch.Tensor,
+            g_ratio: float, T: int, want_trace: bool = False, no_early_exit: bool = False, *,
+            pair: bool = False, cost_kind: int = COST_PLANE, cost_scale: float = 1.0, cost_bias: float = 0.0,
+            want_counts: bool = False, mechanism: str = "moore"):
+    """Run the search for a batch of [B,C,H,W] fp32 CUDA planes (channel 0 is used).
+
+    Returns (histories [B',1,H,W] f32, paths [B',1,H,W] i64, t_solve [B'] i32, n_steps [B'] i32,
+    trace [B',T] i32 or None), all on the inputs' device, asynchronously on the current stream; with
+    `want_counts` a sixth element (n_closed [B'], path_len [B']) is appended.  B' = 2B with `pair`
+    (NASTAR_FWD_PAIR: second half = the same problems with cost = obstacles), else B.
+    `cost_kind` = COST_LOGIT / COST_TAPS: `cost` holds the encoder's raw output [B,1,H,W] / the 9-tap partial
+    products [B,H,W,9] and the kernel prologue finishes encoder.py:32-34 itself (H, W <= 64 only).
+    `mechanism` = "moore" (8-connected, Chebyshev heuristic) or "news" (NASTAR_FWD_NEWS: 4-connected, Manhattan
+    heuristic; both halves of a `pair`).
+    """
+    flags = (FWD_NO_EARLY_EXIT if no_early_exit else 0) | (FWD_PAIR if pair else 0)
+    p, keep, B, H, W, dev = _search_params(cost, start, goal, obst, g_ratio, T, flags, cost_kind, cost_scale,
+                                           cost_bias, mechanism)
+    L = lib()
     Bo = 2 * B if pair else B
     ws_bytes = _ws_cache.get((B, H, W))
     if ws_bytes is None:
@@ -289,36 +300,9 @@ def forward_coupled(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor,
     element (n_closed [B], path_len [B]) is appended.  The first five equal `forward(..., T=T_batch,
     no_early_exit=True)`; goal_clamp is 0 where the goal is selected at least twice within T_batch steps and T_batch
     elsewhere, the `t_solve` that `backward` takes for such a forward."""
-    news = mechanism_code(mechanism) == MECHANISMS["news"]
+    p, keep, B, H, W, dev = _search_params(cost, start, goal, obst, g_ratio, T, 0, cost_kind, cost_scale, cost_bias,
+                                           mechanism)
     L = lib()
-    if not cost.is_cuda:
-        raise RuntimeError("neural_astar (H100): the search runs on CUDA tensors only (no CPU fallback); "
-                           "move the planner inputs to the GPU")
-    dev = cost.device
-    for t_ in (start, goal, obst):
-        if t_.device != dev:
-            raise RuntimeError("all planes must live on the same CUDA device")
-    if start.ndim != 4:
-        raise ValueError("planes are [B,C,H,W]")
-    B, _, H, W = start.shape
-    planes = [("start", start), ("goal", goal), ("obst", obst)]
-    p = FwdParams()
-    if cost_kind == COST_TAPS:
-        if cost.dtype != torch.float32 or tuple(cost.shape) != (B, H, W, 9) or not cost.is_contiguous():
-            raise ValueError("COST_TAPS expects a contiguous fp32 [B,H,W,9] tensor")
-        p.cost, p.cost_stride = cost.data_ptr(), 9 * H * W
-    else:
-        planes.insert(0, ("cost", cost))
-    for _, t_ in planes:
-        if t_.shape[0] != B or t_.shape[-2:] != (H, W):
-            raise ValueError("plane shapes differ")
-    keep = _set_planes(p, planes)
-    gr, omg, _ = host_scalars(g_ratio, W)
-    p.B, p.H, p.W = B, H, W
-    p.g_ratio, p.one_minus_g_ratio = gr, omg
-    p.T = int(T)
-    p.flags = FWD_NEWS if news else 0
-    p.cost_kind, p.cost_scale, p.cost_bias = int(cost_kind), float(cost_scale), float(cost_bias)
     key = (B, H, W, int(T))
     ws_bytes = _coupled_ws_cache.get(key)
     if ws_bytes is None:
