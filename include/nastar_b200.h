@@ -420,6 +420,27 @@ int nastar_b200_decode_png(const uint8_t *data, int64_t data_bytes, const nastar
  * nastar_b200_decode_png rejects with NASTAR_EINVAL or NASTAR_EUNSUPPORTED. */
 size_t nastar_b200_decode_png_workspace_bytes(const nastar_png_desc *desc, int32_t B);
 
+/* The reference's heap A* (pq_astar.solve_single, use_differentiable_astar=False), exactly (DESIGN.md §17).  Planes
+ * fp32 [B][H][W] with map strides in elements: cost, start, goal, map.  Per map: start and goal are the single
+ * non-zero cell of their planes; a neighbour (W, E, N, S, NW, NE, SW, SE order) is entered only where map == 1 and is
+ * charged f_new = ((f_sel - (1-g) h(sel)) + g cost[nb]) + (1-g) h(nb), h = max(dx, dy) + 0.001 sqrt(dx^2 + dy^2),
+ * each operation one fp64 rounding; the open list is a binary heap with pqdict 1.2.0's moves, which decide ties.
+ * Writes histories fp32 [B][H*W] (the closed set), paths int64 [B][H*W] (the parent chain from the goal), status
+ * i32 [B] (0 solved, 1 goal not found: histories and paths zero, 2 start or goal not exactly one cell: zero too) and
+ * expansions i32 [B] (cells closed).  Every check precedes the launch: null pointers, B, H or W <= 0, a stride
+ * below H*W or a workspace not 8-byte aligned give NASTAR_EINVAL; H*W > 1048576 gives NASTAR_EUNSUPPORTED; a workspace below
+ * nastar_b200_pq_astar_workspace_bytes gives NASTAR_EWORKSPACE.  One kernel launch (persistent one-warp CTAs).
+ * Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_pq_astar(const float *cost, int64_t cost_stride, const float *start, int64_t start_stride,
+                         const float *goal, int64_t goal_stride, const float *map, int64_t map_stride, int32_t B,
+                         int32_t H, int32_t W, double g_ratio, float *histories, int64_t *paths, int32_t *status,
+                         int32_t *expansions, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Workspace of nastar_b200_pq_astar: a work counter, plus, for maps whose state does not fit in shared memory, one
+ * 20*H*W-byte slot per persistent CTA (at most 8 per SM and 2 GiB in all, but one per SM always), so it does not grow
+ * with B.  0 for shapes that nastar_b200_pq_astar rejects. */
+size_t nastar_b200_pq_astar_workspace_bytes(int32_t B, int32_t H, int32_t W);
+
 /* Number of kernel launches issued by this library since load (bench.py's gpu_launches). */
 uint64_t nastar_b200_launch_count(void);
 

@@ -17,6 +17,7 @@
 #include "nastar_labels.cuh"
 #include "nastar_maps.cuh"
 #include "nastar_png.cuh"
+#include "nastar_pq.cuh"
 #include "nastar_sampler.cuh"
 #include "nastar_wlabels.cuh"
 #include "nastar_warp32.cuh"
@@ -338,6 +339,27 @@ int png_check(const nastar_png_desc* desc, int32_t B, int64_t data_bytes, int64_
 }
 
 size_t png_slot_bytes(int64_t max_raw) { return round256(size_t(max_raw)); }
+
+// ---- heap A* (nastar_pq.cuh) ----------------------------------------------------------------------------------
+// Maps whose 20 B/cell state fits in this many bytes keep it in shared memory, larger ones in a global slot per CTA
+// (threshold measured on an H100: DESIGN.md §17).
+#ifndef NASTAR_PQ_SMEM_MAX_BYTES
+#define NASTAR_PQ_SMEM_MAX_BYTES (32 * 1024)
+#endif
+constexpr size_t kPqWorkspaceBudget = size_t(2) << 30;   // global slots: at most this much, but one CTA per SM always
+
+size_t pq_state_bytes(int32_t H, int32_t W) { return size_t(nastar::kPqBytesPerCell) * size_t(H) * size_t(W); }
+bool pq_shared(int32_t H, int32_t W) { return pq_state_bytes(H, W) <= size_t(NASTAR_PQ_SMEM_MAX_BYTES); }
+int pq_global_grid(int32_t B, int32_t H, int32_t W) {
+    const size_t slot = round256(pq_state_bytes(H, W));
+    const int64_t fit = int64_t(kPqWorkspaceBudget / slot);
+    const int64_t cap = fit > num_sms() ? fit : num_sms();
+    const int g = capped_grid(B, kGlobalCtasPerSm);
+    return int(g < cap ? g : cap);
+}
+bool pq_shape_ok(int32_t B, int32_t H, int32_t W) {
+    return B > 0 && H > 0 && W > 0 && int64_t(H) * W <= nastar::kPqMaxCells;
+}
 
 template <int C>
 void launch_head(const float* x, int64_t P, const float* w_host, float* taps, cudaStream_t stream) {
@@ -770,6 +792,48 @@ int nastar_b200_decode_png(const uint8_t* data, int64_t data_bytes, const nastar
     if (e != cudaSuccess) return cuda_fail(e);
     const nastar::PngArgs a{data, desc_dev, B, out, status, reinterpret_cast<int32_t*>(ws), ws + 256, int64_t(slot)};
     nastar::decode_png_kernel<<<grid, nastar::kPngThreads, 0, stream>>>(a);
+    return launched();
+}
+
+size_t nastar_b200_pq_astar_workspace_bytes(int32_t B, int32_t H, int32_t W) {
+    if (!pq_shape_ok(B, H, W)) return 0;
+    if (pq_shared(H, W)) return 256;
+    return 256 + size_t(pq_global_grid(B, H, W)) * round256(pq_state_bytes(H, W));
+}
+
+int nastar_b200_pq_astar(const float* cost, int64_t cost_stride, const float* start, int64_t start_stride,
+                         const float* goal, int64_t goal_stride, const float* map, int64_t map_stride, int32_t B,
+                         int32_t H, int32_t W, double g_ratio, float* histories, int64_t* paths, int32_t* status,
+                         int32_t* expansions, void* workspace, size_t workspace_bytes, void* stream_v) {
+    if (!cost || !start || !goal || !map || !histories || !paths || !status || !expansions) return NASTAR_EINVAL;
+    if (B <= 0 || H <= 0 || W <= 0) return NASTAR_EINVAL;
+    const int64_t N = int64_t(H) * W;
+    if (cost_stride < N || start_stride < N || goal_stride < N || map_stride < N) return NASTAR_EINVAL;
+    if (reinterpret_cast<uintptr_t>(workspace) & 7) return NASTAR_EINVAL;   // the slots' fp64 arrays
+    if (!pq_shape_ok(B, H, W)) return NASTAR_EUNSUPPORTED;
+    const bool shared = pq_shared(H, W);
+    const int ggrid = shared ? 0 : pq_global_grid(B, H, W);
+    const size_t slot = round256(pq_state_bytes(H, W));
+    if (!workspace || workspace_bytes < 256 + size_t(ggrid) * slot) return NASTAR_EWORKSPACE;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+    unsigned char* ws = static_cast<unsigned char*>(workspace);
+    cudaError_t e = cudaMemsetAsync(ws, 0, 256, stream);   // the work counter
+    if (e != cudaSuccess) return cuda_fail(e);
+    const nastar::PqArgs a{cost, cost_stride, start, start_stride, goal, goal_stride, map, map_stride, B, H, W, g_ratio,
+                           1.0 - g_ratio, histories, paths, status, expansions, reinterpret_cast<int32_t*>(ws), ws + 256,
+                           int64_t(slot)};
+    if (shared) {
+        const size_t smem = pq_state_bytes(H, W);
+        e = cudaFuncSetAttribute(nastar::pq_astar_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+        int per_sm = 0;
+        if (e == cudaSuccess)
+            e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nastar::pq_astar_kernel<true>, nastar::kPqThreads,
+                                                              smem);
+        if (e != cudaSuccess) return cuda_fail(e);
+        nastar::pq_astar_kernel<true><<<capped_grid(B, per_sm > 0 ? per_sm : 1), nastar::kPqThreads, smem, stream>>>(a);
+    } else {
+        nastar::pq_astar_kernel<false><<<ggrid, nastar::kPqThreads, 0, stream>>>(a);
+    }
     return launched();
 }
 

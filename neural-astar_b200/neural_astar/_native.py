@@ -92,6 +92,9 @@ _SIGNATURES = {
     "nastar_b200_draw_policies": (_int, [_p, _p, _i32, _i32, _p, _p]),
     "nastar_b200_decode_png": (_int, [_p, _i64, _p, _p, _i32, _p, _i64, _p, _p, ctypes.c_size_t, _p]),
     "nastar_b200_decode_png_workspace_bytes": (ctypes.c_size_t, [_p, _i32]),
+    "nastar_b200_pq_astar": (_int, [_p, _i64] * 4 + [_i32] * 3 + [ctypes.c_double] + [_p] * 5
+                             + [ctypes.c_size_t, _p]),
+    "nastar_b200_pq_astar_workspace_bytes": (ctypes.c_size_t, [_i32] * 3),
     "nastar_b200_launch_count": (ctypes.c_uint64, []),
     "nastar_b200_status_string": (ctypes.c_char_p, [_int]),
     "nastar_b200_last_cuda_error": (ctypes.c_char_p, []),
@@ -754,6 +757,41 @@ def decode_png(data: torch.Tensor, desc, desc_dev: torch.Tensor, out_bytes: int)
                                         out.data_ptr(), int(out_bytes), status.data_ptr(), ws.data_ptr(), ws_bytes,
                                         stream), "nastar_b200_decode_png")
     return out, status
+
+
+# status of nastar_b200_pq_astar
+PQ_SOLVED, PQ_NOT_FOUND, PQ_BAD_ENDS = 0, 1, 2
+PQ_MAX_CELLS = 1 << 20
+
+
+def pq_astar(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, map_design: torch.Tensor, g_ratio: float):
+    """The reference's heap A* (include/nastar_b200.h, nastar_b200_pq_astar) on channel 0 of fp32 CUDA planes
+    [B,C,H,W], one launch on the current stream.  Returns histories f32 [B,1,H,W], paths i64 [B,1,H,W], status i32 [B]
+    (PQ_*) and expansions i32 [B]; nothing is read back."""
+    L = lib()
+    planes = (cost, start, goal, map_design)
+    if any(not t.is_cuda or t.dtype != torch.float32 or t.ndim != 4 for t in planes):
+        raise RuntimeError("pq_astar: planes must be fp32 CUDA tensors [B,C,H,W] (there is no CPU fallback)")
+    B, _, H, W = cost.shape
+    if any(t.shape[0] != B or t.shape[-2:] != (H, W) or t.device != cost.device for t in planes):
+        raise ValueError("pq_astar: cost, start, goal and map must share B, H, W and the device")
+    if H * W > PQ_MAX_CELLS:
+        raise ValueError(f"pq_astar: H*W = {H * W} is above {PQ_MAX_CELLS} cells")
+    dev = cost.device
+    keep = [_plane(t.detach()) for t in planes]
+    ws_bytes = int(L.nastar_b200_pq_astar_workspace_bytes(B, H, W))
+    with _on_device(dev) as stream:
+        hist = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
+        paths = torch.empty((B, 1, H, W), dtype=torch.int64, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        expansions = torch.empty((B,), dtype=torch.int32, device=dev)
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        args = [a for _, ptr, stride in keep for a in (ptr, stride)]
+        _check(L.nastar_b200_pq_astar(*args, B, H, W, float(g_ratio), hist.data_ptr(), paths.data_ptr(),
+                                      status.data_ptr(), expansions.data_ptr(), ws.data_ptr(), ws_bytes, stream),
+               "nastar_b200_pq_astar")
+    del keep
+    return hist, paths, status, expansions
 
 
 def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Tensor, t_solve: torch.Tensor,

@@ -2,10 +2,10 @@
 
 API contract mirrored from /root/reference/src/neural_astar/planner/astar.py (:17-102 VanillaAstar,
 :105-213 NeuralAstar): constructor keywords, the `.astar` / `.encoder` attributes, `encode()`,
-`perform_astar()` and `forward()` returning `AstarOutput`.  `use_differentiable_astar=False` used to
-select a CPU heap A* (`pq_astar`); both settings are now served by the same GPU search — identical for
-uniform costs, which is what the reference's own test pins (tests/astar_test.py:33-42); see
-planner/pq_astar.py for the cost-convention difference with learned costs.
+`perform_astar()` and `forward()` returning `AstarOutput`.  `use_differentiable_astar=False` selects
+`pq_astar`, the reference's heap A*: by default served by the dense GPU search (identical for uniform costs, which is
+what the reference's own test pins, tests/astar_test.py:33-42), or with `pq_semantics="reference"` by a GPU heap A*
+that reproduces the reference's results for any costs; see planner/pq_astar.py.
 
 Inference hand-off (SURVEY.md 8(f)-3): in eval / no-grad mode on CUDA, `NeuralAstar.forward` runs
 the input assembly (start+goal add, nearest upsample, concat, NHWC) as one kernel — folded into the first
@@ -24,14 +24,32 @@ import torch.nn.functional as F
 from .. import _native
 from . import encoder as _encoders
 from .differentiable_astar import AstarOutput, DifferentiableAstar, TakesMechanism, _mech_kw
-from .pq_astar import pq_astar  # noqa: F401  re-exported, like the reference module does
+from .pq_astar import _check_semantics, pq_astar  # noqa: F401  pq_astar re-exported, like the reference module does
 
 
-class VanillaAstar(nn.Module, metaclass=TakesMechanism):
+class TakesPlannerKeywords(TakesMechanism):
+    """Metaclass of the planners: TakesMechanism's route for one more keyword-only argument, `pq_semantics` ("engine",
+    the default, or "reference"): the semantics of `pq_astar` when `use_differentiable_astar=False` (see
+    planner/pq_astar.py).  Every __init__ keeps the reference's signature.  An unknown value is a ValueError raised
+    before anything is built; "reference" with `use_differentiable_astar=True` is a ValueError too, since it would
+    select nothing."""
+
+    def __call__(cls, *args, pq_semantics: str = "engine", **kwargs):
+        _check_semantics(pq_semantics)
+        planner = super().__call__(*args, **kwargs)
+        if pq_semantics != "engine" and planner.use_differentiable_astar:
+            raise ValueError(f"pq_semantics={pq_semantics!r} applies to use_differentiable_astar=False only")
+        planner.pq_semantics = pq_semantics
+        return planner
+
+
+class VanillaAstar(nn.Module, metaclass=TakesPlannerKeywords):
     """A* on the given map: cost == obstacles == map design (reference :93-94).
 
     Keyword-only `mechanism` = "moore" (default, 8-connected) or "news" (4-connected with the Manhattan heuristic, for
-    the planning-datasets generator's NEWS datasets); see DifferentiableAstar.
+    the planning-datasets generator's NEWS datasets); see DifferentiableAstar.  Keyword-only `pq_semantics` =
+    "engine" (default) or "reference" (the reference's heap A* exactly), for `use_differentiable_astar=False`; see
+    planner/pq_astar.py.
 
     >>> out = VanillaAstar()(map_designs, start_maps, goal_maps)   # out.histories, out.paths
     """
@@ -44,6 +62,7 @@ class VanillaAstar(nn.Module, metaclass=TakesMechanism):
         self.astar = DifferentiableAstar(g_ratio=g_ratio, Tmax=Tmax)
         self.g_ratio = g_ratio
         self.use_differentiable_astar = use_differentiable_astar
+        self.pq_semantics = "engine"
 
     def _select_mechanism(self, mechanism: str) -> None:
         if not self.use_differentiable_astar:
@@ -56,7 +75,7 @@ class VanillaAstar(nn.Module, metaclass=TakesMechanism):
         if self.use_differentiable_astar:
             return self.astar(map_designs, start_maps, goal_maps, obstacles_maps, store_intermediate_results)
         return pq_astar(map_designs, start_maps, goal_maps, obstacles_maps, store_intermediate_results,
-                        g_ratio=self.g_ratio)
+                        g_ratio=self.g_ratio, semantics=self.pq_semantics)
 
     def forward(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
                 store_intermediate_results: bool = False) -> AstarOutput:
@@ -75,9 +94,11 @@ class NeuralAstar(VanillaAstar):
         encoder_depth: number of conv blocks.
         learn_obstacles: hide the obstacle map from the search (all cells passable).
         const: learnable multiplier on the predicted cost (None = 1).
-        use_differentiable_astar: kept for compatibility, see module docstring.
+        use_differentiable_astar: False runs `pq_astar`, see module docstring.
         mechanism (keyword-only): "moore" (default) or "news": the search's neighbourhood and heuristic, see
             DifferentiableAstar.
+        pq_semantics (keyword-only): "engine" (default) or "reference": which `pq_astar` runs when
+            use_differentiable_astar is False, see planner/pq_astar.py.
     """
 
     def __init__(self, g_ratio: float = 0.5, Tmax: float = 1.0, encoder_input: str = "m+", encoder_arch: str = "CNN",

@@ -34,3 +34,14 @@ mm = torch.rand(3, 1, 20, 27, device="cuda"); s1 = torch.zeros_like(mm); s1[:, :
 _native.conv1_marks(mm, s1, s1, rng.randn(9, 2, 32).astype(np.float32), rng.randn(32).astype(np.float32))
 torch.cuda.synchronize()
 print("glue ok")
+# the reference heap A* (nastar_pq.cuh): shared-memory and global-workspace state, unreachable and start == goal maps
+for (H, W, B) in ((32, 32, 5), (1, 40, 3), (130, 120, 2), (41, 41, 6), (1, 2001, 3)):   # odd H*W: 8-byte slots
+    obst = (rng.rand(B, 1, H, W) > 0.2).astype(np.float32)
+    start = np.zeros_like(obst); goal = np.zeros_like(obst)
+    obst[:, 0, 0, 0] = obst[:, 0, -1, -1] = 1; start[:, 0, 0, 0] = 1; goal[:, 0, -1, -1] = 1
+    goal[1] = start[1]
+    obst[0, 0, :, W // 2] = 0
+    c, s, g, o = (torch.from_numpy(x).cuda() for x in (rng.rand(B, 1, H, W).astype(np.float32), start, goal, obst))
+    _native.pq_astar(c, s, g, o, 0.5)
+torch.cuda.synchronize()
+print("pq ok")
