@@ -21,9 +21,10 @@
 //     three ky taps are the same box at offsets of ky * Wp * 128 B (a multiple of the 1 KB swizzle atom), so each
 //     input byte is loaded 3 times per tile, not 9.
 //   * B operand: the 256 x 32 weight slice of one (ky, kx, chunk), 32 KB, also 128-B swizzled.
-//   * Warp roles: warpgroup 0 is the producer (one thread issues every TMA; setmaxnreg drops the group to 56
-//     registers), warpgroups 1 and 2 each own 64 pixels x 256 channels (m64n256k8, 128 fp32 accumulators per thread;
-//     setmaxnreg raises them to 208).  Rings: 2 A stages, 4 B stages, full/empty mbarriers.
+//   * Warp roles: warpgroup 0 is the producer (one thread issues every TMA; setmaxnreg drops the group to 48
+//     registers), warpgroups 1 and 2 each own 64 pixels x 256 channels (128 fp32 accumulators per thread, two
+//     m64n128k8 per k step, one per half of the output channels; setmaxnreg raises them to 192).  Rings: 2 A stages,
+//     4 B stages, full/empty mbarriers.
 //
 // Three properties of the flagship shape (B = 100, 32x32: M = 102 400, N = 256, K = 1 152, 800 tiles):
 //   * Weight traffic.  The 1.18 MB of weights stay in L2, but every tile streams all of them: 800 x 1.18 MB =
@@ -36,12 +37,18 @@
 //     them is split between the two CTAs of one cluster as two 64-pixel half tiles (one consumer warpgroup active
 //     each), so the last round costs about half a tile: 6.06 / 6.5 = 0.93 of ideal, against 6.06 / 7 = 0.87.
 //   * Co-residency with the search.  The step graph runs the search (astar_warp32_kernel<..., kFused=1>: one
-//     32-thread CTA per map, 72 registers, 17 840 B static shared memory) beside this kernel.  Launch budget:
-//     384 threads x 160 registers = 61 440 of 65 536, leaving 4 096 >= 2 304 for one search CTA; shared memory
-//     128 KB (B) + 2 x 24 KB (A at W = 32; 2 x 32 KB at W = 64) + 10.3 KB (bias, head) + barriers = 187 KB at
-//     W = 32 and 203 KB at W = 64, which leaves room for the search CTA's 17.4 KB (+1 KB reserved per CTA) in the
-//     228 KB of an SM.  setmaxnreg only moves registers inside the CTA's launch allocation (128 x 56 + 256 x 208 =
-//     60 416 <= 61 440); 0 spills under -Xptxas -v.
+//     32-thread CTA per map, 72 registers, 17 840 B static shared memory) beside this kernel.  Registers are
+//     budgeted per SM sub-partition, not per SM: each warp is allocated in one of the four 16 384-register files, and
+//     the 12 warps of a CTA put 3 in each.  At 144 registers that is 3 x 144 x 32 = 13 824, leaving 2 560 for a
+//     search warp of up to 80 registers; at 160 (61 440 of the SM's 65 536, which looks like room) it is 15 360,
+//     leaving 1 024, and a CTA of this kernel cannot start on an SM that still runs a search CTA (on an H100 the
+//     pair then costs conv + search instead of about the longer of the two, tools/residency_probe.py).  ptxas needs
+//     154 launch registers for an m64n256k8 with fp32 accumulators whatever setmaxnreg grants later, hence the two
+//     m64n128k8: each output element is still one k8 step at a time in the same order.  setmaxnreg only moves
+//     registers inside the CTA's launch allocation (128 x 48 + 256 x 192 = 55 296 = 384 x 144); 0 spills under
+//     -Xptxas -v.  Shared memory: 128 KB (B) + 2 x 24 KB (A at W = 32; 2 x 32 KB at W = 64) + 10.3 KB (bias, head)
+//     + barriers = 187 KB at W = 32 and 203 KB at W = 64, which leaves room for the search CTA's 17.4 KB (+1 KB
+//     reserved per CTA) in the 228 KB of an SM.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -66,11 +73,19 @@ constexpr int kCHChunks = kCHCin / kCHChunk;
 constexpr uint32_t kCHBStageBytes = kCHCout * kCHChunk * 4;          // 32 KB
 constexpr uint32_t kCHBSliceRows = kCHCout / kCHCluster;             // output channels each CTA loads
 constexpr uint32_t kCHBSliceBytes = kCHBStageBytes / kCHCluster;
-constexpr int kCHProducerRegs = 56;
-constexpr int kCHConsumerRegs = 208;
+constexpr uint32_t kCHBHalfBytes = kCHBStageBytes / 2;           // output channels 128..255 of a stage
+constexpr int kCHLaunchRegs = 144;         // __maxnreg__ of the launch: see the co-residency budget above
+constexpr int kCHProducerRegs = 48;
+constexpr int kCHConsumerRegs = 192;
 constexpr int kCHMaxSide = 64;
+constexpr int kCHSearchRegs = 80;          // the largest search warp that must fit beside a CTA on every sub-partition
 static_assert(kCHCluster == 2, "the tail split gives each CTA of a cluster one half tile");
-static_assert(128 * kCHProducerRegs + 256 * kCHConsumerRegs <= kCHThreads * 160, "setmaxnreg exceeds the launch budget");
+static_assert(128 * kCHProducerRegs + 256 * kCHConsumerRegs <= kCHThreads * kCHLaunchRegs,
+              "setmaxnreg exceeds the launch budget");
+// a warp's registers come from one SM sub-partition's 16 384-register file, and a CTA's warps are spread evenly
+// over the 4 sub-partitions: each must keep room for one search warp next to its share of this CTA
+static_assert(kCHThreads / 32 / 4 * kCHLaunchRegs * 32 + kCHSearchRegs * 32 <= 16384,
+              "no room for a search warp on an SM sub-partition");
 
 struct ConvHeadWeights {   // the head's folded [C][9] weights, passed by value (constant bank)
     float w[kCHCout * 9];
@@ -157,36 +172,29 @@ __device__ __forceinline__ void ch_wgmma_wait() {
 }
 __device__ __forceinline__ void ch_fence_operand(float& x) { asm volatile("" : "+f"(x)::"memory"); }
 
-// d[64 x 256] (+)= A[64 x 8] * B[8 x 256]^T, TF32 in, fp32 accumulate; scale_d = 0 overwrites d
-__device__ __forceinline__ void ch_wgmma_m64n256k8(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+// d[64 x 128] (+)= A[64 x 8] * B[8 x 128]^T, TF32 in, fp32 accumulate; scale_d = 0 overwrites d.  The accumulators
+// are d[O .. O + 63] of the m64n256 fragment: O = 64 holds output channels 128..255 when B starts 128 rows further.
+template <int O>
+__device__ __forceinline__ void ch_wgmma_m64n128k8(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+    static_assert(O == 0 || O == 64, "one of the two channel halves");
     asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
         "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
         "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
         "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
-        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
-        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111,"
-        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
-        "}, %128, %129, p, 1, 1;\n}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1;\n}\n"
+        : "+f"(d[O + 0]), "+f"(d[O + 1]), "+f"(d[O + 2]), "+f"(d[O + 3]), "+f"(d[O + 4]), "+f"(d[O + 5]), "+f"(d[O + 6]),
+          "+f"(d[O + 7]), "+f"(d[O + 8]), "+f"(d[O + 9]), "+f"(d[O + 10]), "+f"(d[O + 11]), "+f"(d[O + 12]), "+f"(d[O + 13]),
+          "+f"(d[O + 14]), "+f"(d[O + 15]), "+f"(d[O + 16]), "+f"(d[O + 17]), "+f"(d[O + 18]), "+f"(d[O + 19]), "+f"(d[O + 20]),
+          "+f"(d[O + 21]), "+f"(d[O + 22]), "+f"(d[O + 23]), "+f"(d[O + 24]), "+f"(d[O + 25]), "+f"(d[O + 26]), "+f"(d[O + 27]),
+          "+f"(d[O + 28]), "+f"(d[O + 29]), "+f"(d[O + 30]), "+f"(d[O + 31]), "+f"(d[O + 32]), "+f"(d[O + 33]), "+f"(d[O + 34]),
+          "+f"(d[O + 35]), "+f"(d[O + 36]), "+f"(d[O + 37]), "+f"(d[O + 38]), "+f"(d[O + 39]), "+f"(d[O + 40]), "+f"(d[O + 41]),
+          "+f"(d[O + 42]), "+f"(d[O + 43]), "+f"(d[O + 44]), "+f"(d[O + 45]), "+f"(d[O + 46]), "+f"(d[O + 47]), "+f"(d[O + 48]),
+          "+f"(d[O + 49]), "+f"(d[O + 50]), "+f"(d[O + 51]), "+f"(d[O + 52]), "+f"(d[O + 53]), "+f"(d[O + 54]), "+f"(d[O + 55]),
+          "+f"(d[O + 56]), "+f"(d[O + 57]), "+f"(d[O + 58]), "+f"(d[O + 59]), "+f"(d[O + 60]), "+f"(d[O + 61]), "+f"(d[O + 62]),
+          "+f"(d[O + 63])
         : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
 
@@ -218,11 +226,13 @@ __device__ __forceinline__ ConvHeadTile ch_tile(const ConvHeadArgs& a, int i, in
     return t;
 }
 
-__global__ void __cluster_dims__(kCHCluster, 1, 1) __maxnreg__(160)
+__global__ void __cluster_dims__(kCHCluster, 1, 1) __maxnreg__(kCHLaunchRegs)
 conv3x3_head_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
                     const __grid_constant__ ConvHeadArgs a, const __grid_constant__ ConvHeadWeights hw) {
     extern __shared__ unsigned char ch_smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(ch_smem_raw) + 1023) & ~uintptr_t(1023));
+    // offset from the __shared__ array itself (not through an integer), so the compiler keeps the shared address
+    // space and the epilogue's bias and head-weight reads are LDS instead of generic loads
+    unsigned char* smem = ch_smem_raw + ((1024u - (smem_u32(ch_smem_raw) & 1023u)) & 1023u);
     const ConvHeadLayout L(a.a_bytes);
     unsigned char* sB = smem;
     unsigned char* sA = smem + L.a_off();
@@ -317,9 +327,12 @@ conv3x3_head_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
                             const uint32_t first = (kx | ch | ky) == 0;
                             ch_wgmma_fence();
 #pragma unroll
-                            for (int kk = 0; kk < kCHChunk / 8; ++kk)
-                                ch_wgmma_m64n256k8(d, ch_desc(ab + kk * 32), ch_desc(bb + kk * 32),
-                                                   (first && kk == 0) ? 0u : 1u);
+                            for (int kk = 0; kk < kCHChunk / 8; ++kk) {
+                                const uint32_t scale = (first && kk == 0) ? 0u : 1u;
+                                ch_wgmma_m64n128k8<0>(d, ch_desc(ab + kk * 32), ch_desc(bb + kk * 32), scale);
+                                ch_wgmma_m64n128k8<64>(d, ch_desc(ab + kk * 32), ch_desc(bb + kCHBHalfBytes + kk * 32),
+                                                       scale);
+                            }
                             ch_wgmma_commit();
                             ch_wgmma_wait<1>();
                         }
@@ -342,13 +355,22 @@ conv3x3_head_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
             for (int k = 0; k < 9; ++k) t0[k] = t1[k] = 0.f;
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
+                // channels cc0 and cc0 + 1 (cc0 even): their 2 biases and 18 head weights are 8-byte aligned pairs
+                const int cc0 = 8 * j + 2 * q;
+                const float2 bias2 = *reinterpret_cast<const float2*>(s_bias + cc0);
+                float w2[18];
+#pragma unroll
+                for (int i = 0; i < 9; ++i) {
+                    const float2 v = reinterpret_cast<const float2*>(s_head + cc0 * 9)[i];
+                    w2[2 * i] = v.x;
+                    w2[2 * i + 1] = v.y;
+                }
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const int cc = 8 * j + 2 * q + e;
-                    const float bc = s_bias[cc];
+                    const float bc = e ? bias2.y : bias2.x;
                     const float v0 = fmaxf(d[4 * j + e] + bc, 0.f);
                     const float v1 = fmaxf(d[4 * j + 2 + e] + bc, 0.f);
-                    const float* wc = s_head + cc * 9;
+                    const float* wc = w2 + 9 * e;
 #pragma unroll
                     for (int k = 0; k < 9; ++k) {
                         const float wk = wc[k];

@@ -214,20 +214,23 @@ class PipelinedPlanner:
     so both PCIe copies (1.2 MB each way per batch of 100 32x32 maps) hide behind the convolutions.  Batch k's results
     are complete once submit() number k+2 (or drain()) has finished.
 
-    `fork` places the search inside the step: "early" (default) at the start of the step, "late" right before the
-    encoder's last, widest convolution.  Measured on an H100 SXM at 700 W (tools/pipe_breakdown.py, b=100, 32x32): the
-    encoder branch alone takes 321 us and the search branch 93 us; the device step takes 359 us forked early and
-    408 us forked late, the three-stage host step 354 us early and 409 us late (H100 80GB HBM3 at a 400 W power limit,
-    conv4 and the head fused into one TF32 wgmma kernel; the previous cuDNN conv4 + head took 295 us of the branch).
+    `fork` places the search inside the step: "late" right before the encoder's last, widest convolution (the default
+    of the device pipeline), "early" at the start of the step (the default of host=True).  Late puts the search
+    beside the fused conv4 + head kernel, whose CTAs leave room for one search warp on every SM sub-partition.  Measured on an H100 80GB HBM3 at a 700 W power limit
+    (tools/pipe_breakdown.py, b=100, 32x32): the encoder branch alone takes 281 us and the search branch 76 us; the
+    device step takes 298 us forked late and 306 us forked early, the three-stage host step 314 us late and 305 us
+    early.  Before the fused kernel left that room, late cost 360 us against 314 us early on the same card.
     """
 
     def __init__(self, planner: torch.nn.Module, map_designs: torch.Tensor, start_maps: torch.Tensor,
-                 goal_maps: torch.Tensor, host: bool = False, warmup: int = 3, fork: str = "early"):
+                 goal_maps: torch.Tensor, host: bool = False, warmup: int = 3, fork: Optional[str] = None):
         from ..planner.astar import NeuralAstar
 
         if not isinstance(planner, NeuralAstar):
             raise TypeError("PipelinedPlanner overlaps an encoder with the search: it needs a NeuralAstar")
         dev = _check_planner(planner, map_designs)
+        if fork is None:
+            fork = "early" if host else "late"
         if fork not in ("late", "early"):
             raise ValueError("fork must be 'late' or 'early'")
         self.planner, self.device, self.host, self.fork = planner, dev, host, fork
