@@ -441,6 +441,38 @@ int nastar_b200_pq_astar(const float *cost, int64_t cost_stride, const float *st
  * with B.  0 for shapes that nastar_b200_pq_astar rejects. */
 size_t nastar_b200_pq_astar_workspace_bytes(int32_t B, int32_t H, int32_t W);
 
+/* One member of a nastar_b200_deflate batch.  Pointers are device addresses; lengths are in bytes. */
+typedef struct nastar_deflate_desc {
+    const uint8_t *head; /* compressed as the member's first chunk (the .npy header); may be NULL when head_len is 0 */
+    int64_t head_len;    /* at most one chunk, 262144 bytes */
+    const uint8_t *data; /* compressed as the member's next ceil(data_len / 262144) chunks; NULL when data_len is 0 */
+    int64_t data_len;
+    int64_t gap;         /* bytes left untouched in `out` before the member's stream (room for a zip local header) */
+    int64_t chunk0;      /* the member's first chunk: the sum of 1 + ceil(data_len / 262144) over earlier members */
+} nastar_deflate_desc;
+
+/* Raw deflate streams of M members, byte-equal to oracle/deflate_oracle.c (DESIGN.md §18).  Each member is cut into
+ * 256 KiB chunks (its head first, as one chunk of its own), each compressed alone into one dynamic-Huffman block or
+ * stored blocks; chunks other than a member's last end with an empty stored block, and the streams are written back
+ * to back into `out`, member m at out_off[m] (its gap before it), out_len[m] bytes.  crc[m] is the CRC-32 of the
+ * member's raw head || data.  desc: the descriptors in HOST memory, read for the checks; desc_dev: the same M
+ * descriptors in device memory, read by the kernel.  Every check precedes the launch: null pointers, M <= 0, a
+ * negative length or gap, a head_len above 262144, a chunk0 that is not the running chunk count, or an output array
+ * or the workspace overlapping another of them or an input give NASTAR_EINVAL; out_bytes below nastar_b200_deflate_bound or a workspace below
+ * nastar_b200_deflate_workspace_bytes gives NASTAR_EWORKSPACE.  One kernel launch (persistent CTAs, one workspace
+ * slot each).  Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_deflate(const nastar_deflate_desc *desc, const nastar_deflate_desc *desc_dev, int32_t M, uint8_t *out,
+                        int64_t out_bytes, int64_t *out_off, int64_t *out_len, uint32_t *crc, void *workspace,
+                        size_t workspace_bytes, void *stream);
+
+/* The bytes nastar_b200_deflate may write to `out` for these M host descriptors (gaps included), the worst case of
+ * every chunk, as zlib's deflateBound; -1 for descriptors that nastar_b200_deflate rejects with NASTAR_EINVAL. */
+int64_t nastar_b200_deflate_bound(const nastar_deflate_desc *desc, int32_t M);
+
+/* Workspace of nastar_b200_deflate: a chunk counter, a publication ring and one 2.6 MB slot per persistent CTA (one
+ * per SM at most), so it grows with the SMs, not with the input.  0 for descriptors it rejects. */
+size_t nastar_b200_deflate_workspace_bytes(const nastar_deflate_desc *desc, int32_t M);
+
 /* Number of kernel launches issued by this library since load (bench.py's gpu_launches). */
 uint64_t nastar_b200_launch_count(void);
 

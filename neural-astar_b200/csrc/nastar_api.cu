@@ -11,6 +11,7 @@
 #include "../../include/nastar_b200.h"
 #include "nastar_bin16.cuh"
 #include "nastar_convhead.cuh"
+#include "nastar_deflate.cuh"
 #include "nastar_generic.cuh"
 #include "nastar_glue.cuh"
 #include "nastar_goals.cuh"
@@ -339,6 +340,27 @@ int png_check(const nastar_png_desc* desc, int32_t B, int64_t data_bytes, int64_
 }
 
 size_t png_slot_bytes(int64_t max_raw) { return round256(size_t(max_raw)); }
+
+// ---- deflate (nastar_deflate.cuh) -----------------------------------------------------------------------------
+// the bytes nastar_b200_deflate may write (gaps included) and *chunks, or -1 for descriptors it rejects as EINVAL
+int64_t deflate_check(const nastar_deflate_desc* desc, int32_t M, int64_t* chunks) {
+    if (!desc || M <= 0) return -1;
+    int64_t bound = 0, k = 0;
+    for (int32_t i = 0; i < M; ++i) {
+        const nastar_deflate_desc& d = desc[i];
+        if (d.head_len < 0 || d.head_len > nastar::kDeflateChunk || d.data_len < 0 || d.gap < 0 || d.chunk0 != k)
+            return -1;   // the head is one chunk: the slot's buffers hold kDeflateChunk positions
+        if ((d.head_len > 0 && !d.head) || (d.data_len > 0 && !d.data)) return -1;
+        bound += d.gap + nastar::deflate_member_bound(d.head_len, d.data_len);
+        k += nastar::deflate_member_chunks(d.data_len);
+    }
+    *chunks = k;
+    return bound;
+}
+
+constexpr size_t kDeflateCtl = 256 + nastar::kDeflateRing * sizeof(nastar::DeflatePub);   // counter, ring
+
+int deflate_grid(int64_t chunks) { return capped_grid(chunks, 1); }
 
 // ---- heap A* (nastar_pq.cuh) ----------------------------------------------------------------------------------
 // Maps whose 20 B/cell state fits in this many bytes keep it in shared memory, larger ones in a global slot per CTA
@@ -792,6 +814,57 @@ int nastar_b200_decode_png(const uint8_t* data, int64_t data_bytes, const nastar
     if (e != cudaSuccess) return cuda_fail(e);
     const nastar::PngArgs a{data, desc_dev, B, out, status, reinterpret_cast<int32_t*>(ws), ws + 256, int64_t(slot)};
     nastar::decode_png_kernel<<<grid, nastar::kPngThreads, 0, stream>>>(a);
+    return launched();
+}
+
+int64_t nastar_b200_deflate_bound(const nastar_deflate_desc* desc, int32_t M) {
+    int64_t chunks = 0;
+    return deflate_check(desc, M, &chunks);
+}
+
+size_t nastar_b200_deflate_workspace_bytes(const nastar_deflate_desc* desc, int32_t M) {
+    int64_t chunks = 0;
+    if (deflate_check(desc, M, &chunks) < 0) return 0;
+    return kDeflateCtl + size_t(deflate_grid(chunks)) * size_t(nastar::kDeflateSlotBytes);
+}
+
+int nastar_b200_deflate(const nastar_deflate_desc* desc, const nastar_deflate_desc* desc_dev, int32_t M, uint8_t* out,
+                        int64_t out_bytes, int64_t* out_off, int64_t* out_len, uint32_t* crc, void* workspace,
+                        size_t workspace_bytes, void* stream_v) {
+    if (!desc_dev || !out || !out_off || !out_len || !crc || out_bytes < 0) return NASTAR_EINVAL;
+    int64_t chunks = 0;
+    const int64_t bound = deflate_check(desc, M, &chunks);
+    if (bound < 0) return NASTAR_EINVAL;
+    // the four outputs and the inputs: no two of the ranges may overlap
+    auto apart = [](const void* a, int64_t na, const void* b, int64_t nb) {
+        const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+        return na <= 0 || nb <= 0 || x + uint64_t(na) <= y || y + uint64_t(nb) <= x;
+    };
+    const int grid = deflate_grid(chunks);
+    const size_t ws_need = kDeflateCtl + size_t(grid) * size_t(nastar::kDeflateSlotBytes);
+    const void* outs[5] = {out, out_off, out_len, crc, workspace};
+    const int64_t lens[5] = {out_bytes, int64_t(M) * 8, int64_t(M) * 8, int64_t(M) * 4,
+                             int64_t(!workspace ? 0 : workspace_bytes < ws_need ? workspace_bytes : ws_need)};
+    for (int i = 0; i < 5; ++i) {
+        for (int j = i + 1; j < 5; ++j)
+            if (!apart(outs[i], lens[i], outs[j], lens[j])) return NASTAR_EINVAL;
+        if (!apart(outs[i], lens[i], desc_dev, int64_t(M) * int64_t(sizeof(nastar_deflate_desc)))) return NASTAR_EINVAL;
+        for (int32_t m = 0; m < M; ++m)
+            if (!apart(outs[i], lens[i], desc[m].head, desc[m].head_len) ||
+                !apart(outs[i], lens[i], desc[m].data, desc[m].data_len))
+                return NASTAR_EINVAL;
+    }
+    if (out_bytes < bound) return NASTAR_EWORKSPACE;
+    if (!workspace || workspace_bytes < ws_need) return NASTAR_EWORKSPACE;
+    if (reinterpret_cast<uintptr_t>(workspace) & 255) return NASTAR_EINVAL;   // the slots' u32 words
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+    unsigned char* ws = static_cast<unsigned char*>(workspace);
+    cudaError_t e = cudaMemsetAsync(ws, 0, kDeflateCtl, stream);   // the chunk counter and the ring's tags
+    if (e != cudaSuccess) return cuda_fail(e);
+    const nastar::DeflateArgs a{desc_dev, M, chunks, out, out_off, out_len, crc, reinterpret_cast<int32_t*>(ws),
+                                reinterpret_cast<nastar::DeflatePub*>(ws + 256), ws + kDeflateCtl};
+    e = launch_smem(nastar::deflate_kernel, grid, nastar::kDeflateThreads, sizeof(nastar::DeflateSmem), stream, a);
+    if (e != cudaSuccess) return cuda_fail(e);
     return launched();
 }
 

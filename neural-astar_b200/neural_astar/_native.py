@@ -95,6 +95,9 @@ _SIGNATURES = {
     "nastar_b200_pq_astar": (_int, [_p, _i64] * 4 + [_i32] * 3 + [ctypes.c_double] + [_p] * 5
                              + [ctypes.c_size_t, _p]),
     "nastar_b200_pq_astar_workspace_bytes": (ctypes.c_size_t, [_i32] * 3),
+    "nastar_b200_deflate": (_int, [_p, _p, _i32, _p, _i64, _p, _p, _p, _p, ctypes.c_size_t, _p]),
+    "nastar_b200_deflate_bound": (_i64, [_p, _i32]),
+    "nastar_b200_deflate_workspace_bytes": (ctypes.c_size_t, [_p, _i32]),
     "nastar_b200_launch_count": (ctypes.c_uint64, []),
     "nastar_b200_status_string": (ctypes.c_char_p, [_int]),
     "nastar_b200_last_cuda_error": (ctypes.c_char_p, []),
@@ -820,3 +823,45 @@ def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Te
         _check(L.nastar_b200_backward_mech(ctypes.byref(p), mech, stream), "nastar_b200_backward_mech")
     del keep
     return grad_cost
+
+
+# struct nastar_deflate_desc (include/nastar_b200.h) as a NumPy record
+DEFLATE_DESC_DTYPE = np.dtype([("head", "<u8"), ("head_len", "<i8"), ("data", "<u8"), ("data_len", "<i8"),
+                               ("gap", "<i8"), ("chunk0", "<i8")])
+DEFLATE_CHUNK = 256 * 1024   # nastar_deflate.cuh kDeflateChunk
+
+
+def deflate_chunk_counts(data_len) -> np.ndarray:
+    """Chunks of each member: its head, then ceil(data_len / DEFLATE_CHUNK)."""
+    n = np.asarray(data_len, dtype=np.int64)
+    return 1 + (n + DEFLATE_CHUNK - 1) // DEFLATE_CHUNK
+
+
+def deflate(desc, desc_dev: torch.Tensor):
+    """Raw deflate streams of the members in one kernel (include/nastar_b200.h, nastar_b200_deflate).
+
+    desc: a NumPy array of DEFLATE_DESC_DTYPE (the host copy, checked before the launch; head / data are device
+    addresses); desc_dev: the same descriptors' bytes in device memory (a uint8 CUDA tensor).  Returns (out uint8
+    [bound], out_off int64 [M], out_len int64 [M], crc int32 [M] (the CRC-32's bits)) on the current stream; nothing
+    is read back."""
+    L = lib()
+    d = np.ascontiguousarray(desc, dtype=DEFLATE_DESC_DTYPE)
+    if not isinstance(desc_dev, torch.Tensor) or not desc_dev.is_cuda:
+        raise RuntimeError("deflate: desc_dev must be a CUDA tensor (there is no CPU fallback)")
+    if desc_dev.dtype != torch.uint8 or not desc_dev.is_contiguous() or desc_dev.numel() != d.nbytes:
+        raise ValueError(f"deflate: desc_dev must be {d.nbytes} contiguous uint8 bytes")
+    bound = int(L.nastar_b200_deflate_bound(d.ctypes.data, len(d)))
+    if bound < 0:
+        raise ValueError("deflate: invalid descriptors")
+    dev = desc_dev.device
+    ws_bytes = int(L.nastar_b200_deflate_workspace_bytes(d.ctypes.data, len(d)))
+    with _on_device(dev) as stream:
+        out = torch.empty((max(bound, 1),), dtype=torch.uint8, device=dev)
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        out_off = torch.empty((len(d),), dtype=torch.int64, device=dev)
+        out_len = torch.empty((len(d),), dtype=torch.int64, device=dev)
+        crc = torch.empty((len(d),), dtype=torch.int32, device=dev)
+        _check(L.nastar_b200_deflate(d.ctypes.data, desc_dev.data_ptr(), len(d), out.data_ptr(), bound,
+                                     out_off.data_ptr(), out_len.data_ptr(), crc.data_ptr(), ws.data_ptr(), ws_bytes,
+                                     stream), "nastar_b200_deflate")
+    return out, out_off, out_len, crc

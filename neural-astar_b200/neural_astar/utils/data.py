@@ -9,6 +9,8 @@ and the WarCraft `.npy` pairs (:273-282).
 """
 from __future__ import annotations
 
+import os
+
 import numpy as np
 import torch
 import torch.utils.data as data
@@ -773,14 +775,139 @@ def _np(x) -> np.ndarray:
     return x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
 
 
+_ZIP_DOS_DATE = (0 << 9) | (1 << 5) | 1   # 1980-01-01 00:00:00: archives do not depend on the write time
+_U32 = 0xFFFFFFFF
+
+
+def _npy_header(dtype: np.dtype, shape) -> bytes:
+    """The header np.save writes for a C-order array of this dtype and shape (format 1.0, or 2.0 when it must)."""
+    import io
+
+    d = {"descr": np.lib.format.dtype_to_descr(dtype), "fortran_order": False, "shape": tuple(int(s) for s in shape)}
+    buf = io.BytesIO()
+    try:
+        np.lib.format.write_array_header_1_0(buf, d)
+    except ValueError:
+        buf = io.BytesIO()
+        np.lib.format.write_array_header_2_0(buf, d)
+    return buf.getvalue()
+
+
+def _zip_local_header_bytes(name: bytes) -> int:
+    return 30 + len(name) + 20
+
+
+def _zip_finish(image, names, offs, csizes, usizes, crcs, force_zip64: bool = False) -> bytes:
+    """Write each member's local header (ZIP64 extra with both sizes, as np.savez writes them) into `image` just
+    before its stream at offs[i], and return the central directory, ZIP64 end records where needed, and the end
+    record, which follow image's bytes in the file.  Timestamps are fixed; members are stored with method 8."""
+    import struct
+
+    cd = []
+    for name, off, cs, us, crc in zip(names, offs, csizes, usizes, crcs):
+        lh = off - _zip_local_header_bytes(name)
+        image[lh:off] = np.frombuffer(
+            struct.pack("<IHHHHHIIIHH", 0x04034B50, 45, 0, 8, 0, _ZIP_DOS_DATE, crc, _U32, _U32, len(name), 20) + name
+            + struct.pack("<HHQQ", 1, 16, us, cs), np.uint8)
+        ext = [v for v in (us, cs, lh) if force_zip64 or v >= _U32]
+        extra = struct.pack("<HH", 1, 8 * len(ext)) + struct.pack(f"<{len(ext)}Q", *ext) if ext else b""
+        big = force_zip64 or us >= _U32, force_zip64 or cs >= _U32, force_zip64 or lh >= _U32
+        cd.append(struct.pack("<IHHHHHHIIIHHHHHII", 0x02014B50, 45 | (3 << 8), 45, 0, 8, 0, _ZIP_DOS_DATE, crc,
+                              _U32 if big[1] else cs, _U32 if big[0] else us, len(name), len(extra), 0, 0, 0,
+                              0o600 << 16, _U32 if big[2] else lh) + name + extra)
+    cd = b"".join(cd)
+    cd_off, n = len(image), len(names)
+    tail = b""
+    if force_zip64 or n > 0xFFFF or cd_off >= _U32 or len(cd) >= _U32:
+        z64 = cd_off + len(cd)
+        tail = (struct.pack("<IQHHIIQQQQ", 0x06064B50, 44, 45, 45, 0, 0, n, n, len(cd), cd_off)
+                + struct.pack("<IIQI", 0x07064B50, 0, z64, 1))
+        eocd = struct.pack("<IHHHHIIH", 0x06054B50, 0, 0, 0xFFFF, 0xFFFF, _U32, _U32, 0)
+    else:
+        eocd = struct.pack("<IHHHHIIH", 0x06054B50, 0, 0, n, n, len(cd), cd_off, 0)
+    return cd + tail + eocd
+
+
+def savez_compressed_device(file, *args, **kwds) -> None:
+    """np.savez_compressed for CUDA tensors: members arr_0.npy, ... for positional arrays and <name>.npy for keywords,
+    each inflating to the bytes np.save writes for tensor.cpu().numpy().  The members are deflated on the device in one
+    kernel launch (include/nastar_b200.h, nastar_b200_deflate; DESIGN.md §18) with the CRC-32 of their raw bytes;
+    only the compressed bytes are copied to the host, and the archive (fixed timestamps, ZIP64 where needed) is
+    written at once.  `file`: a path (".npz" is appended when missing, as numpy does) or a writable binary file.
+    Non-CUDA arguments raise RuntimeError: there is no CPU fallback."""
+    members = {}
+    for i, a in enumerate(args):
+        members[f"arr_{i}"] = a
+    for k, a in kwds.items():
+        if k in members:
+            raise ValueError(f"Cannot use un-named variables and keyword {k}")
+        members[k] = a
+    if not members:
+        raise ValueError("savez_compressed_device: nothing to save")
+    tensors = list(members.values())
+    if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in tensors):
+        raise RuntimeError("savez_compressed_device: every array must be a CUDA tensor (there is no CPU fallback)")
+    dev = tensors[0].device
+    if any(t.device != dev for t in tensors):
+        raise ValueError("savez_compressed_device: every tensor must be on one device")
+    names = [(k + ".npy").encode() for k in members]
+    flat = [t.detach().contiguous().reshape(-1) for t in tensors]
+    heads = [_npy_header(torch.empty(0, dtype=t.dtype).numpy().dtype, t.shape) for t in tensors]
+    data = [f.view(torch.uint8) if f.numel() else f for f in flat]
+    M = len(tensors)
+    desc = np.zeros(M, _native.DEFLATE_DESC_DTYPE)
+    hlen = np.array([len(h) for h in heads], np.int64)
+    dlen = np.array([f.numel() * f.element_size() for f in flat], np.int64)
+    hoff = np.concatenate([[0], np.cumsum(hlen)])
+    ctl = torch.empty((int(hoff[-1]) + desc.nbytes,), dtype=torch.uint8, pin_memory=True)
+    ctl_dev = torch.empty((ctl.numel(),), dtype=torch.uint8, device=dev)
+    desc["head"] = ctl_dev.data_ptr() + hoff[:-1]
+    desc["head_len"] = hlen
+    desc["data"] = [d.data_ptr() if n else 0 for d, n in zip(data, dlen)]
+    desc["data_len"] = dlen
+    desc["gap"] = [_zip_local_header_bytes(n) for n in names]
+    desc["chunk0"] = np.concatenate([[0], np.cumsum(_native.deflate_chunk_counts(dlen))[:-1]])
+    c = ctl.numpy()
+    c[:hoff[-1]] = np.frombuffer(b"".join(heads), np.uint8)
+    c[hoff[-1]:] = desc.view(np.uint8)
+    with torch.cuda.device(dev):
+        ctl_dev.copy_(ctl, non_blocking=True)
+        out, out_off, out_len, crc = _native.deflate(desc, ctl_dev[int(hoff[-1]):])
+        meta = torch.cat([out_off, out_len, crc.to(torch.int64) & _U32]).to("cpu", non_blocking=True)
+        torch.cuda.current_stream(dev).synchronize()   # the compressed sizes and CRCs
+        meta = meta.numpy().reshape(3, M)
+        offs, csizes, crcs = meta[0].tolist(), meta[1].tolist(), meta[2].tolist()
+        end = offs[-1] + csizes[-1]
+        image = torch.empty((end,), dtype=torch.uint8, pin_memory=True)
+        image.copy_(out[:end], non_blocking=True)
+        torch.cuda.current_stream(dev).synchronize()   # exactly the compressed bytes, known only after the first wait
+    del flat, data, ctl
+    img = image.numpy()
+    tail = _zip_finish(img, names, offs, csizes, (hlen + dlen).tolist(), crcs)
+    if isinstance(file, (str, os.PathLike)):
+        file = os.fspath(file)
+        if not file.endswith(".npz"):
+            file += ".npz"
+        with open(file, "wb") as f:
+            f.write(memoryview(img))
+            f.write(tail)
+    else:
+        file.write(memoryview(img))
+        file.write(tail)
+
+
 def save_planning_dataset(path: str, train, valid, test) -> None:
     """Write a planning-datasets .npz (np.savez_compressed arr_0..arr_11, reference generate_spp_instances.py:48-62)
     that MazeDataset / create_dataloader read.  Each split is (maps [N,H,W] or [N,1,H,W], goal_maps [N,1,H,W],
     opt_policies [N,8,1,H,W] (moore) or [N,4,1,H,W] (news), opt_dists [N,1,H,W]), NumPy arrays or tensors; they are
-    stored in the dtype given."""
+    stored in the dtype given.  When all 12 arrays are CUDA tensors on one device, the file is compressed there
+    (savez_compressed_device); otherwise np.savez_compressed writes it.  np.load reads the same arrays either way."""
+    splits = [tuple(split) for split in (train, valid, test)]
+    flat = [x for split in splits for x in split]
+    device = all(isinstance(x, torch.Tensor) and x.is_cuda for x in flat) and len({x.device for x in flat}) == 1
     arrays = []
-    for name, split in (("train", train), ("valid", valid), ("test", test)):
-        maps, goals, policies, dists = (_np(x) for x in split)
+    for name, split in zip(("train", "valid", "test"), splits):
+        maps, goals, policies, dists = (x.detach() if device else _np(x) for x in split)
         if maps.ndim == 4:
             maps = maps[:, 0]
         N, H, W = maps.shape
@@ -789,11 +916,15 @@ def save_planning_dataset(path: str, train, valid, test) -> None:
             raise ValueError(f"{name}: expected maps [N,H,W], goals / dists [N,1,H,W], policies [N,8|4,1,H,W] "
                              f"(got {maps.shape}, {goals.shape}, {policies.shape}, {dists.shape})")
         arrays += [maps, goals, policies, dists]
-    np.savez_compressed(path, *arrays)
+    if device:
+        savez_compressed_device(path, *arrays)
+    else:
+        np.savez_compressed(path, *arrays)
 
 
 __all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "MazeDataset", "WarCraftDataset",
            "compute_opt_labels", "compute_weighted_opt_labels", "create_dataloader", "create_device_dataloader",
            "create_warcraft_dataloader", "draw_opt_policies", "load_map_images", "maps_from_images",
-           "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset", "save_warcraft_dataset",
+           "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset", "savez_compressed_device",
+           "save_warcraft_dataset",
            "shortest_path_maps", "tile_maps", "visualize_results"]

@@ -7,8 +7,9 @@ resize + Otsu, bit-equal to the generator) -> with --tile-size t > 1, split-size
 come from np.random.RandomState(seed).choice, as the generator draws them (its train tiles replay exactly; its
 validation and test tiles follow label draws and do not) -> sample_device_goal_maps (largest region, corner squares of
 int(edge_ratio * size * t)) -> compute_opt_labels + draw_opt_policies (a uniform member of each maximal action set) ->
-save_planning_dataset.  --mechanism moore (8 actions, the default) or news (4 actions, 4-connected distances) is the
-generator's transition mechanism; the goals are the same for both.  Goals and policies come from a CUDA
+save_planning_dataset, which deflates the twelve arrays on the GPU too (savez_compressed_device, DESIGN.md §18), so only
+the compressed file crosses to the host.  --mechanism moore (8 actions, the default) or news (4 actions, 4-connected
+distances) is the generator's transition mechanism; the goals are the same for both.  Goals and policies come from a CUDA
 torch.Generator seeded with --seed, so they are not the generator's random draws.  With --tile-size 1 the split sizes are ignored and every image is used, as there.
 
     python tools/make_planning_dataset.py --input-path data/mpd/original/mazes --output-path out --maze-size 32 \\
