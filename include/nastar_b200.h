@@ -473,6 +473,68 @@ int64_t nastar_b200_deflate_bound(const nastar_deflate_desc *desc, int32_t M);
  * per SM at most), so it grows with the SMs, not with the input.  0 for descriptors it rejects. */
 size_t nastar_b200_deflate_workspace_bytes(const nastar_deflate_desc *desc, int32_t M);
 
+/* Search animations (DESIGN.md §19): G GIFs over a search of B maps, layout NASTAR_GIF_EACH (one GIF per map, G = B)
+ * or NASTAR_GIF_GRID (one GIF of all maps in make_grid's layout: 8 per row, 2-pixel border, none for B = 1).  GIF g
+ * has T_g steps and T_g + 1 frames, numbered GIF by GIF: frame k < T_g is the closed set before step k and the cell
+ * selected at step k, frame T_g the histories and paths.  Planes are contiguous [B, H, W] (channel 0 of [B,1,H,W]). */
+#define NASTAR_GIF_EACH 0
+#define NASTAR_GIF_GRID 1
+#define NASTAR_GIF_STEPS_MAP 0     /* T_g from the map's t_solve (EACH) */
+#define NASTAR_GIF_STEPS_BATCH 1   /* T_g = the slowest map's steps, the reference loop's T_batch (GRID) */
+#define NASTAR_GIF_STEPS_ALL 2     /* T_g = T: a batch-coupled search that ran exactly T steps (GRID) */
+
+typedef struct nastar_gif_params {
+    const float *maps;        /* map designs, grey level uint8(v * 255) with v in [0, 1] */
+    const float *histories;   /* the search's outputs */
+    const int64_t *paths;
+    const float *goal_maps;   /* the goal is the first maximum */
+    const int32_t *trace;     /* [B, T]: the cell selected at each step (< H*W, the caller's guarantee: the search
+                               * kernels write it so); negative entries stand for the goal */
+    const int32_t *t_solve;   /* [B] */
+    int32_t B, H, W, T;
+    int32_t layout;           /* NASTAR_GIF_EACH or NASTAR_GIF_GRID */
+    int32_t steps_mode;       /* NASTAR_GIF_STEPS_* */
+    int32_t screen_w, screen_h;   /* the logical screen, each 1 .. 65535 */
+    int32_t delay_cs;         /* 0 .. 65535 */
+    /* device tables, back to back in this order: int32 xmap[screen_w] and ymap[screen_h] (screen column / row -> image
+     * column / row, nondecreasing), int32 xspan[Wi][2] and yspan[Hi][2] (image column / row -> its screen columns /
+     * rows [lo, hi)), uint8 lut[G][256] (grey level -> palette index) and uint8 colors[G][2] (number of greys n, LZW
+     * minimum code size m): palette indices 0 .. n-1 are the greys, n green, n+1 red, n+2 transparent.  Wi x Hi is the
+     * make_grid image. */
+    const void *tables;
+} nastar_gif_params;
+
+/* Bytes of the tables of nastar_gif_params for these shapes; -1 for parameters nastar_b200_gif_plan rejects. */
+int64_t nastar_b200_gif_tables_bytes(const nastar_gif_params *p);
+
+/* First of the two launches: writes steps[G] (T_g) and nbytes[G * (T + 1)] (for frame f < sum(T_g + 1): the bytes of
+ * its LZW stream).  Every check precedes the launch: null pointers, B, H, W or T below 1, an unknown layout or
+ * steps_mode (STEPS_MAP with GRID, BATCH or ALL with EACH), a screen side outside 1 .. 65535 or delay_cs outside
+ * 0 .. 65535 give NASTAR_EINVAL (the tables' contents are the caller's); H * W above 2^24 gives NASTAR_EUNSUPPORTED; a workspace
+ * below nastar_b200_gif_workspace_bytes gives NASTAR_EWORKSPACE.  One kernel launch (persistent CTAs).  The same
+ * workspace, untouched, goes to nastar_b200_gif_encode.  Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_gif_plan(const nastar_gif_params *p, int32_t *steps, int32_t *nbytes, void *workspace,
+                         size_t workspace_bytes, void *stream);
+
+/* The bytes of one frame's record for an LZW stream of lzw_bytes: graphic control extension (8), image descriptor
+ * (10), minimum code size (1), the stream in sub-blocks of at most 255 bytes, terminator (1); -1 for lzw_bytes < 1. */
+int64_t nastar_b200_gif_record_bytes(int64_t lzw_bytes);
+
+/* Second launch: every frame's record, frame f at offset[f] of `out`.  p, nbytes and the workspace are those of the
+ * plan; nbytes_host and offset_host are the host copies of nbytes[0 .. n_frames) and offset[0 .. n_frames] that the
+ * checks read (offset_dev: the same offsets in device memory, read by the kernel).  Every check precedes the launch:
+ * the plan's checks, n_frames below 1 or above G * (T + 1), an offset that does not start at 0 or does not advance by
+ * nastar_b200_gif_record_bytes(nbytes[f]), or an out_bytes below offset[n_frames] give NASTAR_EINVAL.  n_frames must
+ * be the sum of T_g + 1 of the plan.  May run again on the same plan and workspace.  One kernel launch.  Asynchronous
+ * on `stream`.  Returns NASTAR_*. */
+int nastar_b200_gif_encode(const nastar_gif_params *p, const int32_t *nbytes, const int32_t *nbytes_host,
+                           const int64_t *offset_host, const int64_t *offset_dev, int64_t n_frames, uint8_t *out,
+                           int64_t out_bytes, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Workspace of the two GIF launches: a control block, per-map goals and first-selection tables (4*H*W bytes each) and
+ * per-frame rectangles (16 bytes each); 0 for parameters they reject. */
+size_t nastar_b200_gif_workspace_bytes(const nastar_gif_params *p);
+
 /* Number of kernel launches issued by this library since load (bench.py's gpu_launches). */
 uint64_t nastar_b200_launch_count(void);
 

@@ -13,6 +13,7 @@
 #include "nastar_convhead.cuh"
 #include "nastar_deflate.cuh"
 #include "nastar_generic.cuh"
+#include "nastar_gif.cuh"
 #include "nastar_glue.cuh"
 #include "nastar_goals.cuh"
 #include "nastar_labels.cuh"
@@ -361,6 +362,68 @@ int64_t deflate_check(const nastar_deflate_desc* desc, int32_t M, int64_t* chunk
 constexpr size_t kDeflateCtl = 256 + nastar::kDeflateRing * sizeof(nastar::DeflatePub);   // counter, ring
 
 int deflate_grid(int64_t chunks) { return capped_grid(chunks, 1); }
+
+// ---- search GIFs (nastar_gif.cuh) ------------------------------------------------------------------------------
+struct GifShape {
+    int64_t G, Hi, Wi;   // GIFs, make_grid image
+    size_t ws_first, ws_rect, ws_bytes;
+};
+
+// the shapes of a GIF call, or false for parameters nastar_b200_gif_plan rejects with NASTAR_EINVAL
+bool gif_shape(const nastar_gif_params* p, GifShape* s) {
+    if (!p || !p->maps || !p->histories || !p->paths || !p->goal_maps || !p->trace || !p->t_solve || !p->tables)
+        return false;
+    if (p->B <= 0 || p->H <= 0 || p->W <= 0 || p->T <= 0) return false;
+    if (p->layout == NASTAR_GIF_EACH ? p->steps_mode != NASTAR_GIF_STEPS_MAP
+                                     : p->layout != NASTAR_GIF_GRID || (p->steps_mode != NASTAR_GIF_STEPS_BATCH &&
+                                                                        p->steps_mode != NASTAR_GIF_STEPS_ALL))
+        return false;
+    if (p->screen_w < 1 || p->screen_w > 65535 || p->screen_h < 1 || p->screen_h > 65535) return false;
+    if (p->delay_cs < 0 || p->delay_cs > 65535) return false;
+    const bool tiled = p->layout == NASTAR_GIF_GRID && p->B > 1;
+    const int64_t xmaps = p->B < 8 ? p->B : 8, ymaps = (p->B + xmaps - 1) / xmaps;
+    s->G = p->layout == NASTAR_GIF_GRID ? 1 : p->B;
+    s->Hi = tiled ? (p->H + 2) * ymaps + 2 : p->H;
+    s->Wi = tiled ? (p->W + 2) * xmaps + 2 : p->W;
+    const int64_t N = int64_t(p->H) * p->W;
+    s->ws_first = round256(size_t(p->B) * 4) + round256(size_t(p->B) * size_t(N) * 4);
+    s->ws_rect = round256(size_t(s->G) * size_t(p->T + 1) * 16);
+    s->ws_bytes = 256 + 2 * round256(size_t(s->G) * 4) + s->ws_first + s->ws_rect;
+    return true;
+}
+
+bool gif_supported(const nastar_gif_params* p) { return int64_t(p->H) * p->W <= (int64_t(1) << 24); }
+
+nastar::GifArgs gif_args(const nastar_gif_params* p, const GifShape& s, void* workspace, int32_t* nbytes) {
+    nastar::GifArgs a{};
+    a.maps = p->maps; a.hist = p->histories; a.paths = p->paths; a.goal = p->goal_maps;
+    a.trace = p->trace; a.t_solve = p->t_solve;
+    a.B = p->B; a.H = p->H; a.W = p->W; a.T = p->T;
+    a.grid = p->layout == NASTAR_GIF_GRID;
+    a.steps_mode = p->steps_mode;
+    a.Hg = int32_t(s.Hi); a.Wg = int32_t(s.Wi);
+    a.SW = p->screen_w; a.SH = p->screen_h;
+    const int32_t* t32 = static_cast<const int32_t*>(p->tables);
+    a.xmap = t32;
+    a.ymap = a.xmap + p->screen_w;
+    a.xspan = a.ymap + p->screen_h;
+    a.yspan = a.xspan + 2 * s.Wi;
+    a.lut = reinterpret_cast<const uint8_t*>(a.yspan + 2 * s.Hi);
+    a.ncolors = a.lut + 256 * s.G;
+    a.delay_cs = p->delay_cs;
+    unsigned char* ws = static_cast<unsigned char*>(workspace);
+    a.ctl = reinterpret_cast<nastar::GifCtl*>(ws);
+    size_t o = 256;
+    a.steps = reinterpret_cast<int32_t*>(ws + o);  o += round256(size_t(s.G) * 4);
+    a.frame0 = reinterpret_cast<int32_t*>(ws + o); o += round256(size_t(s.G) * 4);
+    a.goal_idx = reinterpret_cast<int32_t*>(ws + o); o += round256(size_t(p->B) * 4);
+    a.first = reinterpret_cast<int32_t*>(ws + o);  o += round256(size_t(p->B) * size_t(p->H) * size_t(p->W) * 4);
+    a.rect = reinterpret_cast<uint32_t*>(ws + o);
+    a.nbytes = nbytes;
+    return a;
+}
+
+int gif_grid(int64_t items) { return capped_grid(items, 1); }
 
 // ---- heap A* (nastar_pq.cuh) ----------------------------------------------------------------------------------
 // Maps whose 20 B/cell state fits in this many bytes keep it in shared memory, larger ones in a global slot per CTA
@@ -907,6 +970,73 @@ int nastar_b200_pq_astar(const float* cost, int64_t cost_stride, const float* st
     } else {
         nastar::pq_astar_kernel<false><<<ggrid, nastar::kPqThreads, 0, stream>>>(a);
     }
+    return launched();
+}
+
+int64_t nastar_b200_gif_tables_bytes(const nastar_gif_params* p) {
+    if (!p) return -1;
+    nastar_gif_params q = *p;   // the tables themselves need not exist yet
+    q.tables = &q;
+    GifShape s;
+    if (!gif_shape(&q, &s)) return -1;
+    return 4 * (int64_t(p->screen_w) + p->screen_h + 2 * s.Wi + 2 * s.Hi) + 258 * s.G;
+}
+
+size_t nastar_b200_gif_workspace_bytes(const nastar_gif_params* p) {
+    GifShape s;
+    if (!gif_shape(p, &s) || !gif_supported(p)) return 0;
+    return s.ws_bytes;
+}
+
+int64_t nastar_b200_gif_record_bytes(int64_t n) { return n < 1 ? -1 : 19 + n + (n + 254) / 255 + 1; }
+
+int nastar_b200_gif_plan(const nastar_gif_params* p, int32_t* steps, int32_t* nbytes, void* workspace,
+                         size_t workspace_bytes, void* stream_v) {
+    GifShape s;
+    if (!gif_shape(p, &s) || !steps || !nbytes) return NASTAR_EINVAL;
+    if (!gif_supported(p)) return NASTAR_EUNSUPPORTED;
+    if (!workspace || workspace_bytes < s.ws_bytes) return NASTAR_EWORKSPACE;
+    if (reinterpret_cast<uintptr_t>(workspace) & 255) return NASTAR_EINVAL;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+    nastar::GifArgs a = gif_args(p, s, workspace, nbytes);
+    cudaError_t e = cudaMemsetAsync(workspace, 0, 256, stream);   // counters
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.rect, 0xFF, s.ws_rect, stream);   // empty rectangles
+    if (e != cudaSuccess) return cuda_fail(e);
+    const int grid = gif_grid(p->B > 1024 ? p->B : 1024);
+    e = launch_smem(nastar::gif_plan_kernel, grid, nastar::kGifThreads, sizeof(nastar::GifWarpSmem) * nastar::kGifWarps,
+                    stream, a);
+    if (e != cudaSuccess) return cuda_fail(e);
+    const int st = launched();
+    if (st != NASTAR_OK) return st;
+    e = cudaMemcpyAsync(steps, a.steps, size_t(s.G) * 4, cudaMemcpyDeviceToDevice, stream);   // T_g, for the host
+    return e == cudaSuccess ? NASTAR_OK : cuda_fail(e);
+}
+
+int nastar_b200_gif_encode(const nastar_gif_params* p, const int32_t* nbytes, const int32_t* nbytes_host,
+                           const int64_t* offset_host, const int64_t* offset_dev, int64_t n_frames, uint8_t* out,
+                           int64_t out_bytes, void* workspace, size_t workspace_bytes, void* stream_v) {
+    GifShape s;
+    if (!gif_shape(p, &s) || !nbytes || !nbytes_host || !offset_host || !offset_dev || !out) return NASTAR_EINVAL;
+    if (n_frames < 1 || n_frames > s.G * (int64_t(p->T) + 1)) return NASTAR_EINVAL;
+    if (offset_host[0] != 0) return NASTAR_EINVAL;
+    for (int64_t f = 0; f < n_frames; ++f) {
+        const int64_t r = nastar_b200_gif_record_bytes(nbytes_host[f]);
+        if (r < 0 || offset_host[f + 1] != offset_host[f] + r) return NASTAR_EINVAL;
+    }
+    if (out_bytes < offset_host[n_frames]) return NASTAR_EINVAL;
+    if (!gif_supported(p)) return NASTAR_EUNSUPPORTED;
+    if (!workspace || workspace_bytes < s.ws_bytes) return NASTAR_EWORKSPACE;
+    if (reinterpret_cast<uintptr_t>(workspace) & 255) return NASTAR_EINVAL;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+    nastar::GifArgs a = gif_args(p, s, workspace, const_cast<int32_t*>(nbytes));
+    a.offset = offset_dev;
+    a.out = out;
+    // the encode's frame counter starts over, so the same plan can be encoded again
+    cudaError_t e = cudaMemsetAsync(&a.ctl->encode_next, 0, sizeof(int32_t), stream);
+    if (e != cudaSuccess) return cuda_fail(e);
+    e = launch_smem(nastar::gif_encode_kernel, gif_grid(n_frames), nastar::kGifThreads,
+                                      sizeof(nastar::GifWarpSmem) * nastar::kGifWarps, stream, a);
+    if (e != cudaSuccess) return cuda_fail(e);
     return launched();
 }
 

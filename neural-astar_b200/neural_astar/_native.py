@@ -60,6 +60,19 @@ class BwdParams(ctypes.Structure):
     ]
 
 
+class GifParams(ctypes.Structure):
+    """struct nastar_gif_params (include/nastar_b200.h)"""
+
+    _fields_ = [
+        ("maps", ctypes.c_void_p), ("histories", ctypes.c_void_p), ("paths", ctypes.c_void_p),
+        ("goal_maps", ctypes.c_void_p), ("trace", ctypes.c_void_p), ("t_solve", ctypes.c_void_p),
+        ("B", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32), ("T", ctypes.c_int32),
+        ("layout", ctypes.c_int32), ("steps_mode", ctypes.c_int32),
+        ("screen_w", ctypes.c_int32), ("screen_h", ctypes.c_int32), ("delay_cs", ctypes.c_int32),
+        ("tables", ctypes.c_void_p),
+    ]
+
+
 _p, _i32, _i64, _int = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_int
 
 # every entry point of include/nastar_b200.h: symbol -> (restype, argtypes)
@@ -98,6 +111,12 @@ _SIGNATURES = {
     "nastar_b200_deflate": (_int, [_p, _p, _i32, _p, _i64, _p, _p, _p, _p, ctypes.c_size_t, _p]),
     "nastar_b200_deflate_bound": (_i64, [_p, _i32]),
     "nastar_b200_deflate_workspace_bytes": (ctypes.c_size_t, [_p, _i32]),
+    "nastar_b200_gif_tables_bytes": (_i64, [ctypes.POINTER(GifParams)]),
+    "nastar_b200_gif_plan": (_int, [ctypes.POINTER(GifParams), _p, _p, _p, ctypes.c_size_t, _p]),
+    "nastar_b200_gif_record_bytes": (_i64, [_i64]),
+    "nastar_b200_gif_encode": (_int, [ctypes.POINTER(GifParams), _p, _p, _p, _p, _i64, _p, _i64, _p, ctypes.c_size_t,
+                                      _p]),
+    "nastar_b200_gif_workspace_bytes": (ctypes.c_size_t, [ctypes.POINTER(GifParams)]),
     "nastar_b200_launch_count": (ctypes.c_uint64, []),
     "nastar_b200_status_string": (ctypes.c_char_p, [_int]),
     "nastar_b200_last_cuda_error": (ctypes.c_char_p, []),
@@ -865,3 +884,70 @@ def deflate(desc, desc_dev: torch.Tensor):
                                      out_off.data_ptr(), out_len.data_ptr(), crc.data_ptr(), ws.data_ptr(), ws_bytes,
                                      stream), "nastar_b200_deflate")
     return out, out_off, out_len, crc
+
+
+# NASTAR_GIF_* (include/nastar_b200.h)
+GIF_EACH, GIF_GRID = 0, 1
+GIF_STEPS_MAP, GIF_STEPS_BATCH, GIF_STEPS_ALL = 0, 1, 2
+
+
+def gif_params(maps, hist, paths, goal, trace, t_solve, layout: int, steps_mode: int, screen_w: int, screen_h: int,
+               delay_cs: int):
+    """GifParams of a search's planes ([B,1,H,W] CUDA tensors: fp32 maps, histories and goals, int64 paths; trace
+    [B,T] and t_solve [B] int32), without the tables.  Returns (params, tensors to keep alive)."""
+    planes = [t.detach().contiguous() for t in (maps, hist, paths, goal, trace, t_solve)]
+    if any(not t.is_cuda or t.device != planes[0].device for t in planes):
+        raise RuntimeError("gif: every tensor must be on one CUDA device (there is no CPU fallback)")
+    dtypes = (torch.float32, torch.float32, torch.int64, torch.float32, torch.int32, torch.int32)
+    if any(t.dtype != d for t, d in zip(planes, dtypes)):
+        raise TypeError("gif: maps, histories, goals fp32; paths int64; trace and t_solve int32")
+    B, _, H, W = planes[0].shape
+    p = GifParams()
+    p.maps, p.histories, p.paths, p.goal_maps, p.trace, p.t_solve = (t.data_ptr() for t in planes)
+    p.B, p.H, p.W, p.T = B, H, W, planes[4].shape[1]
+    p.layout, p.steps_mode = layout, steps_mode
+    p.screen_w, p.screen_h, p.delay_cs = screen_w, screen_h, delay_cs
+    return p, planes
+
+
+def gif_tables_bytes(p: GifParams) -> int:
+    return int(lib().nastar_b200_gif_tables_bytes(ctypes.byref(p)))
+
+
+def gif_record_bytes(lzw_bytes) -> np.ndarray:
+    """nastar_b200_gif_record_bytes, vectorised: each frame's record around an LZW stream of lzw_bytes."""
+    n = np.asarray(lzw_bytes, dtype=np.int64)
+    return 19 + n + (n + 254) // 255 + 1
+
+
+def gif_plan(p: GifParams, dev: torch.device):
+    """The first GIF launch (nastar_b200_gif_plan).  p.tables must point at the device tables.  Returns (steps int32
+    [G], nbytes int32 [G*(T+1)], workspace) on the current stream; nothing is read back."""
+    L = lib()
+    G = 1 if p.layout == GIF_GRID else p.B
+    ws_bytes = int(L.nastar_b200_gif_workspace_bytes(ctypes.byref(p)))
+    with _on_device(dev) as stream:
+        steps = torch.empty((G,), dtype=torch.int32, device=dev)
+        nbytes = torch.empty((G * (p.T + 1),), dtype=torch.int32, device=dev)
+        ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
+        _check(L.nastar_b200_gif_plan(ctypes.byref(p), steps.data_ptr(), nbytes.data_ptr(), ws.data_ptr(), ws_bytes,
+                                      stream), "nastar_b200_gif_plan")
+    return steps, nbytes, ws
+
+
+def gif_encode(p: GifParams, nbytes: torch.Tensor, nbytes_host: np.ndarray, offset_host: np.ndarray,
+               offset_dev: torch.Tensor, ws: torch.Tensor) -> torch.Tensor:
+    """The second GIF launch (nastar_b200_gif_encode): every frame's record, frame f at offset_host[f].  Returns out
+    uint8 [offset_host[-1]] on the current stream."""
+    L = lib()
+    nb = np.ascontiguousarray(nbytes_host, dtype=np.int32)
+    off = np.ascontiguousarray(offset_host, dtype=np.int64)
+    if len(off) != len(nb) + 1 or offset_dev.dtype != torch.int64 or offset_dev.numel() != len(off):
+        raise ValueError("gif_encode: offsets are one more than the frames, int64")
+    dev = nbytes.device
+    with _on_device(dev) as stream:
+        out = torch.empty((max(int(off[-1]), 1),), dtype=torch.uint8, device=dev)
+        _check(L.nastar_b200_gif_encode(ctypes.byref(p), nbytes.data_ptr(), nb.ctypes.data, off.ctypes.data,
+                                        offset_dev.data_ptr(), len(nb), out.data_ptr(), int(off[-1]), ws.data_ptr(),
+                                        ws.numel(), stream), "nastar_b200_gif_encode")
+    return out

@@ -23,7 +23,7 @@ import torch.nn.functional as F
 
 from .. import _native
 from . import encoder as _encoders
-from .differentiable_astar import AstarOutput, DifferentiableAstar, TakesMechanism, _mech_kw
+from .differentiable_astar import AstarOutput, DifferentiableAstar, TakesMechanism, _mech_kw, batch_coupled
 from .pq_astar import _check_semantics, pq_astar  # noqa: F401  pq_astar re-exported, like the reference module does
 
 
@@ -189,7 +189,7 @@ class NeuralAstar(VanillaAstar):
         the host procedure of DifferentiableAstar.forward, while under capture search_from_taps couples the batch on
         the device)."""
         H, W = start_maps.shape[-2], start_maps.shape[-1]
-        coupled = float(self.g_ratio) < 0.5 and start_maps.shape[0] > 1
+        coupled = batch_coupled(self.g_ratio, start_maps.shape[0])
         if (not self.use_differentiable_astar or not self.encoder.fast_path_ok(map_designs) or H > 64 or W > 64
                 or not start_maps.is_cuda or (coupled and not torch.cuda.is_current_stream_capturing())
                 or start_maps.dtype != torch.float32 or passable.dtype != torch.float32):

@@ -10,6 +10,7 @@ second kernel evaluating the closed form of SURVEY.md App. B.
 """
 from __future__ import annotations
 
+import contextvars
 from typing import List, NamedTuple, Optional
 
 import torch
@@ -24,6 +25,29 @@ class AstarOutput(NamedTuple):
     histories: torch.Tensor
     paths: torch.Tensor
     intermediate_results: Optional[List[dict]] = None
+
+
+class SearchRecord(NamedTuple):
+    """What the frames of a search are made of, handed out in place of the frame list while `recording_search` is on:
+    T_batch is the batch-coupled step count, or None when the search exited per map."""
+
+    histories: torch.Tensor
+    paths: torch.Tensor
+    goal_maps: torch.Tensor
+    t_solve: torch.Tensor
+    trace: torch.Tensor
+    T: int
+    T_batch: Optional[int]
+
+
+# None: forward returns frames.  "batch": forward returns a SearchRecord of the search it runs.  "each": the same, and
+# the batch is never coupled, so each map's record is that of the map searched alone.  Set by utils.data.search_gifs.
+_recording = contextvars.ContextVar("recording_search", default=None)
+
+
+def batch_coupled(g_ratio: float, B: int) -> bool:
+    """Whether a batch of B maps is searched batch-coupled (the reference's loop, g_ratio < 0.5)."""
+    return float(g_ratio) < 0.5 and B > 1 and _recording.get() != "each"
 
 
 def get_heuristic(goal_maps: torch.Tensor, tb_factor: float = 0.001) -> torch.Tensor:
@@ -212,7 +236,7 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
         if T < 1:
             raise ValueError("Tmax * W * W < 1: the reference loop would not execute (:203)")
         g_ratio = float(self.g_ratio)
-        coupled = g_ratio < 0.5 and cost_maps.shape[0] > 1
+        coupled = batch_coupled(g_ratio, cost_maps.shape[0])
         goal_clamped = None
         if coupled and cost_maps.is_cuda and torch.cuda.is_current_stream_capturing():
             # under CUDA-graph capture the host decision below cannot happen: decide T_batch on the device instead
@@ -235,7 +259,9 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
             self.mechanism)
 
         intermediate_results: List[dict] = []
-        if store_intermediate_results:
+        if store_intermediate_results and _recording.get() is not None:
+            intermediate_results = SearchRecord(hist, paths, goal_maps, t_solve, trace, T, T if coupled else None)
+        elif store_intermediate_results:
             intermediate_results = _materialise_frames(hist, paths, goal_maps, t_solve, n_steps, trace, T,
                                                        T_batch=T if coupled else None)
         return AstarOutput(hist, paths, intermediate_results)
@@ -251,7 +277,7 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
         loop, :251-252), with T_batch decided on the device (_native.forward_coupled); it has no frames."""
         W = start_maps.shape[-1]
         T = self.num_steps(W)
-        if float(self.g_ratio) < 0.5 and start_maps.shape[0] > 1:
+        if batch_coupled(self.g_ratio, start_maps.shape[0]):
             if store_intermediate_results:
                 raise ValueError("store_intermediate_results is not available for a batch-coupled search from taps "
                                  "(g_ratio < 0.5, more than one map): use forward() on the cost maps")
@@ -263,7 +289,9 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
             taps, start_maps, goal_maps, obstacles_maps, float(self.g_ratio), T, bool(store_intermediate_results),
             cost_kind=_native.COST_TAPS, cost_scale=scale, cost_bias=bias, **_mech_kw(self.mechanism))
         frames: List[dict] = []
-        if store_intermediate_results:
+        if store_intermediate_results and _recording.get() is not None:
+            frames = SearchRecord(hist, paths, goal_maps, t_solve, trace, T, None)
+        elif store_intermediate_results:
             frames = _materialise_frames(hist, paths, goal_maps, t_solve, n_steps, trace, T)
         return AstarOutput(hist, paths, frames)
 

@@ -69,6 +69,180 @@ def visualize_results(map_designs: torch.Tensor, planner_outputs, scale: int = 1
     return results
 
 
+_GIF_GREEN, _GIF_RED = (51, 204, 0), (255, 0, 0)   # uint8 of visualize_results' (0.2, 0.8, 0) * 255 and (1, 0, 0)
+
+
+def _gif_index_map(n_in: int, n_out: int) -> np.ndarray:
+    """The source index of each of n_out samples that Pillow's NEAREST resize takes from n_in, read from Pillow
+    itself by resizing a row of indices."""
+    if n_in == n_out:
+        return np.arange(n_in, dtype=np.int32)
+    from PIL import Image
+
+    row = Image.fromarray(np.arange(n_in, dtype=np.int32)[None, :])
+    return np.asarray(row.resize((n_out, 1), resample=Image.NEAREST), dtype=np.int32)[0]
+
+
+def _gif_geometry(B: int, H: int, W: int, scale: int, grid: bool):
+    """(image rows, image columns, screen width, screen height) of visualize_results(maps, ., scale): the
+    make_grid image, enlarged to (rows * scale, cols * scale) given to Pillow as (width, height)."""
+    if grid and B > 1:
+        xmaps = min(8, B)
+        Hi, Wi = (H + 2) * (-(-B // xmaps)) + 2, (W + 2) * xmaps + 2
+    else:
+        Hi, Wi = H, W
+    SW, SH = (Hi * scale, Wi * scale) if scale > 1 else (Wi, Hi)
+    if SW > 0xFFFF or SH > 0xFFFF:
+        raise ValueError(f"search_gifs: the {SW}x{SH} screen has a side above 65535")
+    return Hi, Wi, SW, SH
+
+
+def _gif_lzw_pixel(m: int, index: int) -> bytes:
+    """The LZW stream of one pixel: clear, the index, end of information, each m + 1 bits, LSB first."""
+    v = (1 << m) | (index << (m + 1)) | (((1 << m) + 1) << (2 * (m + 1)))
+    return v.to_bytes(-(-3 * (m + 1) // 8), "little")
+
+
+def search_gifs(planner, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
+                scale: int = 4, fps: float = 30, hold: int = 15, layout: str = "each", loop: int = 0):
+    """Animated GIFs of the planner's search, as bytes (DESIGN.md §19).
+
+    The planner (VanillaAstar or NeuralAstar with the differentiable search) runs once with a trace, then two kernel
+    launches draw and LZW-encode every frame on the device.  layout "each": one GIF per map, whose frames are
+    visualize_results(map_designs[b:b+1], f, scale) for f in the intermediate_results of the planner run on map b
+    alone, then the last frame `hold` more times.  layout "grid": one GIF whose frames are visualize_results of the
+    whole batch over the batched call's intermediate_results, then `hold` copies of the last.  Exact colours: the
+    maps' grey levels, (51, 204, 0) explored, (255, 0, 0) selected or on the path, black border.  Each frame after the
+    first covers only the pixels that changed, the rest transparent; a frame equal to the previous one is one
+    transparent pixel.  map_designs: [B,1,H,W] CUDA tensor with values in [0, 1].  A NeuralAstar in train mode
+    normalises its encoder's batch with the batch's own statistics, so there GIF b of "each" shows map b searched within
+    the batch, which equals map b searched alone only for a batch of one.  The search runs in the caller's autograd mode,
+    because a NeuralAstar's encoder takes its folded inference path only without autograd, and the frames are those of
+    a plain call in the same mode; call it under torch.no_grad() for inference (any graph is freed on return).  The host waits three times: for the
+    maps' grey levels, for the frame sizes and for the bytes (a batch-coupled grid search waits once more itself)."""
+    from ..planner.astar import VanillaAstar
+    from ..planner.differentiable_astar import _recording
+
+    if not isinstance(planner, VanillaAstar):
+        raise TypeError("search_gifs: the planner must be a VanillaAstar or a NeuralAstar")
+    if not planner.use_differentiable_astar:
+        raise ValueError("search_gifs: use_differentiable_astar=False (pq_astar) has no intermediate results")
+    if layout not in ("each", "grid"):
+        raise ValueError(f"search_gifs: layout must be 'each' or 'grid' (got {layout!r})")
+    if map_designs.ndim != 4 or map_designs.shape[1] != 1:
+        raise ValueError(f"search_gifs: map_designs must be [B,1,H,W] grey maps (got {tuple(map_designs.shape)})")
+    if int(scale) != scale or scale < 1 or hold < 0 or int(hold) != hold or not fps > 0 or not 0 <= loop <= 0xFFFF:
+        raise ValueError("search_gifs: scale >= 1 and hold >= 0 are integers, fps > 0, 0 <= loop <= 65535")
+    delay = round(100 / fps)
+    if delay > 0xFFFF:
+        raise ValueError("search_gifs: fps is too low for a 16-bit delay")
+    B, _, H, W = map_designs.shape
+    grid = layout == "grid"
+    Hi, Wi, SW, SH = _gif_geometry(B, H, W, int(scale), grid)
+    if not map_designs.is_cuda:
+        raise RuntimeError("search_gifs: map_designs must be a CUDA tensor (there is no CPU fallback)")
+    dev = map_designs.device
+    maps = map_designs.detach().float()
+    G = 1 if grid else B
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream(dev)
+        # wait 1: the grey levels of each GIF's maps and their range, before anything runs
+        grey = (maps * 255).to(torch.uint8).reshape(B, -1).long()
+        present = torch.zeros((B, 256), dtype=torch.bool, device=dev).scatter_(1, grey, True)
+        if grid:
+            present = present.any(0, keepdim=True)
+        lo_hi = torch.stack(torch.aminmax(maps)).reshape(1, 2)
+        probe = torch.cat([present.float(), lo_hi.expand(G, 2)], 1).to("cpu", non_blocking=True)
+        stream.synchronize()
+        probe = probe.numpy()
+        if not (probe[0, 256] >= 0 and probe[0, 257] <= 1):
+            raise ValueError("search_gifs: map_designs must hold values in [0, 1]")
+        present = probe[:, :256] > 0
+        present[:, 0] = True
+        n_grey = present.sum(1)
+        bits = np.maximum(2, np.ceil(np.log2(n_grey + 3))).astype(np.int64)
+        if bits.max() > 8:
+            raise ValueError(f"search_gifs: {int(n_grey.max())} grey levels and 3 more colours do not fit a "
+                             "256-entry palette")
+        token = _recording.set("batch" if grid else "each")
+        try:
+            rec = planner(map_designs, start_maps, goal_maps, store_intermediate_results=True).intermediate_results
+        finally:
+            _recording.reset(token)
+        if grid:
+            steps_mode = _native.GIF_STEPS_ALL if rec.T_batch is not None else _native.GIF_STEPS_BATCH
+        else:
+            steps_mode = _native.GIF_STEPS_MAP
+        p, keep = _native.gif_params(maps, rec.histories, rec.paths, rec.goal_maps.float(), rec.trace,
+                                     rec.t_solve, _native.GIF_GRID if grid else _native.GIF_EACH, steps_mode, SW, SH,
+                                     delay)
+        xmap = _gif_index_map(Wi, SW)
+        ymap = _gif_index_map(Hi, SH)
+        xspan = np.stack([np.searchsorted(xmap, np.arange(Wi), "left"), np.searchsorted(xmap, np.arange(Wi), "right")],
+                         1)
+        yspan = np.stack([np.searchsorted(ymap, np.arange(Hi), "left"), np.searchsorted(ymap, np.arange(Hi), "right")],
+                         1)
+        lut = np.zeros((G, 256), np.uint8)
+        for g in range(G):
+            levels = np.flatnonzero(present[g])
+            lut[g, levels] = np.arange(len(levels))
+        colors = np.stack([n_grey, bits], 1).astype(np.uint8)
+        host = np.concatenate([np.concatenate([xmap, ymap, xspan.ravel(), yspan.ravel()]).astype("<i4").view(np.uint8),
+                               lut.ravel(), colors.ravel()])
+        assert len(host) == _native.gif_tables_bytes(p)
+        tables_h = torch.from_numpy(host).pin_memory()
+        tables = tables_h.to(dev, non_blocking=True)
+        p.tables = tables.data_ptr()
+        steps, nbytes, ws = _native.gif_plan(p, dev)
+        # wait 2: the steps of each GIF and the size of every frame's LZW stream
+        steps_h = steps.to("cpu", non_blocking=True)
+        nbytes_h = nbytes.to("cpu", non_blocking=True)
+        stream.synchronize()
+        steps_h = steps_h.numpy().astype(np.int64)
+        F = int((steps_h + 1).sum())
+        nb = nbytes_h.numpy()[:F]
+        offset = np.concatenate([[0], np.cumsum(_native.gif_record_bytes(nb))]).astype(np.int64)
+        offset_h = torch.from_numpy(offset).pin_memory()
+        offset_d = offset_h.to(dev, non_blocking=True)
+        out = _native.gif_encode(p, nbytes, nb, offset, offset_d, ws)
+        # wait 3: exactly the records' bytes
+        image = torch.empty((int(offset[-1]),), dtype=torch.uint8, pin_memory=True)
+        image.copy_(out[:int(offset[-1])], non_blocking=True)
+        stream.synchronize()
+        del keep, tables_h, offset_h
+    img = image.numpy().tobytes()
+    frame0 = np.concatenate([[0], np.cumsum(steps_h + 1)])
+    gifs = []
+    for g in range(G):
+        P = 1 << int(bits[g])
+        levels = np.flatnonzero(present[g])
+        pal = np.zeros((P, 3), np.uint8)
+        pal[:len(levels)] = levels[:, None]
+        pal[len(levels)] = _GIF_GREEN
+        pal[len(levels) + 1] = _GIF_RED
+        m = int(bits[g])
+        head = (b"GIF89a" + SW.to_bytes(2, "little") + SH.to_bytes(2, "little") + bytes([0x80 | (m - 1) << 4 | (m - 1), 0, 0])
+                + pal.tobytes() + b"\x21\xff\x0bNETSCAPE2.0\x03\x01" + int(loop).to_bytes(2, "little") + b"\x00")
+        lzw = _gif_lzw_pixel(m, len(levels) + 2)
+        still = (b"\x21\xf9\x04\x05" + delay.to_bytes(2, "little") + bytes([len(levels) + 2, 0])
+                 + b"\x2c\x00\x00\x00\x00\x01\x00\x01\x00\x00" + bytes([m, len(lzw)]) + lzw + b"\x00")
+        gifs.append(head + img[offset[frame0[g]]:offset[frame0[g + 1]]] + still * int(hold) + b";")
+    return gifs
+
+
+def save_search_gifs(paths, planner, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
+                     **kwargs) -> None:
+    """search_gifs(planner, map_designs, start_maps, goal_maps, **kwargs), each GIF written to its path (one path for
+    layout "grid", one per map for "each")."""
+    paths = [paths] if isinstance(paths, (str, os.PathLike)) else list(paths)
+    G = 1 if kwargs.get("layout", "each") == "grid" else map_designs.shape[0]
+    if len(paths) != G:
+        raise ValueError(f"save_search_gifs: {G} GIFs, {len(paths)} paths")
+    for path, gif in zip(paths, search_gifs(planner, map_designs, start_maps, goal_maps, **kwargs)):
+        with open(path, "wb") as f:
+            f.write(gif)
+
+
 class MazeDataset(data.Dataset):
     def __init__(self, filename: str, split: str, pct1: float = 0.55, pct2: float = 0.70, pct3: float = 0.85,
                  num_starts: int = 1):
@@ -925,6 +1099,6 @@ def save_planning_dataset(path: str, train, valid, test) -> None:
 __all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "MazeDataset", "WarCraftDataset",
            "compute_opt_labels", "compute_weighted_opt_labels", "create_dataloader", "create_device_dataloader",
            "create_warcraft_dataloader", "draw_opt_policies", "load_map_images", "maps_from_images",
-           "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset", "savez_compressed_device",
-           "save_warcraft_dataset",
+           "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset", "save_search_gifs",
+           "savez_compressed_device", "save_warcraft_dataset", "search_gifs",
            "shortest_path_maps", "tile_maps", "visualize_results"]
