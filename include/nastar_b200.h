@@ -224,11 +224,19 @@ int nastar_b200_conv1_marks(const float *map_designs, const float *start, int64_
                             const float *bias_host, float *out, void *stream);
 
 /* Head of the encoder (its last 3x3 conv has ONE output channel, encoder.py:60-78): taps[p][k] = sum_c x[p][c] *
- * w[c][k] for every pixel p of the channels-last activation x (fp32 [P][C], C in {32,64,128,256}), k = ky*3+kx.
+ * w[c][k] for every pixel p of the channels-last activation x (fp32 [P][C], C in {16,32,64,128,256}), k = ky*3+kx.
  * `w` is a HOST pointer to C*9 floats ([c][k], BatchNorm folded): it is passed to the kernel by value (constant
  * bank), so it may change between calls without any device copy.  The 9-tap spatial gather + bias + sigmoid * const
  * that finish the layer happen in nastar_b200_forward's NASTAR_COST_TAPS prologue (or nastar_b200_cost_from_taps). */
 int nastar_b200_head_taps(const float *x, int64_t P, int32_t C, const float *w_host, float *taps, void *stream);
+
+/* Input of a U-Net decoder block (planner/encoder.py Unet): out[b][y][x][:] = concat(dec[b][y/2][x/2][0..Cd-1],
+ * skip[b][y][x][0..Cs-1]) for y < 2h, x < 2w, i.e. torch.cat((F.interpolate(dec, scale_factor=2, mode="nearest"),
+ * skip), 1) bit for bit.  dec: channels-last fp32 [B][h][w][Cd]; skip: channels-last fp32 [B][2h][2w][Cs], or NULL with
+ * Cs = 0 (the last block has no skip); out: channels-last fp32 [B][2h][2w][Cd+Cs].  Every pointer 16-B aligned, Cd > 0
+ * and Cs >= 0 multiples of 4, else NASTAR_EINVAL before any launch.  One kernel launch, asynchronous on `stream`. */
+int nastar_b200_upsample_concat(const float *dec, int32_t B, int32_t h, int32_t w, int32_t Cd, const float *skip,
+                                int32_t Cs, float *out, void *stream);
 
 /* The encoder's last body layer fused with the head products (encoder.py:60-78, the 128 -> 256 conv + BatchNorm + ReLU
  * followed by nastar_b200_head_taps): taps[p][k] = sum_c relu(bias[c] + conv3x3(x, w)[p][c]) * head_w[c][k], pad 1,

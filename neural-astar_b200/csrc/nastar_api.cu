@@ -683,12 +683,27 @@ int nastar_b200_head_taps(const float* x, int64_t P, int32_t C, const float* w_h
     if (P > (int64_t(1) << 31) * 127) return NASTAR_EINVAL;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
     switch (C) {
+        case 16: launch_head<16>(x, P, w_host, taps, stream); break;
         case 32: launch_head<32>(x, P, w_host, taps, stream); break;
         case 64: launch_head<64>(x, P, w_host, taps, stream); break;
         case 128: launch_head<128>(x, P, w_host, taps, stream); break;
         case 256: launch_head<256>(x, P, w_host, taps, stream); break;
         default: return NASTAR_EUNSUPPORTED;
     }
+    return launched();
+}
+
+int nastar_b200_upsample_concat(const float* dec, int32_t B, int32_t h, int32_t w, int32_t Cd, const float* skip,
+                                int32_t Cs, float* out, void* stream_v) {
+    if (!dec || !out || (Cs > 0 && !skip) || B <= 0 || h <= 0 || w <= 0 || Cd <= 0 || Cs < 0) return NASTAR_EINVAL;
+    if ((Cd & 3) || (Cs & 3)) return NASTAR_EINVAL;
+    if ((reinterpret_cast<uintptr_t>(dec) | reinterpret_cast<uintptr_t>(skip) | reinterpret_cast<uintptr_t>(out)) & 15)
+        return NASTAR_EINVAL;
+    if (int64_t(B) * 2 * h > INT32_MAX || int64_t(2) * w > INT32_MAX) return NASTAR_EINVAL;
+    const int64_t total = int64_t(B) * h * w * (Cd / 4) + int64_t(B) * 4 * h * w * (Cs / 4);
+    nastar::upsample_concat_kernel<<<capped_grid((total + 255) / 256, 16), 256, 0, static_cast<cudaStream_t>(stream_v)>>>(
+        reinterpret_cast<const float4*>(dec), B, h, w, Cd / 4, reinterpret_cast<const float4*>(skip), Cs / 4,
+        reinterpret_cast<float4*>(out));
     return launched();
 }
 

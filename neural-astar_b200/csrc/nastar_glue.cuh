@@ -150,12 +150,14 @@ struct HeadWeights {
 };
 
 constexpr int kHeadWarps = 4;
-constexpr int kHeadSlice = 32;                       // channels staged per pass (128 contiguous bytes per pixel)
+// channels staged per pass: 32 (128 contiguous bytes per pixel), or all 16 of the U-Net's depth-5 head
+template <int C>
+constexpr int kHeadSlice = C < 32 ? C : 32;
 
 template <int C>
 __device__ __forceinline__ void head_issue_slice(const float* __restrict__ x, int64_t P, int64_t p0, int s0, uint32_t dst_s,
                                                  int lane) {
-    constexpr int kRow = kHeadSlice + 4, kChunks = kHeadSlice / 4;
+    constexpr int kRow = kHeadSlice<C> + 4, kChunks = kHeadSlice<C> / 4;
 #pragma unroll
     for (int i = 0; i < kChunks; ++i) {              // 32 lanes x kChunks copies of 16 B = the 32 x kHeadSlice tile
         const int idx = i * 32 + lane;
@@ -173,9 +175,9 @@ template <int C>
 __global__ void __launch_bounds__(32 * kHeadWarps) head_taps_kernel(const float* __restrict__ x, int64_t P,
                                                                     const __grid_constant__ HeadWeights<C> hw,
                                                                     float* __restrict__ out) {
-    constexpr int kRow = kHeadSlice + 4;             // padded row (floats): 16 B aligned, quarter-warps hit 32 distinct banks
-    constexpr int kChunks = kHeadSlice / 4;          // float4 per pixel and slice
-    constexpr int kSlices = C / kHeadSlice;
+    constexpr int kRow = kHeadSlice<C> + 4;          // padded row (floats): 16 B aligned, quarter-warps hit 32 distinct banks
+    constexpr int kChunks = kHeadSlice<C> / 4;       // float4 per pixel and slice
+    constexpr int kSlices = C / kHeadSlice<C>;
     __shared__ __align__(16) float sX[kHeadWarps][2][32 * kRow];   // per warp: two slices in flight / in use
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t st_s = uint32_t(__cvta_generic_to_shared(&sX[warp][0][0]));
@@ -196,7 +198,7 @@ __global__ void __launch_bounds__(32 * kHeadWarps) head_taps_kernel(const float*
             const bool last = (sl == kSlices - 1);
             const int64_t gn = last ? grp + gstride : grp;
             if (gn < groups)
-                head_issue_slice<C>(x, P, gn * 32, last ? 0 : (sl + 1) * kHeadSlice, st_s + uint32_t((buf ^ 1) * 32 * kRow) * 4u, lane);
+                head_issue_slice<C>(x, P, gn * 32, last ? 0 : (sl + 1) * kHeadSlice<C>, st_s + uint32_t((buf ^ 1) * 32 * kRow) * 4u, lane);
             else
                 asm volatile("cp.async.commit_group;" ::: "memory");
             asm volatile("cp.async.wait_group 1;" ::: "memory");
@@ -207,10 +209,10 @@ __global__ void __launch_bounds__(32 * kHeadWarps) head_taps_kernel(const float*
                 const float4 v = *reinterpret_cast<const float4*>(st + lane * kRow + c4 * 4);
 #pragma unroll
                 for (int k = 0; k < 9; ++k) {
-                    acc[k] = fmaf(v.x, hw.w[(sl * kHeadSlice + 4 * c4 + 0) * 9 + k], acc[k]);
-                    acc[k] = fmaf(v.y, hw.w[(sl * kHeadSlice + 4 * c4 + 1) * 9 + k], acc[k]);
-                    acc[k] = fmaf(v.z, hw.w[(sl * kHeadSlice + 4 * c4 + 2) * 9 + k], acc[k]);
-                    acc[k] = fmaf(v.w, hw.w[(sl * kHeadSlice + 4 * c4 + 3) * 9 + k], acc[k]);
+                    acc[k] = fmaf(v.x, hw.w[(sl * kHeadSlice<C> + 4 * c4 + 0) * 9 + k], acc[k]);
+                    acc[k] = fmaf(v.y, hw.w[(sl * kHeadSlice<C> + 4 * c4 + 1) * 9 + k], acc[k]);
+                    acc[k] = fmaf(v.z, hw.w[(sl * kHeadSlice<C> + 4 * c4 + 2) * 9 + k], acc[k]);
+                    acc[k] = fmaf(v.w, hw.w[(sl * kHeadSlice<C> + 4 * c4 + 3) * 9 + k], acc[k]);
                 }
             }
             __syncwarp();                            // all lanes done reading before this buffer is refilled
@@ -223,6 +225,39 @@ __global__ void __launch_bounds__(32 * kHeadWarps) head_taps_kernel(const float*
         }
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
+}
+
+// ---- U-Net decoder block input: nearest x2 upsample and skip concat (planner/encoder.py Unet) --------------------
+// out[b][y][x][0..Cd-1] = dec[b][y/2][x/2][..], out[b][y][x][Cd..Cd+Cs-1] = skip[b][y][x][..]; channels-last fp32,
+// out is [B][2h][2w][Cd+Cs].  A pure copy, so the result is bit-equal to cat(interpolate(dec, x2, nearest), skip).
+// Two index spaces share one grid-stride loop: the first B*h*w*Cd/4 items each read one float4 of dec and store it to
+// the four output pixels it covers, the remaining B*2h*2w*Cs/4 items each move one float4 of skip.  Every input byte is
+// read once; consecutive threads read and write consecutive 16-byte vectors of one pixel's channel run.
+__global__ void __launch_bounds__(256) upsample_concat_kernel(const float4* __restrict__ dec, int B, int h, int w, int cd4,
+                                                              const float4* __restrict__ skip, int cs4,
+                                                              float4* __restrict__ out) {
+    const int W = 2 * w, co4 = cd4 + cs4;
+    const int64_t n_dec = int64_t(B) * h * w * cd4;
+    const int64_t total = n_dec + int64_t(B) * 2 * h * W * cs4;
+    for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
+        if (i < n_dec) {
+            const int64_t pix = i / cd4;                 // (b*h + yy)*w + xx
+            const int c = int(i - pix * cd4);
+            const int xx = int(pix % w);
+            const int64_t by = pix / w;                  // b*h + yy: output rows 2*by and 2*by+1 of the flattened batch
+            const float4 v = __ldg(dec + i);
+            float4* o = out + (2 * by * W + 2 * xx) * co4 + c;
+            o[0] = v;
+            o[co4] = v;
+            o[int64_t(W) * co4] = v;
+            o[int64_t(W) * co4 + co4] = v;
+        } else {
+            const int64_t j = i - n_dec;
+            const int64_t pix = j / cs4;
+            const int c = int(j - pix * cs4);
+            out[pix * co4 + cd4 + c] = __ldg(skip + j);
+        }
+    }
 }
 
 }  // namespace nastar

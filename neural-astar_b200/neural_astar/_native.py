@@ -93,6 +93,7 @@ _SIGNATURES = {
     "nastar_b200_head_taps": (_int, [_p, _i64, _i32, _p, _p, _p]),
     "nastar_b200_conv1_marks": (_int, [_p, _p, _i64, _p, _i64, _i32, _i32, _i32, _p, _p, _p, _p]),
     "nastar_b200_conv3x3_head_taps": (_int, [_p] + [_i32] * 5 + [_p] * 5),
+    "nastar_b200_upsample_concat": (_int, [_p] + [_i32] * 4 + [_p, _i32, _p, _p]),
     "nastar_b200_selftest_sqrt": (_int, [_i32, _p, _p]),
     "nastar_b200_opt_labels": (_int, [_p, _i64, _p, _i32, _i32, _i32, _p, _p, _p, _p]),
     "nastar_b200_opt_labels_mech": (_int, [_p, _i64, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _p]),
@@ -376,7 +377,7 @@ def pack_inputs(map_designs: torch.Tensor, start: torch.Tensor, goal: torch.Tens
     return out.permute(0, 3, 1, 2)   # logical NCHW view with channels-last strides
 
 
-HEAD_CHANNELS = (32, 64, 128, 256)
+HEAD_CHANNELS = (16, 32, 64, 128, 256)
 
 
 def conv1_marks(map_designs: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, w_host, bias_host) -> torch.Tensor:
@@ -410,7 +411,7 @@ def head_taps(x: torch.Tensor, w_host, out: Optional[torch.Tensor] = None) -> to
     L = lib()
     B, C, H, W = x.shape
     if C not in HEAD_CHANNELS or x.dtype != torch.float32 or not x.is_contiguous(memory_format=torch.channels_last):
-        raise ValueError("head_taps expects a channels-last fp32 activation with 32/64/128/256 channels")
+        raise ValueError("head_taps expects a channels-last fp32 activation with 16/32/64/128/256 channels")
     if w_host.dtype.name != "float32" or w_host.shape != (C, 9) or not w_host.flags["C_CONTIGUOUS"]:
         raise ValueError("w_host must be a C-contiguous float32 [C,9] array")
     dev = x.device
@@ -420,6 +421,29 @@ def head_taps(x: torch.Tensor, w_host, out: Optional[torch.Tensor] = None) -> to
         _check(L.nastar_b200_head_taps(x.data_ptr(), B * H * W, C, w_host.ctypes.data, out.data_ptr(),
                                        stream), "nastar_b200_head_taps")
     return out
+
+
+def upsample_concat(dec: torch.Tensor, skip: Optional[torch.Tensor]) -> torch.Tensor:
+    """torch.cat((F.interpolate(dec, scale_factor=2, mode="nearest"), skip), 1) in one kernel, bit for bit: the input of
+    a U-Net decoder block.  dec: channels-last fp32 CUDA [B,Cd,h,w]; skip: channels-last fp32 [B,Cs,2h,2w] on the same
+    device, or None for the last block.  Channel counts must be multiples of 4.  Returns a channels-last
+    [B,Cd+Cs,2h,2w] tensor."""
+    L = lib()
+    B, Cd, h, w = dec.shape
+    Cs = 0 if skip is None else skip.shape[1]
+    if (not dec.is_cuda or dec.dtype != torch.float32 or not dec.is_contiguous(memory_format=torch.channels_last)
+            or Cd % 4 or Cs % 4):
+        raise ValueError("upsample_concat expects channels-last fp32 CUDA tensors with channel counts divisible by 4")
+    if skip is not None and (tuple(skip.shape) != (B, Cs, 2 * h, 2 * w) or skip.dtype != torch.float32
+                             or skip.device != dec.device
+                             or not skip.is_contiguous(memory_format=torch.channels_last)):
+        raise ValueError("upsample_concat expects a channels-last fp32 skip [B,Cs,2h,2w] on dec's device")
+    dev = dec.device
+    with _on_device(dev) as stream:
+        out = torch.empty((B, 2 * h, 2 * w, Cd + Cs), dtype=torch.float32, device=dev)
+        _check(L.nastar_b200_upsample_concat(dec.data_ptr(), B, h, w, Cd, skip.data_ptr() if Cs else None, Cs,
+                                             out.data_ptr(), stream), "nastar_b200_upsample_concat")
+    return out.permute(0, 3, 1, 2)
 
 
 CONVHEAD_CHANNELS = (128, 256)    # (C_in, C_out) of the fused last-conv + head kernel

@@ -12,6 +12,7 @@ from typing import List, Optional
 
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 # Precision of the eval fast path's 3x3 convolutions: TF32 tensor-core math (what torch's own default
 # `torch.backends.cudnn.allow_tf32 = True` gives the reference on any Ampere+ GPU) or full fp32.  The head
@@ -268,21 +269,207 @@ class CNNDownSize(CNN):
         return _conv_stack([input_dim] + self.CHANNELS[:encoder_depth] + [1], pool=True)
 
 
+# torchvision's vgg16_bn feature stack (cfg "D"): 13 conv/BatchNorm/ReLU blocks and 5 max-pools, modules 0..43.  The
+# U-Net's encoder stages split it at each pool, the pool opening the next stage: module ranges [start, end) of s0..s5.
+_VGG16 = [64, 64, "M", 128, 128, "M", 256, 256, 256, "M", 512, 512, 512, "M", 512, 512, 512, "M"]
+_VGG16_STAGES = [(0, 6), (6, 13), (13, 23), (23, 33), (33, 43), (43, 44)]
+_VGG16_STAGE_CHANNELS = [64, 128, 256, 512, 512, 512]
+
+
+def _check_sides(x: torch.Tensor, depth: int) -> None:
+    m = 2 ** depth
+    if x.shape[-2] % m or x.shape[-1] % m:
+        raise ValueError(f"Unet with encoder_depth={depth} needs input sides divisible by 2**{depth} = {m}, "
+                         f"got {tuple(x.shape[-2:])}")
+
+
+def _conv2d_relu(cin: int, cout: int) -> nn.Sequential:
+    return nn.Sequential(nn.Conv2d(cin, cout, 3, padding=1, bias=False), nn.BatchNorm2d(cout), nn.ReLU(inplace=True))
+
+
+class _VggEncoder(nn.Module):
+    def __init__(self, input_dim: int, depth: int):
+        super().__init__()
+        layers: List[nn.Module] = []
+        cin = input_dim
+        for v in _VGG16:
+            if v == "M":
+                layers.append(nn.MaxPool2d(kernel_size=2, stride=2))
+            else:
+                layers += [nn.Conv2d(cin, v, kernel_size=3, padding=1), nn.BatchNorm2d(v), nn.ReLU(inplace=True)]
+                cin = v
+        self.features = nn.Sequential(*layers)
+        self.depth = depth
+
+    def forward(self, x: torch.Tensor) -> List[torch.Tensor]:
+        """Outputs of stages s0..s_depth."""
+        feats = []
+        for a, b in _VGG16_STAGES[:self.depth + 1]:
+            for m in self.features[a:b]:
+                x = m(x)
+            feats.append(x)
+        return feats
+
+
+class _DecoderBlock(nn.Module):
+    def __init__(self, cin: int, cskip: int, cout: int):
+        super().__init__()
+        self.conv1 = _conv2d_relu(cin + cskip, cout)
+        self.attention1 = nn.Identity()
+        self.conv2 = _conv2d_relu(cout, cout)
+        self.attention2 = nn.Identity()
+
+    def forward(self, x: torch.Tensor, skip: Optional[torch.Tensor]) -> torch.Tensor:
+        x = F.interpolate(x, scale_factor=2, mode="nearest")
+        if skip is not None:
+            x = torch.cat([x, skip], dim=1)
+        return self.attention2(self.conv2(self.conv1(self.attention1(x))))
+
+
+class _UnetDecoder(nn.Module):
+    def __init__(self, stage_channels: List[int], decoder_channels: List[int]):
+        super().__init__()
+        enc = stage_channels[1:][::-1]          # s_d .. s1: the full-resolution s0 is not a skip
+        head = enc[0]
+        ins = [head] + decoder_channels[:-1]
+        skips = enc[1:] + [0]
+        self.center = nn.Sequential(_conv2d_relu(head, head), _conv2d_relu(head, head))
+        self.blocks = nn.ModuleList([_DecoderBlock(i, s, o) for i, s, o in zip(ins, skips, decoder_channels)])
+
+    def forward(self, feats: List[torch.Tensor]) -> torch.Tensor:
+        feats = feats[1:][::-1]
+        x = self.center(feats[0])
+        skips = feats[1:]
+        for i, block in enumerate(self.blocks):
+            x = block(x, skips[i] if i < len(skips) else None)
+        return x
+
+
+class _UnetModel(nn.Module):
+    """smp 0.3.1's `Unet(encoder_name="vgg16_bn", classes=1)` in plain torch.nn: same modules, names and shapes."""
+
+    def __init__(self, input_dim: int, decoder_channels: List[int]):
+        super().__init__()
+        depth = len(decoder_channels)
+        self.depth = depth
+        self.encoder = _VggEncoder(input_dim, depth)
+        self.decoder = _UnetDecoder(_VGG16_STAGE_CHANNELS[:depth + 1], decoder_channels)
+        self.segmentation_head = nn.Sequential(nn.Conv2d(decoder_channels[-1], 1, kernel_size=3, padding=1))
+        # smp's initialisation: torchvision's VGG init, except that the first conv is re-created for input_dim != 3
+        # and keeps PyTorch's default init; kaiming-uniform decoder convs; a xavier head with a zero bias
+        for i, m in enumerate(self.encoder.features):
+            if isinstance(m, nn.Conv2d) and not (i == 0 and input_dim != 3):
+                nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
+                nn.init.zeros_(m.bias)
+        for m in self.decoder.modules():
+            if isinstance(m, nn.Conv2d):
+                nn.init.kaiming_uniform_(m.weight, mode="fan_in", nonlinearity="relu")
+        for m in self.modules():
+            if isinstance(m, nn.BatchNorm2d):
+                nn.init.ones_(m.weight)
+                nn.init.zeros_(m.bias)
+        nn.init.xavier_uniform_(self.segmentation_head[0].weight)
+        nn.init.zeros_(self.segmentation_head[0].bias)
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        _check_sides(x, self.depth)
+        return self.segmentation_head(self.decoder(self.encoder(x)))
+
+
+def _fold(conv: nn.Conv2d, bn: nn.BatchNorm2d):
+    """A conv + BatchNorm(running stats) + ReLU block as one plan layer (see EncoderBase._inference_plan)."""
+    with torch.no_grad():
+        scale = bn.weight / torch.sqrt(bn.running_var + bn.eps)
+        w = (conv.weight * scale.view(-1, 1, 1, 1)).contiguous(memory_format=torch.channels_last)
+        bias = conv.bias if conv.bias is not None else torch.zeros_like(bn.running_mean)
+        b = ((bias - bn.running_mean) * scale + bn.bias).contiguous()
+    return (w, b, conv.stride, conv.padding, conv.dilation, True, None, None)
+
+
 class Unet(EncoderBase):
-    """U-Net encoder; needs the optional third-party `segmentation_models_pytorch` (reference :37-57)."""
+    """U-Net with a VGG-16-BN backbone: the network of segmentation_models_pytorch 0.3.1's
+    `Unet(encoder_name="vgg16_bn", encoder_weights=None, classes=1, in_channels=input_dim, encoder_depth=d,
+    decoder_channels=DECODER_CHANNELS[:d])` (reference :37-57), built from torch.nn so that state dicts load in either
+    direction.  Input sides must be divisible by 2**encoder_depth.
+
+    Eval fast path (`head_taps`): BatchNorm folded into every conv, channels-last cuDNN convolutions, each decoder
+    block's upsample + concat as one kernel (`_native.upsample_concat`), and the head's per-pixel [C] x [C,9] products
+    handed to the search's NASTAR_COST_TAPS prologue like the CNN's."""
 
     DECODER_CHANNELS = [256, 128, 64, 32, 16]
 
     def construct_encoder(self, input_dim: int, encoder_depth: int) -> nn.Module:
-        try:
-            import segmentation_models_pytorch as smp
-        except ImportError as e:  # not shipped in this image; used by no reference config
-            raise ImportError("encoder_arch='Unet' needs segmentation_models_pytorch==0.3.1") from e
-        return smp.Unet(
-            encoder_name="vgg16_bn",
-            encoder_weights=None,
-            classes=1,
-            in_channels=input_dim,
-            encoder_depth=encoder_depth,
-            decoder_channels=self.DECODER_CHANNELS[:encoder_depth],
-        )
+        if encoder_depth not in range(1, 6):
+            raise ValueError(f"Unet needs encoder_depth in 1..5, got {encoder_depth}")
+        return _UnetModel(input_dim, self.DECODER_CHANNELS[:encoder_depth])
+
+    def prepare_channels_last(self) -> None:
+        if not self._nhwc:
+            self.model.to(memory_format=torch.channels_last)
+            self._nhwc = True
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        _check_sides(x, self.model.depth)
+        if x.is_cuda and x.dim() == 4:
+            self.prepare_channels_last()
+            x = x.contiguous(memory_format=torch.channels_last)
+        return super().forward(x)
+
+    def head_taps_marks(self, map_designs, start_maps, goal_maps, out=None, on_last_conv=None):
+        """None: the U-Net's 2 -> 64 first conv has no fused kernel, so "m+" inputs go through pack_inputs."""
+        return None
+
+    def head_taps(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, on_last_conv=None):
+        """EncoderBase.head_taps for the U-Net: the folded plan up to the head's per-pixel products."""
+        from .. import _native
+
+        _check_sides(x, self.model.depth)
+        # the plan folds the weights in the layout forward() leaves them in, so that the fused route and encode() run
+        # the very same cuDNN convolutions
+        self.prepare_channels_last()
+        stages, center, blocks, head_w = self._unet_plan(x.device)
+        x = x.contiguous(memory_format=torch.channels_last)
+        with _conv_flags():
+            feats = []
+            for i, stage in enumerate(stages):
+                if i:
+                    x = F.max_pool2d(x, 2)
+                x = _run_plan_inner(stage, x)
+                feats.append(x)
+            skips = feats[1:-1][::-1] + [None]
+            x = _run_plan_inner(center, x)
+            for k, ((conv1, conv2), skip) in enumerate(zip(blocks, skips)):
+                cl = torch.channels_last
+                x = _native.upsample_concat(x.contiguous(memory_format=cl),
+                                            None if skip is None else skip.contiguous(memory_format=cl))
+                x = _run_plan_inner([conv1], x)
+                if on_last_conv is not None and k == len(blocks) - 1:
+                    on_last_conv()
+                x = _run_plan_inner([conv2], x)
+        x = x.contiguous(memory_format=torch.channels_last)
+        return _native.head_taps(x, head_w, out=out), self._head_scalars[0], self._head_scalars[1]
+
+    def _unet_plan(self, device):
+        """(encoder stages, center, decoder blocks, head weights) folded like EncoderBase._inference_plan and cached on
+        the parameters' versions: stages and center are lists of plan layers, blocks (conv1, conv2) pairs, the head
+        [C,9] float32 on the host."""
+        tensors = list(self.model.parameters()) + list(self.model.buffers())
+        if isinstance(self.const, torch.Tensor):
+            tensors.append(self.const)
+        key = (str(device),) + tuple((t.data_ptr(), t._version) for t in tensors)
+        if key == self._plan_key:
+            return self._plan
+        feats = self.model.encoder.features
+        stages = []
+        for a, b in _VGG16_STAGES[:self.model.depth + 1]:
+            mods = list(feats[a:b])
+            stages.append([_fold(c, n) for c, n in zip(mods, mods[1:]) if isinstance(c, nn.Conv2d)])
+        dec = self.model.decoder
+        center = [_fold(blk[0], blk[1]) for blk in dec.center]
+        blocks = [(_fold(blk.conv1[0], blk.conv1[1]), _fold(blk.conv2[0], blk.conv2[1])) for blk in dec.blocks]
+        head = self.model.segmentation_head[0]
+        head_w = head.weight.detach()[0].reshape(head.in_channels, 9).cpu().numpy().astype("float32", order="C")
+        self._head_scalars = (float(head.bias.detach()[0]),
+                              float(self.const) if not isinstance(self.const, float) else self.const)
+        self._plan, self._plan_key = (stages, center, blocks, head_w), key
+        return self._plan
