@@ -218,6 +218,7 @@ FWD_NO_EARLY_EXIT = 1
 FWD_PAIR = 2
 FWD_NEWS = 4
 COST_PLANE, COST_LOGIT, COST_TAPS = 0, 1, 2
+TAPS_MAX_SIDE = 64     # largest H and W whose search reads COST_LOGIT / COST_TAPS (engines 1 and 4)
 
 
 # NASTAR_MECH_*: the planning-datasets generator's --mechanism values

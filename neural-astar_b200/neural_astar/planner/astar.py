@@ -115,42 +115,62 @@ class NeuralAstar(VanillaAstar):
     def encode(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor) -> torch.Tensor:
         """Cost maps from the encoder; with a "+" input the start/goal marks ride along as an extra channel,
         nearest-upsampled when the image is larger than the planning grid (reference :154-180)."""
-        if ("+" in self.encoder_input and self.encoder.fast_path_ok(map_designs) and start_maps.is_cuda
-                and start_maps.dtype == torch.float32):
-            head = self.encoder.head_taps_marks(map_designs, start_maps, goal_maps)   # same kernels as forward()
-            if head is not None:
-                return _native.cost_from_taps(*head)
+        return self._cost(self._head_taps(map_designs, start_maps, goal_maps), map_designs, start_maps, goal_maps)
+
+    def _cost(self, head, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor) -> torch.Tensor:
+        """Cost maps from _head_taps()'s result (the same arithmetic as the search's TAPS prologue), or from the
+        module path when there is none."""
+        if head is not None:
+            return _native.cost_from_taps(*head)
         return self.encoder(self._encoder_input(map_designs, start_maps, goal_maps))
 
     def _encoder_input(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor) -> torch.Tensor:
-        x = map_designs
-        if "+" in self.encoder_input:
-            if self.encoder.fast_path_ok(x) and start_maps.is_cuda and start_maps.dtype == torch.float32:
-                return _native.pack_inputs(x, start_maps, goal_maps)    # one kernel, channels-last result
-            marks = start_maps + goal_maps
-            if marks.shape[-1] != x.shape[-1]:
-                marks = F.interpolate(marks, size=x.shape[-2:], mode="nearest")
-            x = torch.cat((x, marks), dim=1)
-        return x
+        if "+" not in self.encoder_input:
+            return map_designs
+        marks = start_maps + goal_maps
+        if marks.shape[-1] != map_designs.shape[-1]:
+            marks = F.interpolate(marks, size=map_designs.shape[-2:], mode="nearest")
+        return torch.cat((map_designs, marks), dim=1)
 
     def _head_taps(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor, out=None,
                    on_last_conv=None):
-        """Encoder up to the 9-tap products of its head (EncoderBase.head_taps), from the un-assembled inputs: the
-        "m+" CNN reads the three planes in its first layer's kernel, everything else packs them first."""
-        if "+" in self.encoder_input and start_maps.is_cuda and start_maps.dtype == torch.float32:
-            head = self.encoder.head_taps_marks(map_designs, start_maps, goal_maps, out=out, on_last_conv=on_last_conv)
-            if head is not None:
-                return head
-        return self.encoder.head_taps(self._encoder_input(map_designs, start_maps, goal_maps), out=out,
-                                      on_last_conv=on_last_conv)
+        """The eval fast path from the un-assembled inputs to the 9-tap products of the encoder's head
+        (EncoderBase.head_taps): the "m+" CNN reads the three planes in its first layer's kernel, other "+" encoders
+        get them packed by one kernel.  None when the fast path does not apply: training, autograd, inputs other than
+        fp32 CUDA, or an encoder the plan cannot fold."""
+        if not self.encoder.fast_path_ok(map_designs):
+            return None
+        if "+" not in self.encoder_input:
+            return self.encoder.head_taps(map_designs, out=out, on_last_conv=on_last_conv)
+        if not (start_maps.is_cuda and start_maps.dtype == torch.float32):
+            return None
+        head = self.encoder.head_taps_marks(map_designs, start_maps, goal_maps, out=out, on_last_conv=on_last_conv)
+        if head is None:
+            head = self.encoder.head_taps(_native.pack_inputs(map_designs, start_maps, goal_maps), out=out,
+                                          on_last_conv=on_last_conv)
+        return head
+
+    @staticmethod
+    def _searchable(head, start_maps: torch.Tensor) -> bool:
+        """The search's TAPS prologue can read these taps: fp32 CUDA marks on the taps' grid, at most
+        TAPS_MAX_SIDE on a side."""
+        H, W = start_maps.shape[-2:]
+        return (head is not None and start_maps.is_cuda and start_maps.dtype == torch.float32
+                and tuple(head[0].shape[1:3]) == (H, W) and H <= _native.TAPS_MAX_SIDE and W <= _native.TAPS_MAX_SIDE)
 
     def forward(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
                 store_intermediate_results: bool = False) -> AstarOutput:
+        """In eval mode without autograd the encoder runs once, up to its head's 9-tap products.  The search kernel
+        consumes them directly (NASTAR_COST_TAPS), so no cost plane, sigmoid, bias add or layout conversion is
+        launched, unless the taps do not fit its prologue or the search does not take them: pq_astar, and g_ratio < 0.5
+        batches outside CUDA-graph capture, which keep the host procedure of DifferentiableAstar.forward (under capture
+        search_from_taps couples the batch on the device).  Those search the cost plane of the same taps."""
         passable = torch.ones_like(start_maps) if self.learn_obstacles else map_designs
-        fused = self._fused_forward(map_designs, start_maps, goal_maps, passable, store_intermediate_results)
-        if fused is not None:
-            return fused
-        cost_maps = self.encode(map_designs, start_maps, goal_maps)
+        head = self._head_taps(map_designs, start_maps, goal_maps)
+        if (self._searchable(head, start_maps) and self.use_differentiable_astar and passable.dtype == torch.float32
+                and (not batch_coupled(self.g_ratio, start_maps.shape[0]) or torch.cuda.is_current_stream_capturing())):
+            return self.astar.search_from_taps(*head, start_maps, goal_maps, passable, store_intermediate_results)
+        cost_maps = self._cost(head, map_designs, start_maps, goal_maps)
         return self.perform_astar(cost_maps, start_maps, goal_maps, passable, store_intermediate_results)
 
     def forward_pair(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
@@ -166,37 +186,14 @@ class NeuralAstar(VanillaAstar):
                 or (float(self.g_ratio) < 0.5 and B > 1) or map_designs.shape[-2:] != start_maps.shape[-2:]
                 or map_designs.dtype != torch.float32 or start_maps.dtype != torch.float32):
             return None
-        H, W = start_maps.shape[-2], start_maps.shape[-1]
-        T = self.astar.num_steps(W)
+        T = self.astar.num_steps(start_maps.shape[-1])
         kw = _mech_kw(self.astar.mechanism)
-        cost = None
-        if H <= 64 and W <= 64 and self.encoder.fast_path_ok(map_designs):
-            head = self._head_taps(map_designs, start_maps, goal_maps)
-            if head is not None:
-                cost, bias, scale = head
-                kw.update(cost_kind=_native.COST_TAPS, cost_bias=bias, cost_scale=scale)
-        if cost is None:
-            cost = self.encode(map_designs, start_maps, goal_maps)
+        head = self._head_taps(map_designs, start_maps, goal_maps)
+        if self._searchable(head, start_maps):
+            cost, bias, scale = head
+            kw.update(cost_kind=_native.COST_TAPS, cost_bias=bias, cost_scale=scale)
+        else:
+            cost = self._cost(head, map_designs, start_maps, goal_maps)
         hist, paths, _, _, _, counts = _native.forward(cost, start_maps, goal_maps, map_designs, float(self.g_ratio), T,
                                                        pair=True, want_counts=True, **kw)
         return (AstarOutput(hist[:B], paths[:B], []), AstarOutput(hist[B:], paths[B:], []), tuple(counts))
-
-    def _fused_forward(self, map_designs, start_maps, goal_maps, passable, store_intermediate_results):
-        """Inference fast path: the search kernel consumes the encoder's 9-tap partial products directly
-        (NASTAR_COST_TAPS), so no cost plane, sigmoid, bias add or layout conversion is launched.  Returns None
-        when it does not apply (training / autograd, CPU tensors, planning grids above 64x64, encoders without a
-        single-output-channel conv head, pq_astar, and g_ratio < 0.5 batches outside CUDA-graph capture: those keep
-        the host procedure of DifferentiableAstar.forward, while under capture search_from_taps couples the batch on
-        the device)."""
-        H, W = start_maps.shape[-2], start_maps.shape[-1]
-        coupled = batch_coupled(self.g_ratio, start_maps.shape[0])
-        if (not self.use_differentiable_astar or not self.encoder.fast_path_ok(map_designs) or H > 64 or W > 64
-                or not start_maps.is_cuda or (coupled and not torch.cuda.is_current_stream_capturing())
-                or start_maps.dtype != torch.float32 or passable.dtype != torch.float32):
-            return None
-        head = self._head_taps(map_designs, start_maps, goal_maps)
-        if head is None or head[0].shape[1:3] != (H, W):
-            return None
-        taps, bias, scale = head
-        return self.astar.search_from_taps(taps, bias, scale, start_maps, goal_maps, passable,
-                                           store_intermediate_results)

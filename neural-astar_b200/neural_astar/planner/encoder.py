@@ -8,11 +8,14 @@ CNNDownSize) in between, trailing activation(s) dropped; output = sigmoid(model(
 from __future__ import annotations
 
 import os
-from typing import List, Optional
+from typing import List, NamedTuple, Optional
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+
+from .. import _native
 
 # Precision of the eval fast path's 3x3 convolutions: TF32 tensor-core math (what torch's own default
 # `torch.backends.cudnn.allow_tf32 = True` gives the reference on any Ampere+ GPU) or full fp32.  The head
@@ -29,182 +32,62 @@ HEAD_KERNEL = os.environ.get("NASTAR_B200_HEAD_KERNEL", "1") != "0"
 CONV1_KERNEL = os.environ.get("NASTAR_B200_CONV1_KERNEL", "1") != "0"
 
 
-class EncoderBase(nn.Module):
-    def __init__(self, input_dim: int, encoder_depth: int = 4, const: Optional[float] = None):
-        super().__init__()
-        self.model = self.construct_encoder(input_dim, encoder_depth)
-        # learnable scale when given (reference :25-28); plain 1.0 otherwise
-        self.const = nn.Parameter(torch.ones(1) * const) if const is not None else 1.0
-        self._plan = None       # cached inference plan (folded weights) for the cuDNN fast path
-        self._plan_key = None
-        self._nhwc = False      # conv weights converted to channels-last (done lazily on the first CUDA batch)
-        self._head_scalars = (0.0, 1.0)   # (folded bias of the head conv, const) as Python floats
-        self._head_w_host = None          # folded [C,9] weights of the head conv on the host (kernel parameter)
-        self._conv1 = None                # folded ([9,2,32] weights, [32] bias) of a 2->32 first layer, NumPy on the host
+class _Layer(NamedTuple):
+    """A conv + BatchNorm (running statistics) block folded into one convolution: cuDNN's conv + bias (+ ReLU) op,
+    then the block's max-pool if it has one."""
+    w: torch.Tensor              # folded weights, channels-last
+    b: torch.Tensor              # folded bias
+    stride: tuple
+    padding: tuple
+    dilation: tuple
+    relu: bool
+    pool: Optional[nn.MaxPool2d]
 
-    def construct_encoder(self, input_dim: int, encoder_depth: int) -> nn.Module:
-        raise NotImplementedError
 
-    def fast_path_ok(self, x: torch.Tensor) -> bool:
-        """Eval-mode, no-grad, fp32 CUDA input: the folded cuDNN plan (and the fused hand-off) may be used."""
-        return (not self.training) and x.is_cuda and not torch.is_grad_enabled() and x.dtype == torch.float32
+class _Plan(NamedTuple):
+    """An encoder's eval fast path: BatchNorm folded into every conv, ready for channels-last cuDNN convolutions."""
+    body: object                 # what the class's _run_body runs up to the last conv (CNN: a list of _Layer)
+    last: Optional[_Layer]       # the last conv before the head, run by cuDNN or the fused conv + head kernel (None
+                                 # for a CNN of depth 0, whose head reads the input)
+    head_w: np.ndarray           # the head's [C,9] weights on the host (a parameter of the head kernels)
+    head_wm: torch.Tensor        # the same on the device, for torch.mm
+    head_b: float                # the head's bias
+    const: float
+    conv1: Optional[tuple]       # host ([9,2,32], [32]) weights of conv1_marks for a 2 -> 32 first layer, else None
 
-    def prepare_channels_last(self) -> None:
-        """One-off, explicit: store the conv weights channels-last (cuDNN's tensor-core convolutions are
-        NHWC-native).  Pure memory-format change: the Parameter objects,
-        shapes and state-dict contents are unchanged.  Call it once after moving the module to the GPU — before
-        wrapping it in DDP or capturing a CUDA graph.  forward() calls it on the first CUDA batch otherwise."""
-        if not self._nhwc and isinstance(self.model, nn.Sequential):
-            self.model.to(memory_format=torch.channels_last)
-            self._nhwc = True
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.fast_path_ok(x):
-            head = self.head_taps(x)
-            if head is not None:
-                # sigmoid(.)*const finished by the engine's glue kernel: the very arithmetic the fused search
-                # prologue performs (NASTAR_COST_TAPS), so encode() and the fused forward agree bit for bit
-                from .. import _native
+def _fold(conv: nn.Conv2d, bn: nn.BatchNorm2d, relu: bool = True, pool: Optional[nn.MaxPool2d] = None) -> _Layer:
+    """One plan layer; a conv without bias gets a zero one.  The op order fixes the folded weights' bits."""
+    scale = bn.weight / torch.sqrt(bn.running_var + bn.eps)
+    w = (conv.weight * scale.view(-1, 1, 1, 1)).contiguous(memory_format=torch.channels_last)
+    bias = conv.bias if conv.bias is not None else torch.zeros_like(bn.running_mean)
+    b = ((bias - bn.running_mean) * scale + bn.bias).contiguous()
+    return _Layer(w, b, conv.stride, conv.padding, conv.dilation, relu, pool)
 
-                taps, bias, scale = head
-                return _native.cost_from_taps(taps, bias, scale)
-            plan = self._inference_plan(x.device)
-            if plan is not None:
-                return torch.sigmoid(_run_plan(plan, x)) * self.const
-        if x.is_cuda and x.dim() == 4 and isinstance(self.model, nn.Sequential):
-            self.prepare_channels_last()
-            x = x.contiguous(memory_format=torch.channels_last)
-        return torch.sigmoid(self.model(x)) * self.const
 
-    def head_taps(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, on_last_conv=None):
-        """Eval fast path up to (not including) the 9-tap gather of the single-output-channel head:
-        returns (taps [B,H,W,9] fp32 contiguous, folded bias, const) as (tensor, float, float), or None when the
-        encoder does not end in such a head.  bias/const are cached Python floats (no host sync per call)."""
-        plan = self._inference_plan(x.device)
-        if plan is None or plan[-1][7] is None:
-            return None
-        x = x.contiguous(memory_format=torch.channels_last)
-        return self._head_from(plan, 0, x, out, on_last_conv)
+def _host(t: torch.Tensor) -> np.ndarray:
+    return t.cpu().numpy().astype("float32", order="C")
 
-    def head_taps_marks(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
-                        out: Optional[torch.Tensor] = None, on_last_conv=None):
-        """head_taps() of the "m+" input cat(map_designs, start_maps + goal_maps) without materialising it: the first
-        layer reads the three planes directly (one kernel instead of pack_inputs + cuDNN's conv1).  None when the
-        encoder's first layer is not the 2->32 3x3/ReLU block, the maps are not one-channel or the marks live on a
-        different grid; callers then pack the input and use head_taps()."""
-        if not CONV1_KERNEL or map_designs.shape[1] != 1 or map_designs.shape[-2:] != start_maps.shape[-2:]:
-            return None
-        plan = self._inference_plan(map_designs.device)
-        if plan is None or plan[-1][7] is None or self._conv1 is None or len(plan) < 2:
-            return None
-        from .. import _native
 
-        x = _native.conv1_marks(map_designs, start_maps, goal_maps, self._conv1[0], self._conv1[1])
-        return self._head_from(plan, 1, x, out, on_last_conv)
+def _head_fields(w: torch.Tensor, b: torch.Tensor):
+    """(head_w, head_wm, head_b) of a single-output-channel 3x3 head with weights [1,C,3,3] and bias [1]."""
+    wm = w[0].reshape(w.shape[1], 9).contiguous()
+    return _host(wm), wm, float(b.reshape(-1)[0])
 
-    def _head_from(self, plan, first: int, x: torch.Tensor, out: Optional[torch.Tensor], on_last_conv=None):
-        """Layers plan[first:-1] (cuDNN) and the head's products.  `on_last_conv`, if given, is called once, after the
-        second-to-last convolution has been enqueued and before the last (widest) one: PipelinedPlanner forks the
-        previous batch's search there (see its docstring)."""
-        body = plan[first:-1]
-        with _conv_flags():
-            x = _run_plan_inner(body[:-1], x)
-            if on_last_conv is not None:
-                on_last_conv()
-            if body and self._fused_last_conv_ok(body[-1], x):
-                # the last conv and the head products in one TF32 tensor-core kernel: its activation never reaches HBM
-                from .. import _native
 
-                w, b = body[-1][0], body[-1][1]
-                x = x.contiguous(memory_format=torch.channels_last)
-                taps = _native.conv3x3_head_taps(x, w, b, self._head_w_host, out=out)
-                return taps, self._head_scalars[0], self._head_scalars[1]
-            x = _run_plan_inner(body[-1:], x)
-        if not x.is_contiguous(memory_format=torch.channels_last):
-            x = x.contiguous(memory_format=torch.channels_last)
-        wm = plan[-1][7][0]
-        B, C, H, W = x.shape
-        if HEAD_KERNEL and self._head_w_host is not None and C in (32, 64, 128, 256):
-            from .. import _native
+def _conv(layer: _Layer, x: torch.Tensor) -> torch.Tensor:
+    w, b, stride, padding, dilation, relu, pool = layer
+    if relu:
+        x = torch.cudnn_convolution_relu(x, w, b, stride, padding, dilation, 1)
+    else:
+        x = F.conv2d(x, w, b, stride, padding, dilation, 1)
+    return pool(x) if pool is not None else x
 
-            return _native.head_taps(x, self._head_w_host, out=out), self._head_scalars[0], self._head_scalars[1]
-        a = x.permute(0, 2, 3, 1).reshape(-1, C)
-        if out is not None:     # write the GEMM result straight into a caller-owned [B,H,W,9] buffer
-            taps = torch.mm(a, wm, out=out.view(-1, 9)).view(B, H, W, 9)
-        else:
-            taps = torch.mm(a, wm).view(B, H, W, 9)
-        return taps, self._head_scalars[0], self._head_scalars[1]
 
-    def _fused_last_conv_ok(self, layer, x: torch.Tensor) -> bool:
-        """The engine's fused last conv + head kernel covers this layer: TF32 convolutions allowed, the head kernel on,
-        a 3x3 / pad 1 / stride 1 128 -> 256 conv with ReLU and no pooling, maps up to 64x64."""
-        from .. import _native
-
-        w, b, stride, padding, dilation, relu, pool, head = layer
-        return (ALLOW_TF32 and HEAD_KERNEL and self._head_w_host is not None and relu and pool is None and head is None
-                and tuple(w.shape) == (_native.CONVHEAD_CHANNELS[1], _native.CONVHEAD_CHANNELS[0], 3, 3)
-                and tuple(stride) == (1, 1) and tuple(padding) == (1, 1) and tuple(dilation) == (1, 1)
-                and x.is_cuda and x.dtype == torch.float32 and x.shape[1] == _native.CONVHEAD_CHANNELS[0]
-                and x.shape[-2] <= _native.CONVHEAD_MAX_SIDE and x.shape[-1] <= _native.CONVHEAD_MAX_SIDE)
-
-    # ---- eval-mode cuDNN fast path (SURVEY 8(f) rank 3: encoder -> search hand-off) -----------------
-    # Still plain PyTorch/cuDNN: BatchNorm (running stats) is folded into the preceding conv, activations
-    # run channels-last (no NCHW<->NHWC transposes), and conv+bias+ReLU is one cuDNN fused op.  Same math
-    # as self.model(x) up to fp32 re-association of the BN scale; training / autograd use self.model.
-    def _inference_plan(self, device):
-        if not isinstance(self.model, nn.Sequential):
-            return None
-        tensors = [t for t in list(self.model.parameters()) + list(self.model.buffers())]
-        if isinstance(self.const, torch.Tensor):
-            tensors.append(self.const)
-        key = (str(device),) + tuple((t.data_ptr(), t._version) for t in tensors)
-        if key == self._plan_key:
-            return self._plan
-        mods = list(self.model)
-        plan, i = [], 0
-        while i < len(mods):
-            conv = mods[i]
-            if not (isinstance(conv, nn.Conv2d) and i + 1 < len(mods) and isinstance(mods[i + 1], nn.BatchNorm2d)
-                    and conv.groups == 1 and conv.bias is not None):
-                self._plan, self._plan_key = None, key
-                return None
-            bn = mods[i + 1]
-            i += 2
-            relu = i < len(mods) and isinstance(mods[i], nn.ReLU)
-            i += 1 if relu else 0
-            pool = mods[i] if i < len(mods) and isinstance(mods[i], nn.MaxPool2d) else None
-            i += 1 if pool is not None else 0
-            with torch.no_grad():
-                scale = bn.weight / torch.sqrt(bn.running_var + bn.eps)
-                w = (conv.weight * scale.view(-1, 1, 1, 1)).contiguous(memory_format=torch.channels_last)
-                b = ((conv.bias - bn.running_mean) * scale + bn.bias).contiguous()
-            head = None
-            if (conv.out_channels == 1 and conv.kernel_size == (3, 3) and conv.stride == (1, 1)
-                    and conv.padding == (1, 1) and conv.dilation == (1, 1) and not relu and pool is None):
-                # single-output-channel head: cuDNN's implicit GEMM wastes a 256-wide tile on one channel; a
-                # per-pixel [C] x [C,9] GEMM followed by a 9-tap gather is the same sum in a different order
-                # — see _conv3x3_single_output
-                with torch.no_grad():
-                    taps = torch.zeros(1, 9, 3, 3, device=w.device, dtype=w.dtype)
-                    for k in range(9):
-                        taps[0, k, k // 3, k % 3] = 1.0
-                    head = (w[0].reshape(w.shape[1], 9).contiguous(), taps)
-            plan.append((w, b, conv.stride, conv.padding, conv.dilation, relu, pool, head))
-        # scalars of the fused hand-off, read back once per weight version (one host sync at plan build)
-        last_bias = plan[-1][1]
-        self._head_scalars = (float(last_bias.reshape(-1)[0]) if last_bias.numel() == 1 else 0.0,
-                              float(self.const) if not isinstance(self.const, float) else self.const)
-        head = plan[-1][7]
-        self._head_w_host = head[0].detach().cpu().numpy().astype("float32", order="C") if head is not None else None
-        w0, b0, st0, pad0, dil0, relu0, pool0, head0 = plan[0]
-        self._conv1 = None
-        if (tuple(w0.shape) == (32, 2, 3, 3) and tuple(st0) == (1, 1) and tuple(pad0) == (1, 1) and tuple(dil0) == (1, 1)
-                and relu0 and pool0 is None and head0 is None and w0.is_cuda and w0.dtype == torch.float32):
-            with torch.no_grad():       # [cout, cin, ky, kx] -> [tap, cin, cout]
-                self._conv1 = (w0.permute(2, 3, 1, 0).reshape(9, 2, 32).cpu().numpy().astype("float32", order="C"),
-                               b0.detach().cpu().numpy().astype("float32", order="C"))
-        self._plan, self._plan_key = plan, key
-        return plan
+def _run_layers(layers, x: torch.Tensor) -> torch.Tensor:
+    for layer in layers:
+        x = _conv(layer, x)
+    return x
 
 
 def _conv_flags():
@@ -216,35 +99,132 @@ def _conv_flags():
     return torch.backends.cudnn.flags(enabled=True, benchmark=not det, deterministic=det, allow_tf32=ALLOW_TF32)
 
 
-def _run_plan(plan, x: torch.Tensor) -> torch.Tensor:
-    x = x.contiguous(memory_format=torch.channels_last)
-    with _conv_flags():
-        return _run_plan_inner(plan, x)
+def _fuses(last: _Layer, x: torch.Tensor) -> bool:
+    """The engine's fused last conv + head kernel covers this conv: TF32 convolutions allowed, the head kernel on,
+    a 3x3 / pad 1 / stride 1 128 -> 256 conv with ReLU and no pooling, maps up to 64x64."""
+    return (ALLOW_TF32 and HEAD_KERNEL and last.relu and last.pool is None
+            and tuple(last.w.shape) == (_native.CONVHEAD_CHANNELS[1], _native.CONVHEAD_CHANNELS[0], 3, 3)
+            and tuple(last.stride) == (1, 1) and tuple(last.padding) == (1, 1) and tuple(last.dilation) == (1, 1)
+            and x.is_cuda and x.dtype == torch.float32 and x.shape[1] == _native.CONVHEAD_CHANNELS[0]
+            and x.shape[-2] <= _native.CONVHEAD_MAX_SIDE and x.shape[-1] <= _native.CONVHEAD_MAX_SIDE)
 
 
-def _conv3x3_single_output(x: torch.Tensor, wm: torch.Tensor, taps: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    """3x3 / pad 1 convolution with ONE output channel on a channels-last activation:
-    t[n,y,x,k] = <x[n,y,x,:], w[:,k]> for the 9 taps (one skinny fp32 GEMM over the pixels), then
-    out[n,y,x] = b + sum_k t[n, y+ky-1, x+kx-1, k] (a 9->1 one-hot 3x3 convolution, kept in full fp32)."""
-    B, C, H, W = x.shape
-    t = (x.permute(0, 2, 3, 1).reshape(-1, C) @ wm).view(B, H, W, 9).permute(0, 3, 1, 2)
-    det = bool(torch.backends.cudnn.deterministic)
-    with torch.backends.cudnn.flags(enabled=True, benchmark=not det, deterministic=det, allow_tf32=False):
-        return torch.nn.functional.conv2d(t, taps, b, padding=1)
+class EncoderBase(nn.Module):
+    def __init__(self, input_dim: int, encoder_depth: int = 4, const: Optional[float] = None):
+        super().__init__()
+        self.model = self.construct_encoder(input_dim, encoder_depth)
+        # learnable scale when given (reference :25-28); plain 1.0 otherwise
+        self.const = nn.Parameter(torch.ones(1) * const) if const is not None else 1.0
+        self._plan = None       # cached _Plan of the eval fast path
+        self._plan_key = None
+        self._nhwc = False      # conv weights converted to channels-last (done lazily on the first CUDA batch)
 
+    def construct_encoder(self, input_dim: int, encoder_depth: int) -> nn.Module:
+        raise NotImplementedError
 
-def _run_plan_inner(plan, x: torch.Tensor) -> torch.Tensor:
-    for w, b, stride, padding, dilation, relu, pool, head in plan:
-        if head is not None and x.is_contiguous(memory_format=torch.channels_last):
-            x = _conv3x3_single_output(x, head[0], head[1], b)
-            continue
-        if relu:
-            x = torch.cudnn_convolution_relu(x, w, b, stride, padding, dilation, 1)
-        else:
-            x = torch.nn.functional.conv2d(x, w, b, stride, padding, dilation, 1)
-        if pool is not None:
-            x = pool(x)
-    return x
+    def _fold_plan(self) -> Optional[_Plan]:
+        """The modules folded into a _Plan (called without autograd), or None when they do not fold."""
+        raise NotImplementedError
+
+    def _run_body(self, plan: _Plan, x: torch.Tensor) -> torch.Tensor:
+        """plan.body on the channels-last input x: the activation that plan.last takes."""
+        raise NotImplementedError
+
+    def fast_path_ok(self, x: torch.Tensor) -> bool:
+        """Eval-mode, no-grad, fp32 CUDA input: the folded cuDNN plan (and the fused hand-off) may be used."""
+        return (not self.training) and x.is_cuda and not torch.is_grad_enabled() and x.dtype == torch.float32
+
+    def prepare_channels_last(self) -> None:
+        """One-off, explicit: store the conv weights channels-last (cuDNN's tensor-core convolutions are
+        NHWC-native).  Pure memory-format change: the Parameter objects,
+        shapes and state-dict contents are unchanged.  Call it once after moving the module to the GPU — before
+        wrapping it in DDP or capturing a CUDA graph.  forward() calls it on the first CUDA batch otherwise."""
+        if not self._nhwc:
+            self.model.to(memory_format=torch.channels_last)
+            self._nhwc = True
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        if self.fast_path_ok(x):
+            head = self.head_taps(x)
+            if head is not None:
+                # sigmoid(.)*const finished by the engine's glue kernel: the very arithmetic the fused search
+                # prologue performs (NASTAR_COST_TAPS), so encode() and the fused forward agree bit for bit
+                return _native.cost_from_taps(*head)
+        if x.is_cuda and x.dim() == 4:
+            self.prepare_channels_last()
+            x = x.contiguous(memory_format=torch.channels_last)
+        return torch.sigmoid(self.model(x)) * self.const
+
+    def head_taps(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, on_last_conv=None):
+        """Eval fast path up to (not including) the 9-tap gather of the single-output-channel head:
+        returns (taps [B,H,W,9] fp32 contiguous, folded bias, const) as (tensor, float, float), or None when the
+        encoder does not fold.  bias/const are cached Python floats (no host sync per call)."""
+        plan = self._inference_plan(x.device)
+        if plan is None:
+            return None
+        with _conv_flags():
+            x = self._run_body(plan, x.contiguous(memory_format=torch.channels_last))
+            return self._head_step(plan, x, plan.last, out, on_last_conv)
+
+    def head_taps_marks(self, map_designs: torch.Tensor, start_maps: torch.Tensor, goal_maps: torch.Tensor,
+                        out: Optional[torch.Tensor] = None, on_last_conv=None):
+        """head_taps() of the "m+" input cat(map_designs, start_maps + goal_maps) without materialising it: the first
+        layer reads the three planes directly (one kernel instead of pack_inputs + cuDNN's conv1).  None when the
+        encoder's first layer is not the 2->32 3x3/ReLU block, the maps are not one-channel or the marks live on a
+        different grid; callers then pack the input and use head_taps()."""
+        if not CONV1_KERNEL or map_designs.shape[1] != 1 or map_designs.shape[-2:] != start_maps.shape[-2:]:
+            return None
+        plan = self._inference_plan(map_designs.device)
+        if plan is None or plan.conv1 is None:
+            return None
+        x = _native.conv1_marks(map_designs, start_maps, goal_maps, *plan.conv1)
+        with _conv_flags():
+            if not plan.body:       # conv1 is the last conv itself
+                return self._head_step(plan, x, None, out, on_last_conv)
+            # only a CNN has conv1 weights, and its body is a list of layers: conv1_marks computed the first
+            return self._head_step(plan, _run_layers(plan.body[1:], x), plan.last, out, on_last_conv)
+
+    def _head_step(self, plan: _Plan, x: torch.Tensor, last: Optional[_Layer], out: Optional[torch.Tensor],
+                   on_last_conv):
+        """The conv `last` on x (None: x is already its output) and the head's products, written into `out` if given.
+        `on_last_conv`, if given, is called once, before the last (widest) conv is enqueued: PipelinedPlanner forks the
+        previous batch's search there (see its docstring)."""
+        if on_last_conv is not None:
+            on_last_conv()
+        if last is not None and _fuses(last, x):
+            # the last conv and the head products in one TF32 tensor-core kernel: its activation never reaches HBM
+            x = x.contiguous(memory_format=torch.channels_last)
+            return _native.conv3x3_head_taps(x, last.w, last.b, plan.head_w, out=out), plan.head_b, plan.const
+        if last is not None:
+            x = _conv(last, x)
+        x = x.contiguous(memory_format=torch.channels_last)
+        B, C, H, W = x.shape
+        if HEAD_KERNEL and C in _native.HEAD_CHANNELS:
+            taps = _native.head_taps(x, plan.head_w, out=out)
+        else:   # torch.mm writes straight into a caller-owned [B,H,W,9] buffer
+            a = x.permute(0, 2, 3, 1).reshape(-1, C)
+            taps = torch.mm(a, plan.head_wm, out=None if out is None else out.view(-1, 9)).view(B, H, W, 9)
+        return taps, plan.head_b, plan.const
+
+    # ---- eval-mode cuDNN fast path (SURVEY 8(f) rank 3: encoder -> search hand-off) -----------------
+    # Still plain PyTorch/cuDNN: BatchNorm (running stats) is folded into the preceding conv, activations
+    # run channels-last (no NCHW<->NHWC transposes), and conv+bias+ReLU is one cuDNN fused op.  Same math
+    # as self.model(x) up to fp32 re-association of the BN scale; training / autograd use self.model.
+    def _inference_plan(self, device) -> Optional[_Plan]:
+        """The _Plan of the current weights, rebuilt (one host sync) when a parameter or buffer has changed."""
+        # the weights' layout first: the key then stays put between a warm-up and a captured call
+        self.prepare_channels_last()
+        tensors = list(self.model.parameters()) + list(self.model.buffers())
+        if isinstance(self.const, torch.Tensor):
+            tensors.append(self.const)
+        key = (str(device),) + tuple((t.data_ptr(), t._version) for t in tensors)
+        if key != self._plan_key:
+            with torch.no_grad():
+                self._plan, self._plan_key = self._fold_plan(), key
+        return self._plan
+
+    def _const(self) -> float:
+        return float(self.const) if not isinstance(self.const, float) else self.const
 
 
 def _conv_stack(widths: List[int], pool: bool) -> nn.Sequential:
@@ -262,6 +242,38 @@ class CNN(EncoderBase):
 
     def construct_encoder(self, input_dim: int, encoder_depth: int) -> nn.Module:
         return _conv_stack([input_dim] + self.CHANNELS[:encoder_depth] + [1], pool=False)
+
+    def _fold_plan(self) -> Optional[_Plan]:
+        """Conv, BatchNorm[, ReLU][, MaxPool] blocks; the last one, without ReLU or pool, a 3x3 one-output head."""
+        mods, layers, i = list(self.model), [], 0
+        while i < len(mods):
+            conv = mods[i]
+            if not (isinstance(conv, nn.Conv2d) and conv.groups == 1 and i + 1 < len(mods)
+                    and isinstance(mods[i + 1], nn.BatchNorm2d)):
+                return None
+            bn = mods[i + 1]
+            i += 2
+            relu = i < len(mods) and isinstance(mods[i], nn.ReLU)
+            i += 1 if relu else 0
+            pool = mods[i] if i < len(mods) and isinstance(mods[i], nn.MaxPool2d) else None
+            i += 1 if pool is not None else 0
+            layers.append(_fold(conv, bn, relu, pool))
+        head = layers.pop()
+        if not (head.w.shape[:1] == (1,) and head.w.shape[2:] == (3, 3) and tuple(head.stride) == (1, 1)
+                and tuple(head.padding) == (1, 1) and tuple(head.dilation) == (1, 1) and not head.relu
+                and head.pool is None):
+            return None
+        conv1 = None
+        if layers:
+            w0, b0, st0, pad0, dil0, relu0, pool0 = layers[0]
+            if (tuple(w0.shape) == (32, 2, 3, 3) and tuple(st0) == (1, 1) and tuple(pad0) == (1, 1)
+                    and tuple(dil0) == (1, 1) and relu0 and pool0 is None and w0.is_cuda and w0.dtype == torch.float32):
+                conv1 = (_host(w0.permute(2, 3, 1, 0).reshape(9, 2, 32)), _host(b0))   # [tap, cin, cout]
+        last = layers.pop() if layers else None
+        return _Plan(layers, last, *_head_fields(head.w, head.b), self._const(), conv1)
+
+    def _run_body(self, plan: _Plan, x: torch.Tensor) -> torch.Tensor:
+        return _run_layers(plan.body, x)
 
 
 class CNNDownSize(CNN):
@@ -376,16 +388,6 @@ class _UnetModel(nn.Module):
         return self.segmentation_head(self.decoder(self.encoder(x)))
 
 
-def _fold(conv: nn.Conv2d, bn: nn.BatchNorm2d):
-    """A conv + BatchNorm(running stats) + ReLU block as one plan layer (see EncoderBase._inference_plan)."""
-    with torch.no_grad():
-        scale = bn.weight / torch.sqrt(bn.running_var + bn.eps)
-        w = (conv.weight * scale.view(-1, 1, 1, 1)).contiguous(memory_format=torch.channels_last)
-        bias = conv.bias if conv.bias is not None else torch.zeros_like(bn.running_mean)
-        b = ((bias - bn.running_mean) * scale + bn.bias).contiguous()
-    return (w, b, conv.stride, conv.padding, conv.dilation, True, None, None)
-
-
 class Unet(EncoderBase):
     """U-Net with a VGG-16-BN backbone: the network of segmentation_models_pytorch 0.3.1's
     `Unet(encoder_name="vgg16_bn", encoder_weights=None, classes=1, in_channels=input_dim, encoder_depth=d,
@@ -403,62 +405,9 @@ class Unet(EncoderBase):
             raise ValueError(f"Unet needs encoder_depth in 1..5, got {encoder_depth}")
         return _UnetModel(input_dim, self.DECODER_CHANNELS[:encoder_depth])
 
-    def prepare_channels_last(self) -> None:
-        if not self._nhwc:
-            self.model.to(memory_format=torch.channels_last)
-            self._nhwc = True
-
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        _check_sides(x, self.model.depth)
-        if x.is_cuda and x.dim() == 4:
-            self.prepare_channels_last()
-            x = x.contiguous(memory_format=torch.channels_last)
-        return super().forward(x)
-
-    def head_taps_marks(self, map_designs, start_maps, goal_maps, out=None, on_last_conv=None):
-        """None: the U-Net's 2 -> 64 first conv has no fused kernel, so "m+" inputs go through pack_inputs."""
-        return None
-
-    def head_taps(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, on_last_conv=None):
-        """EncoderBase.head_taps for the U-Net: the folded plan up to the head's per-pixel products."""
-        from .. import _native
-
-        _check_sides(x, self.model.depth)
-        # the plan folds the weights in the layout forward() leaves them in, so that the fused route and encode() run
-        # the very same cuDNN convolutions
-        self.prepare_channels_last()
-        stages, center, blocks, head_w = self._unet_plan(x.device)
-        x = x.contiguous(memory_format=torch.channels_last)
-        with _conv_flags():
-            feats = []
-            for i, stage in enumerate(stages):
-                if i:
-                    x = F.max_pool2d(x, 2)
-                x = _run_plan_inner(stage, x)
-                feats.append(x)
-            skips = feats[1:-1][::-1] + [None]
-            x = _run_plan_inner(center, x)
-            for k, ((conv1, conv2), skip) in enumerate(zip(blocks, skips)):
-                cl = torch.channels_last
-                x = _native.upsample_concat(x.contiguous(memory_format=cl),
-                                            None if skip is None else skip.contiguous(memory_format=cl))
-                x = _run_plan_inner([conv1], x)
-                if on_last_conv is not None and k == len(blocks) - 1:
-                    on_last_conv()
-                x = _run_plan_inner([conv2], x)
-        x = x.contiguous(memory_format=torch.channels_last)
-        return _native.head_taps(x, head_w, out=out), self._head_scalars[0], self._head_scalars[1]
-
-    def _unet_plan(self, device):
-        """(encoder stages, center, decoder blocks, head weights) folded like EncoderBase._inference_plan and cached on
-        the parameters' versions: stages and center are lists of plan layers, blocks (conv1, conv2) pairs, the head
-        [C,9] float32 on the host."""
-        tensors = list(self.model.parameters()) + list(self.model.buffers())
-        if isinstance(self.const, torch.Tensor):
-            tensors.append(self.const)
-        key = (str(device),) + tuple((t.data_ptr(), t._version) for t in tensors)
-        if key == self._plan_key:
-            return self._plan
+    def _fold_plan(self) -> _Plan:
+        """body = (encoder stages, center, decoder blocks): stages and center lists of layers, each block its convs; the
+        last block's conv2 is plan.last."""
         feats = self.model.encoder.features
         stages = []
         for a, b in _VGG16_STAGES[:self.model.depth + 1]:
@@ -466,10 +415,25 @@ class Unet(EncoderBase):
             stages.append([_fold(c, n) for c, n in zip(mods, mods[1:]) if isinstance(c, nn.Conv2d)])
         dec = self.model.decoder
         center = [_fold(blk[0], blk[1]) for blk in dec.center]
-        blocks = [(_fold(blk.conv1[0], blk.conv1[1]), _fold(blk.conv2[0], blk.conv2[1])) for blk in dec.blocks]
+        blocks = [[_fold(blk.conv1[0], blk.conv1[1]), _fold(blk.conv2[0], blk.conv2[1])] for blk in dec.blocks]
+        last = blocks[-1].pop()
         head = self.model.segmentation_head[0]
-        head_w = head.weight.detach()[0].reshape(head.in_channels, 9).cpu().numpy().astype("float32", order="C")
-        self._head_scalars = (float(head.bias.detach()[0]),
-                              float(self.const) if not isinstance(self.const, float) else self.const)
-        self._plan, self._plan_key = (stages, center, blocks, head_w), key
-        return self._plan
+        return _Plan((stages, center, blocks), last, *_head_fields(head.weight, head.bias), self._const(), None)
+
+    def _run_body(self, plan: _Plan, x: torch.Tensor) -> torch.Tensor:
+        _check_sides(x, self.model.depth)
+        stages, center, blocks = plan.body
+        feats = []
+        for i, stage in enumerate(stages):
+            if i:
+                x = F.max_pool2d(x, 2)
+            x = _run_layers(stage, x)
+            feats.append(x)
+        skips = feats[1:-1][::-1] + [None]
+        x = _run_layers(center, x)
+        cl = torch.channels_last
+        for layers, skip in zip(blocks, skips):
+            x = _native.upsample_concat(x.contiguous(memory_format=cl),
+                                        None if skip is None else skip.contiguous(memory_format=cl))
+            x = _run_layers(layers, x)
+        return x

@@ -105,13 +105,11 @@ def _conv3_output(na, maps, start, goal):
 
     plan = na.encoder._inference_plan(maps.device)
     with enc._conv_flags():
-        x = _native.conv1_marks(maps, start, goal, *na.encoder._conv1)
-        for li in (1, 2):
-            x = torch.cudnn_convolution_relu(x, *plan[li][:5], 1)
+        x = enc._run_layers(plan.body[1:], _native.conv1_marks(maps, start, goal, *plan.conv1))
     return plan, x.contiguous(memory_format=torch.channels_last)
 
 
-def test_fused_taps_match_cudnn_tf32_conv_and_head(native):
+def test_fused_taps_match_cudnn_tf32_last_conv_and_head(native):
     """Flagship batch (100 maps of 32x32, shipped checkpoint): the fused taps against cuDNN's TF32 conv4 followed by
     head_taps.  Both carry TF32 operand error, so they may differ by up to twice the bound; the cost maps stay within
     the 3e-3 the module's own path tolerance allows."""
@@ -122,13 +120,13 @@ def test_fused_taps_match_cudnn_tf32_conv_and_head(native):
     maps, start, goal = _flagship_inputs()
     with torch.no_grad():
         plan, x3 = _conv3_output(na, maps, start, goal)
-        w, b = plan[3][0], plan[3][1]
-        fused = native.conv3x3_head_taps(x3, w, b, na.encoder._head_w_host)
+        w, b = plan.last.w, plan.last.b
+        fused = native.conv3x3_head_taps(x3, w, b, plan.head_w)
         with torch.backends.cudnn.flags(enabled=True, allow_tf32=True):
-            a4 = torch.cudnn_convolution_relu(x3, *plan[3][:5], 1).contiguous(memory_format=torch.channels_last)
-        old = native.head_taps(a4, na.encoder._head_w_host)
-        _, bound = _fp64_taps_and_bound(x3, w, b, na.encoder._head_w_host)
-        bias, scale = na.encoder._head_scalars
+            a4 = torch.cudnn_convolution_relu(x3, *plan.last[:5], 1).contiguous(memory_format=torch.channels_last)
+        old = native.head_taps(a4, plan.head_w)
+        _, bound = _fp64_taps_and_bound(x3, w, b, plan.head_w)
+        bias, scale = plan.head_b, plan.const
         c_new = native.cost_from_taps(fused, bias, scale)
         c_old = native.cost_from_taps(old, bias, scale)
     diff = (fused.double() - old.double()).abs()
@@ -138,7 +136,7 @@ def test_fused_taps_match_cudnn_tf32_conv_and_head(native):
     assert float((c_new - c_old).abs().max()) < 3e-3
 
 
-def test_encoder_selects_fused_kernel_only_with_tf32(native, monkeypatch):
+def test_head_step_selects_fused_kernel_only_with_tf32(native, monkeypatch):
     """With TF32 allowed the encoder runs the fused kernel in place of cuDNN conv4 + head_taps; with ALLOW_TF32 off the
     taps are bit-identical to cuDNN fp32 conv4 followed by head_taps (the fused kernel is not selected)."""
     from neural_astar.planner import encoder as enc
@@ -157,7 +155,7 @@ def test_encoder_selects_fused_kernel_only_with_tf32(native, monkeypatch):
         assert len(calls) == 1
         plan, x3 = _conv3_output(na, maps, start, goal)
         with enc._conv_flags():
-            a4 = torch.cudnn_convolution_relu(x3, *plan[3][:5], 1).contiguous(memory_format=torch.channels_last)
-        want = native.head_taps(a4, na.encoder._head_w_host)
+            a4 = torch.cudnn_convolution_relu(x3, *plan.last[:5], 1).contiguous(memory_format=torch.channels_last)
+        want = native.head_taps(a4, plan.head_w)
     assert torch.equal(t_fp32, want)
     assert not torch.equal(t_tf32, t_fp32)

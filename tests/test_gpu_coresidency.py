@@ -22,7 +22,7 @@ def _ckpt_planner():
 
 
 @pytest.mark.parametrize("name,B", [("mazes032_vanilla_test", 100), ("inputs_mazes032_all1000", 1000)])
-def test_taps_beside_the_search_equal_taps_alone(name, B):
+def test_fused_taps_beside_the_search_equal_taps_alone(name, B):
     from neural_astar import _native
     from neural_astar.planner import encoder as enc_mod
 
@@ -34,21 +34,19 @@ def test_taps_beside_the_search_equal_taps_alone(name, B):
     with torch.no_grad():
         plan = enc._inference_plan(maps.device)
         with enc_mod._conv_flags():
-            x = _native.conv1_marks(maps, start, goal, *enc._conv1)
-            for li in (1, 2):
-                x = torch.cudnn_convolution_relu(x, *plan[li][:5], 1)
+            x = enc_mod._run_layers(plan.body[1:], _native.conv1_marks(maps, start, goal, *plan.conv1))
         x3 = x.contiguous(memory_format=torch.channels_last)
-        w, b = plan[3][0], plan[3][1]
-        alone = _native.conv3x3_head_taps(x3, w, b, enc._head_w_host)
+        w, b = plan.last.w, plan.last.b
+        alone = _native.conv3x3_head_taps(x3, w, b, plan.head_w)
         search_taps = alone.clone()
-        bias, scale = enc._head_scalars
+        bias, scale = plan.head_b, plan.const
         torch.cuda.synchronize()
         main, side = torch.cuda.current_stream(), torch.cuda.Stream()
         for _ in range(3):
             side.wait_stream(main)
             with torch.cuda.stream(side):          # the search first, so its CTAs are resident when the conv starts
                 out = na.astar.search_from_taps(search_taps, bias, scale, start, goal, maps)
-            beside = _native.conv3x3_head_taps(x3, w, b, enc._head_w_host)
+            beside = _native.conv3x3_head_taps(x3, w, b, plan.head_w)
             main.wait_stream(side)
             torch.cuda.synchronize()
             assert torch.equal(beside, alone)

@@ -110,13 +110,22 @@ def test_fused_forward_matches_encode_then_search(d, inp, mech):
     assert 0.05 < float(cost.mean()) < 0.95, "logits saturated: the comparison would be vacuous"
 
 
-@pytest.mark.parametrize("inp", ["m", "m+"])
-@pytest.mark.parametrize("d", [4, 5])
-def test_encode_matches_eager_module(d, inp, monkeypatch):
+ENCODE_CASES = [(d, inp, head) for head in ("kernel", "mm") for d in (4, 5) for inp in ("m", "m+")]
+
+
+@pytest.mark.parametrize("d,inp,head", ENCODE_CASES,
+                         ids=[f"{d}-{inp}" + ("" if head == "kernel" else "-mm") for d, inp, head in ENCODE_CASES])
+def test_encode_matches_eager_module(d, inp, head, monkeypatch):
+    """encode() against the eager module, with the head's products from the head kernel or, with
+    NASTAR_B200_HEAD_KERNEL=0, from torch.mm."""
+    from neural_astar import _native
     from neural_astar.planner import encoder
 
     maps, starts, goals = _inputs()
     p = _planner(d, inp)
+    monkeypatch.setattr(encoder, "HEAD_KERNEL", head == "kernel")
+    if head == "mm":
+        monkeypatch.setattr(_native, "head_taps", lambda *a, **k: pytest.fail("head kernel ran with HEAD_KERNEL off"))
     x = p._encoder_input(maps, starts, goals)
     old = torch.backends.cudnn.allow_tf32
     try:
@@ -133,7 +142,7 @@ def test_encode_matches_eager_module(d, inp, monkeypatch):
     # fp32 re-association alone moved the costs by 2.4e-5 .. 3.8e-5 on an H100 80GB HBM3 (700 W)
     torch.testing.assert_close(fp32, eager, atol=1e-4, rtol=0)
     diff = float((tf32 - eager).abs().max())
-    print(f"\nUnet d={d} {inp}: max |encode() - eager| = {float((fp32 - eager).abs().max()):.3g} (fp32), "
+    print(f"\nUnet d={d} {inp} {head}: max |encode() - eager| = {float((fp32 - eager).abs().max()):.3g} (fp32), "
           f"{diff:.3g} (TF32)")
     assert diff < 5e-2
 

@@ -62,18 +62,18 @@ res["copy_only_us"] = timed(lambda k: pipe._stacked[k & 1].copy_(ring[k % RING],
 # encoder kernels one by one (eager, back to back on one stream; includes launch gaps when shorter than the CPU issue time)
 plan = na.encoder._inference_plan(maps.device)
 with torch.no_grad(), enc_mod._conv_flags():
-    x0 = [_native.conv1_marks(ring[i][0], ring[i][1], ring[i][2], *na.encoder._conv1).contiguous(memory_format=torch.channels_last) for i in range(4)]
-    res["conv1_us"] = timed(lambda k: _native.conv1_marks(ring[k % RING][0], ring[k % RING][1], ring[k % RING][2], *na.encoder._conv1))
+    x0 = [_native.conv1_marks(ring[i][0], ring[i][1], ring[i][2], *plan.conv1).contiguous(memory_format=torch.channels_last) for i in range(4)]
+    res["conv1_us"] = timed(lambda k: _native.conv1_marks(ring[k % RING][0], ring[k % RING][1], ring[k % RING][2], *plan.conv1))
     xs = x0
-    for li in (1, 2, 3):
-        w, b, st, pad, dil, relu, pool, head = plan[li]
+    for li, layer in enumerate(plan.body[1:] + [plan.last], 1):
+        w, b, st, pad, dil, relu, pool = layer
         res[f"conv{li + 1}_us"] = timed(lambda k: torch.cudnn_convolution_relu(xs[k & 3], w, b, st, pad, dil, 1))
         xs = [torch.cudnn_convolution_relu(x, w, b, st, pad, dil, 1) for x in xs]
-    res["head_us"] = timed(lambda k: _native.head_taps(xs[k & 3], na.encoder._head_w_host))
+    res["head_us"] = timed(lambda k: _native.head_taps(xs[k & 3], plan.head_w))
     # conv4 immediately followed by the head (the head then finds part of conv4's output in L2)
-    w, b, st, pad, dil, relu, pool, head = plan[3]
-    x3 = [torch.cudnn_convolution_relu(torch.cudnn_convolution_relu(x, *plan[1][:5], 1), *plan[2][:5], 1) for x in x0]
-    res["conv4_plus_head_us"] = timed(lambda k: _native.head_taps(torch.cudnn_convolution_relu(x3[k & 3], w, b, st, pad, dil, 1), na.encoder._head_w_host))
+    w, b, st, pad, dil, relu, pool = plan.last
+    x3 = [enc_mod._run_layers(plan.body[1:], x) for x in x0]
+    res["conv4_plus_head_us"] = timed(lambda k: _native.head_taps(torch.cudnn_convolution_relu(x3[k & 3], w, b, st, pad, dil, 1), plan.head_w))
     # the same two layers as the one fused kernel the eval path selects with TF32 on (csrc/nastar_convhead.cuh)
-    res["conv4_head_fused_us"] = timed(lambda k: _native.conv3x3_head_taps(x3[k & 3], w, b, na.encoder._head_w_host))
+    res["conv4_head_fused_us"] = timed(lambda k: _native.conv3x3_head_taps(x3[k & 3], w, b, plan.head_w))
 print(json.dumps({k: round(v, 1) for k, v in res.items()}))

@@ -50,10 +50,10 @@ if what in ("c2", "all"):
         res["eager_ms"] = ev_time(lambda: na(maps, start, goal), reps=20, warm=5)[0]
         cost = na.encode(maps, start, goal)
         res["search_plane_us"] = ev_time(lambda: _native.forward(cost, start, goal, maps, 0.5, 1024), reps=20, warm=5)[0] * 1e3
-        head = na.encoder.head_taps(na._encoder_input(maps, start, goal))
+        head = na._head_taps(maps, start, goal)
         res["search_taps_us"] = ev_time(lambda: _native.forward(head[0], start, goal, maps, 0.5, 1024, cost_kind=2, cost_bias=head[1], cost_scale=head[2]), reps=20, warm=5)[0] * 1e3
         res["pack_us"] = ev_time(lambda: _native.pack_inputs(maps, start, goal), reps=20, warm=5)[0] * 1e3
-        x = na._encoder_input(maps, start, goal)
+        x = _native.pack_inputs(maps, start, goal)
         res["encoder_to_taps_us"] = ev_time(lambda: na.encoder.head_taps(x), reps=20, warm=5)[0] * 1e3
     fast = GraphedPlanner(na, maps, start, goal)
     res["graph_ms"] = ev_time(lambda: fast.replay(), reps=50, warm=5)[0]

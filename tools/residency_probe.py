@@ -54,13 +54,11 @@ def main():
     with torch.no_grad():
         plan = enc._inference_plan(dev)
         with enc_mod._conv_flags():
-            x = _native.conv1_marks(maps, start, goal, *enc._conv1)
-            for li in (1, 2):
-                x = torch.cudnn_convolution_relu(x, *plan[li][:5], 1)
+            x = enc_mod._run_layers(plan.body[1:], _native.conv1_marks(maps, start, goal, *plan.conv1))
         x3 = x.contiguous(memory_format=torch.channels_last)
-    w, b = plan[3][0], plan[3][1]
-    hw = enc._head_w_host
-    bias, scale = enc._head_scalars
+    w, b = plan.last.w, plan.last.b
+    hw = plan.head_w
+    bias, scale = plan.head_b, plan.const
     taps = torch.empty(tuple(maps.shape[:1]) + tuple(maps.shape[2:]) + (9,), device=dev)
     side = torch.cuda.Stream(device=dev)
 

@@ -78,7 +78,7 @@ def main(argv=None):
     planner = NeuralAstar(encoder_arch="Unet", encoder_depth=4, encoder_input="m+").to(dev).eval()
     rows = {}
     with torch.no_grad():
-        x = planner._encoder_input(maps, starts, goals)
+        x = _native.pack_inputs(maps, starts, goals)
 
         def eager_plane_search():
             planner.encoder.prepare_channels_last()
