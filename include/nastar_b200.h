@@ -481,6 +481,43 @@ int64_t nastar_b200_deflate_bound(const nastar_deflate_desc *desc, int32_t M);
  * per SM at most), so it grows with the SMs, not with the input.  0 for descriptors it rejects. */
 size_t nastar_b200_deflate_workspace_bytes(const nastar_deflate_desc *desc, int32_t M);
 
+/* One image of a PNG encode batch (DESIGN.md §21).  Pointers are device addresses; offsets are in bytes. */
+typedef struct nastar_png_enc_desc {
+    const uint8_t *pixels; /* H*W uint8 grey levels, row-major and contiguous */
+    int64_t filt_off;      /* the image's filtered stream, H*(W+1) bytes, in `filt` */
+    int32_t W, H;          /* 1 .. 2048 each */
+} nastar_png_enc_desc;
+
+/* First of the three launches of a PNG encode: filt_off gets each image's filtered scanlines (filter byte, then the
+ * row under the filter type 0..4 with the least sum of |byte as int8|, ties to the lowest type; row 0 sees zeros
+ * above it) and adler[i] the Adler-32 of those H*(W+1) bytes.  Then nastar_b200_deflate compresses them: member i is
+ * head_len 0, data filt + filt_off[i], data_len H*(W+1), gap nastar_b200_png_gap(i), into an `out` of
+ * nastar_b200_png_encode_bound bytes.  desc: the descriptors in HOST memory, read for the checks; desc_dev: the same B
+ * descriptors in device memory, read by the kernel.  Every check precedes the launch: null pointers (a pixels pointer
+ * included), B <= 0, a side <= 0 or a negative filt_off give NASTAR_EINVAL; a side above 2048 gives
+ * NASTAR_EUNSUPPORTED; a filtered range past filt_bytes gives NASTAR_EWORKSPACE.  One kernel launch (one CTA per
+ * image).  Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_png_filter(const nastar_png_enc_desc *desc, const nastar_png_enc_desc *desc_dev, int32_t B,
+                           uint8_t *filt, int64_t filt_bytes, uint32_t *adler, void *stream);
+
+/* Third launch: around image i's deflate stream (out_off[i], out_len[i] from nastar_b200_deflate), the 43 bytes of
+ * signature, IHDR (8-bit grey, not interlaced) with its CRC, IDAT length and type and zlib header 78 DA before it,
+ * and the 20 bytes of Adler-32, IDAT CRC-32 and an IEND chunk after it, all computed on the device.  File i is then
+ * out[out_off[i] - 43, out_off[i] + out_len[i] + 20), and the files lie back to back.  Every check precedes the
+ * launch: those of nastar_b200_png_filter (filt_off is not read) and null out_off, out_len, adler or out give
+ * NASTAR_EINVAL; out_bytes below nastar_b200_png_encode_bound gives NASTAR_EWORKSPACE.  One kernel launch (one CTA per
+ * image).  Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_png_finish(const nastar_png_enc_desc *desc, const nastar_png_enc_desc *desc_dev, int32_t B,
+                           const int64_t *out_off, const int64_t *out_len, const uint32_t *adler, uint8_t *out,
+                           int64_t out_bytes, void *stream);
+
+/* The deflate gap before image i's stream: 43 bytes of its head, plus 20 of image i-1's tail when i > 0. */
+int64_t nastar_b200_png_gap(int32_t i);
+
+/* The bytes `out` needs for these B host descriptors: nastar_b200_deflate_bound of the members above plus the last
+ * image's 20-byte tail; -1 for descriptors nastar_b200_png_filter rejects. */
+int64_t nastar_b200_png_encode_bound(const nastar_png_enc_desc *desc, int32_t B);
+
 /* Search animations (DESIGN.md §19): G GIFs over a search of B maps, layout NASTAR_GIF_EACH (one GIF per map, G = B)
  * or NASTAR_GIF_GRID (one GIF of all maps in make_grid's layout: 8 per row, 2-pixel border, none for B = 1).  GIF g
  * has T_g steps and T_g + 1 frames, numbered GIF by GIF: frame k < T_g is the closed set before step k and the cell

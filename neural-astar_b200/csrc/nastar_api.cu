@@ -19,6 +19,7 @@
 #include "nastar_labels.cuh"
 #include "nastar_maps.cuh"
 #include "nastar_png.cuh"
+#include "nastar_png_encode.cuh"
 #include "nastar_pq.cuh"
 #include "nastar_sampler.cuh"
 #include "nastar_wlabels.cuh"
@@ -362,6 +363,27 @@ int64_t deflate_check(const nastar_deflate_desc* desc, int32_t M, int64_t* chunk
 constexpr size_t kDeflateCtl = 256 + nastar::kDeflateRing * sizeof(nastar::DeflatePub);   // counter, ring
 
 int deflate_grid(int64_t chunks) { return capped_grid(chunks, 1); }
+
+// ---- PNG encode (nastar_png_encode.cuh) -----------------------------------------------------------------------------
+// NASTAR_OK, or the status nastar_b200_png_filter returns for these descriptors (filt_bytes < 0: the filtered ranges
+// are not checked); *bound = nastar_b200_png_encode_bound
+int png_enc_check(const nastar_png_enc_desc* desc, int32_t B, int64_t filt_bytes, int64_t* bound) {
+    if (!desc || B <= 0) return NASTAR_EINVAL;
+    int st = NASTAR_OK;
+    *bound = nastar::kPngEncTail;
+    for (int32_t i = 0; i < B; ++i) {
+        const nastar_png_enc_desc& d = desc[i];
+        if (!d.pixels || d.W <= 0 || d.H <= 0 || d.filt_off < 0) return NASTAR_EINVAL;
+        if (d.W > nastar::kPngEncMaxSide || d.H > nastar::kPngEncMaxSide) {
+            st = NASTAR_EUNSUPPORTED;   // a later descriptor may still be invalid, which takes precedence
+            continue;
+        }
+        const int64_t n = nastar::png_filtered_bytes(d.W, d.H);
+        if (filt_bytes >= 0 && d.filt_off > filt_bytes - n && st == NASTAR_OK) st = NASTAR_EWORKSPACE;
+        *bound += nastar::png_gap(i) + nastar::deflate_member_bound(0, n);
+    }
+    return st;
+}
 
 // ---- search GIFs (nastar_gif.cuh) ------------------------------------------------------------------------------
 struct GifShape {
@@ -1051,6 +1073,41 @@ int nastar_b200_gif_encode(const nastar_gif_params* p, const int32_t* nbytes, co
     if (e != cudaSuccess) return cuda_fail(e);
     e = launch_smem(nastar::gif_encode_kernel, gif_grid(n_frames), nastar::kGifThreads,
                                       sizeof(nastar::GifWarpSmem) * nastar::kGifWarps, stream, a);
+    if (e != cudaSuccess) return cuda_fail(e);
+    return launched();
+}
+
+int64_t nastar_b200_png_gap(int32_t i) { return nastar::png_gap(i); }
+
+int64_t nastar_b200_png_encode_bound(const nastar_png_enc_desc* desc, int32_t B) {
+    int64_t bound = 0;
+    return png_enc_check(desc, B, -1, &bound) == NASTAR_OK ? bound : -1;
+}
+
+int nastar_b200_png_filter(const nastar_png_enc_desc* desc, const nastar_png_enc_desc* desc_dev, int32_t B,
+                           uint8_t* filt, int64_t filt_bytes, uint32_t* adler, void* stream_v) {
+    if (!desc_dev || !filt || !adler || filt_bytes < 0) return NASTAR_EINVAL;
+    int64_t bound = 0;
+    const int st = png_enc_check(desc, B, filt_bytes, &bound);
+    if (st != NASTAR_OK) return st;
+    const nastar::PngFilterArgs a{desc_dev, filt, adler};
+    const cudaError_t e = launch_smem(nastar::png_filter_kernel, B, nastar::kPngEncThreads, 0,
+                                      static_cast<cudaStream_t>(stream_v), a);
+    if (e != cudaSuccess) return cuda_fail(e);
+    return launched();
+}
+
+int nastar_b200_png_finish(const nastar_png_enc_desc* desc, const nastar_png_enc_desc* desc_dev, int32_t B,
+                           const int64_t* out_off, const int64_t* out_len, const uint32_t* adler, uint8_t* out,
+                           int64_t out_bytes, void* stream_v) {
+    if (!desc_dev || !out_off || !out_len || !adler || !out) return NASTAR_EINVAL;
+    int64_t bound = 0;
+    const int st = png_enc_check(desc, B, -1, &bound);
+    if (st != NASTAR_OK) return st;
+    if (out_bytes < bound) return NASTAR_EWORKSPACE;
+    const nastar::PngFinishArgs a{desc_dev, out_off, out_len, adler, out, out_bytes};
+    const cudaError_t e = launch_smem(nastar::png_finish_kernel, B, nastar::kPngEncThreads, 0,
+                                      static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();
 }

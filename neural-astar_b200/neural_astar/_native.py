@@ -112,6 +112,10 @@ _SIGNATURES = {
     "nastar_b200_deflate": (_int, [_p, _p, _i32, _p, _i64, _p, _p, _p, _p, ctypes.c_size_t, _p]),
     "nastar_b200_deflate_bound": (_i64, [_p, _i32]),
     "nastar_b200_deflate_workspace_bytes": (ctypes.c_size_t, [_p, _i32]),
+    "nastar_b200_png_filter": (_int, [_p, _p, _i32, _p, _i64, _p, _p]),
+    "nastar_b200_png_finish": (_int, [_p, _p, _i32, _p, _p, _p, _p, _i64, _p]),
+    "nastar_b200_png_gap": (_i64, [_i32]),
+    "nastar_b200_png_encode_bound": (_i64, [_p, _i32]),
     "nastar_b200_gif_tables_bytes": (_i64, [ctypes.POINTER(GifParams)]),
     "nastar_b200_gif_plan": (_int, [ctypes.POINTER(GifParams), _p, _p, _p, ctypes.c_size_t, _p]),
     "nastar_b200_gif_record_bytes": (_i64, [_i64]),
@@ -881,13 +885,13 @@ def deflate_chunk_counts(data_len) -> np.ndarray:
     return 1 + (n + DEFLATE_CHUNK - 1) // DEFLATE_CHUNK
 
 
-def deflate(desc, desc_dev: torch.Tensor):
+def deflate(desc, desc_dev: torch.Tensor, tail: int = 0):
     """Raw deflate streams of the members in one kernel (include/nastar_b200.h, nastar_b200_deflate).
 
     desc: a NumPy array of DEFLATE_DESC_DTYPE (the host copy, checked before the launch; head / data are device
     addresses); desc_dev: the same descriptors' bytes in device memory (a uint8 CUDA tensor).  Returns (out uint8
-    [bound], out_off int64 [M], out_len int64 [M], crc int32 [M] (the CRC-32's bits)) on the current stream; nothing
-    is read back."""
+    [bound + tail], out_off int64 [M], out_len int64 [M], crc int32 [M] (the CRC-32's bits)) on the current stream;
+    nothing is read back.  `tail` bytes after the bound are left for the caller (a PNG's last trailer)."""
     L = lib()
     d = np.ascontiguousarray(desc, dtype=DEFLATE_DESC_DTYPE)
     if not isinstance(desc_dev, torch.Tensor) or not desc_dev.is_cuda:
@@ -900,15 +904,61 @@ def deflate(desc, desc_dev: torch.Tensor):
     dev = desc_dev.device
     ws_bytes = int(L.nastar_b200_deflate_workspace_bytes(d.ctypes.data, len(d)))
     with _on_device(dev) as stream:
-        out = torch.empty((max(bound, 1),), dtype=torch.uint8, device=dev)
+        out = torch.empty((max(bound + int(tail), 1),), dtype=torch.uint8, device=dev)
         ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
         out_off = torch.empty((len(d),), dtype=torch.int64, device=dev)
         out_len = torch.empty((len(d),), dtype=torch.int64, device=dev)
         crc = torch.empty((len(d),), dtype=torch.int32, device=dev)
-        _check(L.nastar_b200_deflate(d.ctypes.data, desc_dev.data_ptr(), len(d), out.data_ptr(), bound,
+        _check(L.nastar_b200_deflate(d.ctypes.data, desc_dev.data_ptr(), len(d), out.data_ptr(), bound + int(tail),
                                      out_off.data_ptr(), out_len.data_ptr(), crc.data_ptr(), ws.data_ptr(), ws_bytes,
                                      stream), "nastar_b200_deflate")
     return out, out_off, out_len, crc
+
+
+# struct nastar_png_enc_desc (include/nastar_b200.h) as a NumPy record
+PNG_ENC_DESC_DTYPE = np.dtype([("pixels", "<u8"), ("filt_off", "<i8"), ("W", "<i4"), ("H", "<i4")])
+PNG_ENC_HEAD, PNG_ENC_TAIL = 43, 20   # the bytes of a file before and after its deflate stream
+
+
+def png_gaps(B: int) -> np.ndarray:
+    """nastar_b200_png_gap of images 0 .. B-1: the deflate gap before each image's stream."""
+    return np.where(np.arange(B) > 0, PNG_ENC_HEAD + PNG_ENC_TAIL, PNG_ENC_HEAD).astype(np.int64)
+
+
+def png_encode_bound(desc) -> int:
+    """nastar_b200_png_encode_bound of a NumPy array of PNG_ENC_DESC_DTYPE descriptors (-1 when they are rejected)."""
+    d = np.ascontiguousarray(desc, dtype=PNG_ENC_DESC_DTYPE)
+    return int(lib().nastar_b200_png_encode_bound(d.ctypes.data, len(d)))
+
+
+def png_filter(desc, desc_dev: torch.Tensor, filt: torch.Tensor) -> torch.Tensor:
+    """The first PNG encode launch (include/nastar_b200.h, nastar_b200_png_filter): every image's filtered scanlines
+    into `filt` (a uint8 CUDA tensor) at its filt_off.  desc: a NumPy array of PNG_ENC_DESC_DTYPE (the host copy,
+    checked before the launch); desc_dev: the same descriptors' bytes in device memory.  Returns the Adler-32s, int32
+    [B] (their bits), on the current stream."""
+    L = lib()
+    d = np.ascontiguousarray(desc, dtype=PNG_ENC_DESC_DTYPE)
+    if not filt.is_cuda or filt.dtype != torch.uint8 or not desc_dev.is_cuda:
+        raise RuntimeError("png_filter: filt and desc_dev must be CUDA tensors (there is no CPU fallback)")
+    if desc_dev.dtype != torch.uint8 or not desc_dev.is_contiguous() or desc_dev.numel() != d.nbytes:
+        raise ValueError(f"png_filter: desc_dev must be {d.nbytes} contiguous uint8 bytes")
+    with _on_device(filt.device) as stream:
+        adler = torch.empty((len(d),), dtype=torch.int32, device=filt.device)
+        _check(L.nastar_b200_png_filter(d.ctypes.data, desc_dev.data_ptr(), len(d), filt.data_ptr(), filt.numel(),
+                                        adler.data_ptr(), stream), "nastar_b200_png_filter")
+    return adler
+
+
+def png_finish(desc, desc_dev: torch.Tensor, out_off: torch.Tensor, out_len: torch.Tensor, adler: torch.Tensor,
+               out: torch.Tensor) -> None:
+    """The third PNG encode launch (nastar_b200_png_finish): each file's head and tail around its deflate stream in
+    `out`, on the current stream."""
+    L = lib()
+    d = np.ascontiguousarray(desc, dtype=PNG_ENC_DESC_DTYPE)
+    with _on_device(out.device) as stream:
+        _check(L.nastar_b200_png_finish(d.ctypes.data, desc_dev.data_ptr(), len(d), out_off.data_ptr(),
+                                        out_len.data_ptr(), adler.data_ptr(), out.data_ptr(), out.numel(), stream),
+               "nastar_b200_png_finish")
 
 
 # NASTAR_GIF_* (include/nastar_b200.h)

@@ -1096,9 +1096,124 @@ def save_planning_dataset(path: str, train, valid, test) -> None:
         np.savez_compressed(path, *arrays)
 
 
+def encode_pngs(images) -> list:
+    """PNG files of 8-bit grey images, encoded on the GPU (DESIGN.md §21): colour type 0, not interlaced, one IDAT
+    chunk each.  Every scanline takes the filter type 0..4 with the least sum of |byte as int8| (libpng's heuristic,
+    ties to the lowest type), the filtered streams are deflated by nastar_b200_deflate and each file's chunks, CRCs and
+    Adler-32 are written around its stream on the device: three kernel launches in all.  The host waits twice, once
+    for the files' offsets and once for exactly their bytes.
+
+    images: a CUDA uint8 tensor [B,H,W], or a list of CUDA uint8 [H,W] tensors of any sizes on one device; sides
+    1 .. 2048.  Returns one `bytes` per image, in order.  Non-CUDA images raise RuntimeError: there is no CPU
+    fallback."""
+    if isinstance(images, torch.Tensor):
+        if not images.is_cuda:
+            raise RuntimeError("encode_pngs runs on CUDA tensors only (there is no CPU fallback)")
+        if images.ndim != 3:
+            raise ValueError(f"encode_pngs: images are [B,H,W] (got {tuple(images.shape)})")
+        planes = list(images.detach().contiguous().unbind(0))
+    else:
+        planes = list(images)
+    if not planes:
+        return []
+    if not all(isinstance(p, torch.Tensor) and p.is_cuda for p in planes):
+        raise RuntimeError("encode_pngs runs on CUDA tensors only (there is no CPU fallback)")
+    dev = planes[0].device
+    for p in planes:
+        if p.dtype != torch.uint8:
+            raise TypeError(f"encode_pngs: images are uint8 grey levels (got {p.dtype})")
+        if p.ndim != 2 or not (1 <= p.shape[0] <= _native.PNG_MAX_SIDE and 1 <= p.shape[1] <= _native.PNG_MAX_SIDE):
+            raise ValueError(f"encode_pngs: images are [H,W] with sides 1..{_native.PNG_MAX_SIDE} "
+                             f"(got {tuple(p.shape)})")
+        if p.device != dev:
+            raise ValueError("encode_pngs: every image must be on one device")
+    planes = [p.detach().contiguous() for p in planes]
+    B = len(planes)
+    H = np.array([p.shape[0] for p in planes], np.int64)
+    W = np.array([p.shape[1] for p in planes], np.int64)
+    n = H * (W + 1)
+    foff = np.concatenate([[0], np.cumsum(n)[:-1]])
+    enc = np.zeros(B, _native.PNG_ENC_DESC_DTYPE)
+    enc["pixels"] = [p.data_ptr() for p in planes]
+    enc["filt_off"], enc["W"], enc["H"] = foff, W, H
+    filt = torch.empty((int(n.sum()),), dtype=torch.uint8, device=dev)
+    desc = np.zeros(B, _native.DEFLATE_DESC_DTYPE)
+    desc["data"] = filt.data_ptr() + foff
+    desc["data_len"] = n
+    desc["gap"] = _native.png_gaps(B)
+    desc["chunk0"] = np.concatenate([[0], np.cumsum(_native.deflate_chunk_counts(n))[:-1]])
+    ctl = torch.empty((enc.nbytes + desc.nbytes,), dtype=torch.uint8, pin_memory=True)
+    c = ctl.numpy()
+    c[:enc.nbytes] = enc.view(np.uint8)
+    c[enc.nbytes:] = desc.view(np.uint8)
+    with torch.cuda.device(dev):
+        ctl_dev = torch.empty((ctl.numel(),), dtype=torch.uint8, device=dev)
+        ctl_dev.copy_(ctl, non_blocking=True)
+        enc_dev = ctl_dev[:enc.nbytes]
+        adler = _native.png_filter(enc, enc_dev, filt)
+        out, out_off, out_len, _ = _native.deflate(desc, ctl_dev[enc.nbytes:], tail=_native.PNG_ENC_TAIL)
+        _native.png_finish(enc, enc_dev, out_off, out_len, adler, out)
+        meta = torch.cat([out_off, out_len]).to("cpu", non_blocking=True)
+        torch.cuda.current_stream(dev).synchronize()   # the files' offsets
+        meta = meta.numpy().reshape(2, B)
+        starts = meta[0] - _native.PNG_ENC_HEAD
+        ends = meta[0] + meta[1] + _native.PNG_ENC_TAIL
+        image = torch.empty((int(ends[-1]),), dtype=torch.uint8, pin_memory=True)
+        image.copy_(out[:int(ends[-1])], non_blocking=True)
+        torch.cuda.current_stream(dev).synchronize()   # exactly the files' bytes, known only after the first wait
+    del planes, filt, ctl
+    img = image.numpy()
+    return [img[a:b].tobytes() for a, b in zip(starts.tolist(), ends.tolist())]
+
+
+def save_pngs(paths, images) -> None:
+    """Write image i of `images` (what encode_pngs takes) as a PNG file to paths[i], every file encoded on the GPU in
+    one encode_pngs call."""
+    paths = list(paths)
+    n = images.shape[0] if isinstance(images, torch.Tensor) and images.ndim == 3 else len(images)
+    if len(paths) != n:
+        raise ValueError(f"save_pngs: {len(paths)} paths for {n} images")
+    for path, blob in zip(paths, encode_pngs(images)):
+        with open(path, "wb") as f:
+            f.write(blob)
+
+
+STREET_SPLITS = ("train", "validation", "test")
+
+
+def street_crop_boxes(train_files, test_files, size: int = 128, counts=(160, 20, 40), seed: int = 1372,
+                      source_size: int = 256):
+    """The crop boxes of the CSM street maps (planning-datasets' preprocess_street_dataset.py, crop_images), replayed
+    on the host: np.random.RandomState(seed) draws randint(0, source_size - size, [count, 2]) per file, first for
+    every train file (counts[0] each), then for the same train files again (validation, counts[1] each), then for every
+    test file (counts[2] each).  A draw's row (left, top) is the box (left, top, left + size, top + size) of the
+    source resized to source_size x source_size, saved as "<fileid>_<n:05d>.png" with fileid the file name before
+    "_256.png".
+
+    train_files, test_files: the sources in the order the draws take them (the generator takes glob order).  Returns
+    {split: dict(source int64 [N] (index into that split's file list), n, left, top int64 [N], name list of str)}."""
+    import re
+
+    rng = np.random.RandomState(seed)
+    result = {}
+    for split, files, count in zip(STREET_SPLITS, (train_files, train_files, test_files), counts):
+        src, n, lt, names = [], [], [], []
+        for k, f in enumerate(files):
+            fileid = re.split("_256.png", re.split("/", os.fspath(f))[-1])[0]
+            draw = rng.randint(0, source_size - size, [int(count), 2])
+            src += [k] * int(count)
+            n += list(range(int(count)))
+            lt.append(draw)
+            names += ["%s_%05d.png" % (fileid, i) for i in range(int(count))]
+        lt = np.concatenate(lt).astype(np.int64) if lt else np.zeros((0, 2), np.int64)
+        result[split] = dict(source=np.array(src, np.int64), n=np.array(n, np.int64), left=lt[:, 0], top=lt[:, 1],
+                             name=names)
+    return result
+
+
 __all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "MazeDataset", "WarCraftDataset",
            "compute_opt_labels", "compute_weighted_opt_labels", "create_dataloader", "create_device_dataloader",
-           "create_warcraft_dataloader", "draw_opt_policies", "load_map_images", "maps_from_images",
-           "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset", "save_search_gifs",
+           "create_warcraft_dataloader", "draw_opt_policies", "encode_pngs", "load_map_images", "maps_from_images",
+           "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset", "save_pngs", "save_search_gifs",
            "savez_compressed_device", "save_warcraft_dataset", "search_gifs",
-           "shortest_path_maps", "tile_maps", "visualize_results"]
+           "shortest_path_maps", "street_crop_boxes", "tile_maps", "visualize_results"]
