@@ -518,6 +518,35 @@ int64_t nastar_b200_png_gap(int32_t i);
  * image's 20-byte tail; -1 for descriptors nastar_b200_png_filter rejects. */
 int64_t nastar_b200_png_encode_bound(const nastar_png_enc_desc *desc, int32_t B);
 
+/* One source image of nastar_b200_crop_resize_rgb.  pixels is a device address. */
+typedef struct nastar_rgb_image {
+    const uint8_t *pixels; /* H rows of W RGB triples, row y at pixels + y * pitch */
+    int64_t pitch;         /* bytes between rows, >= 3 W */
+    int32_t W, H;          /* 1 .. 4096 each */
+} nastar_rgb_image;
+
+/* One crop of nastar_b200_crop_resize_rgb: the box [x0, x1) x [y0, y1) of image `src` in its pixels, which may extend
+ * past any edge, resized into output image `out`. */
+typedef struct nastar_rgb_crop {
+    int32_t src, out;
+    int32_t x0, y0, x1, y1;
+} nastar_rgb_crop;
+
+/* RGB crops resized to Wo x Ho, bit-equal to Pillow's np.array(image.crop(box).resize((Wo, Ho))) (BICUBIC,
+ * reducing_gap=None) for an RGB image (DESIGN.md §22).  A box pixel outside its source is 0 in every channel; each
+ * channel is resized as Pillow resizes an L image: a horizontal pass into a uint8 intermediate when x1 - x0 != Wo,
+ * then a vertical pass when y1 - y0 != Ho, with 22-bit fixed-point weights.  Writes out uint8 [N][Ho][Wo][3], crop i
+ * to image crops[i].out.  src / crops: the S images and N crops in HOST memory, read for the checks; src_dev /
+ * crops_dev: the same descriptors in device memory, read by the kernel.  CTA i takes crops[i], so list the largest
+ * boxes first: the long CTAs then start first.  Every check precedes the launch: null pointers (a pixels pointer
+ * included), S, N, Ho or Wo <= 0, a side <= 0, a pitch below 3 W, a src outside [0, S), out indices that are not a
+ * permutation of 0 .. N-1, or an empty box (x1 <= x0 or y1 <= y0) give NASTAR_EINVAL; a source side or box side above
+ * 4096, or Ho or Wo above 1024, gives NASTAR_EUNSUPPORTED.  Needs no workspace.  One kernel launch (one CTA per crop).
+ * Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_crop_resize_rgb(const nastar_rgb_image *src, const nastar_rgb_image *src_dev, int32_t S,
+                                const nastar_rgb_crop *crops, const nastar_rgb_crop *crops_dev, int32_t N, int32_t Ho,
+                                int32_t Wo, uint8_t *out, void *stream);
+
 /* Search animations (DESIGN.md §19): G GIFs over a search of B maps, layout NASTAR_GIF_EACH (one GIF per map, G = B)
  * or NASTAR_GIF_GRID (one GIF of all maps in make_grid's layout: 8 per row, 2-pixel border, none for B = 1).  GIF g
  * has T_g steps and T_g + 1 frames, numbered GIF by GIF: frame k < T_g is the closed set before step k and the cell

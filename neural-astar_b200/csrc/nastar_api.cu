@@ -7,10 +7,12 @@
 #include <cstdlib>
 #include <cstring>
 #include <type_traits>
+#include <vector>
 
 #include "../../include/nastar_b200.h"
 #include "nastar_bin16.cuh"
 #include "nastar_convhead.cuh"
+#include "nastar_crops.cuh"
 #include "nastar_deflate.cuh"
 #include "nastar_generic.cuh"
 #include "nastar_gif.cuh"
@@ -1107,6 +1109,40 @@ int nastar_b200_png_finish(const nastar_png_enc_desc* desc, const nastar_png_enc
     if (out_bytes < bound) return NASTAR_EWORKSPACE;
     const nastar::PngFinishArgs a{desc_dev, out_off, out_len, adler, out, out_bytes};
     const cudaError_t e = launch_smem(nastar::png_finish_kernel, B, nastar::kPngEncThreads, 0,
+                                      static_cast<cudaStream_t>(stream_v), a);
+    if (e != cudaSuccess) return cuda_fail(e);
+    return launched();
+}
+
+int nastar_b200_crop_resize_rgb(const nastar_rgb_image* src, const nastar_rgb_image* src_dev, int32_t S,
+                                const nastar_rgb_crop* crops, const nastar_rgb_crop* crops_dev, int32_t N, int32_t Ho,
+                                int32_t Wo, uint8_t* out, void* stream_v) {
+    if (!src || !src_dev || !crops || !crops_dev || !out || S <= 0 || N <= 0 || Ho <= 0 || Wo <= 0)
+        return NASTAR_EINVAL;
+    // an invalid descriptor takes precedence over an unsupported one found earlier
+    int st = Ho > nastar::kCropMaxOut || Wo > nastar::kCropMaxOut ? NASTAR_EUNSUPPORTED : NASTAR_OK;
+    for (int32_t i = 0; i < S; ++i) {
+        const nastar_rgb_image& m = src[i];
+        if (!m.pixels || m.W <= 0 || m.H <= 0 || m.pitch < int64_t(m.W) * 3) return NASTAR_EINVAL;
+        if (m.W > nastar::kCropMaxSide || m.H > nastar::kCropMaxSide) st = NASTAR_EUNSUPPORTED;
+    }
+    std::vector<uint8_t> seen(size_t(N), 0);
+    size_t smem = nastar::kCropSmemTarget;
+    for (int32_t i = 0; i < N; ++i) {
+        const nastar_rgb_crop& c = crops[i];
+        const int64_t cw = int64_t(c.x1) - c.x0, ch = int64_t(c.y1) - c.y0;
+        if (c.src < 0 || c.src >= S || c.out < 0 || c.out >= N || seen[c.out] || cw <= 0 || ch <= 0)
+            return NASTAR_EINVAL;
+        seen[c.out] = 1;
+        if (cw > nastar::kCropMaxSide || ch > nastar::kCropMaxSide) st = NASTAR_EUNSUPPORTED;
+        if (st != NASTAR_OK) continue;
+        const size_t need = nastar::crop_smem_need(int(cw), int(ch), Ho, Wo);
+        smem = need > smem ? need : smem;
+    }
+    if (st != NASTAR_OK) return st;
+    if (smem > kMaxDynSmem) return NASTAR_EUNSUPPORTED;
+    const nastar::CropArgs a{src_dev, crops_dev, Ho, Wo, int64_t(smem), out};
+    const cudaError_t e = launch_smem(nastar::crop_resize_rgb_kernel, N, nastar::kCropThreads, smem,
                                       static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();

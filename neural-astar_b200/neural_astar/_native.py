@@ -116,6 +116,7 @@ _SIGNATURES = {
     "nastar_b200_png_finish": (_int, [_p, _p, _i32, _p, _p, _p, _p, _i64, _p]),
     "nastar_b200_png_gap": (_i64, [_i32]),
     "nastar_b200_png_encode_bound": (_i64, [_p, _i32]),
+    "nastar_b200_crop_resize_rgb": (_int, [_p, _p, _i32, _p, _p] + [_i32] * 3 + [_p, _p]),
     "nastar_b200_gif_tables_bytes": (_i64, [ctypes.POINTER(GifParams)]),
     "nastar_b200_gif_plan": (_int, [ctypes.POINTER(GifParams), _p, _p, _p, ctypes.c_size_t, _p]),
     "nastar_b200_gif_record_bytes": (_i64, [_i64]),
@@ -959,6 +960,62 @@ def png_finish(desc, desc_dev: torch.Tensor, out_off: torch.Tensor, out_len: tor
         _check(L.nastar_b200_png_finish(d.ctypes.data, desc_dev.data_ptr(), len(d), out_off.data_ptr(),
                                         out_len.data_ptr(), adler.data_ptr(), out.data_ptr(), out.numel(), stream),
                "nastar_b200_png_finish")
+
+
+# struct nastar_rgb_image / nastar_rgb_crop (include/nastar_b200.h) as NumPy records
+RGB_IMAGE_DTYPE = np.dtype([("pixels", "<u8"), ("pitch", "<i8"), ("W", "<i4"), ("H", "<i4")])
+RGB_CROP_DTYPE = np.dtype([("src", "<i4"), ("out", "<i4"), ("x0", "<i4"), ("y0", "<i4"), ("x1", "<i4"),
+                           ("y1", "<i4")])
+CROP_MAX_SIDE = 4096   # source and box sides
+CROP_MAX_OUT = 1024    # Ho, Wo
+
+
+def crop_resize_rgb(images, src, boxes, Ho: int, Wo: int) -> torch.Tensor:
+    """RGB crops resized to Wo x Ho in one kernel (include/nastar_b200.h, nastar_b200_crop_resize_rgb), bit-equal to
+    Pillow's image.crop(box).resize((Wo, Ho)).
+
+    images: S uint8 CUDA tensors [H,W,3] on one device (rows may be strided; pixels within a row contiguous); src:
+    int [N] source indices; boxes: int [N,4] (x0, y0, x1, y1), past any edge allowed.  Returns uint8 [N,Ho,Wo,3] on
+    the current stream.  The CTAs take the crops in descending box area, so the largest start first."""
+    L = lib()
+    images = list(images)
+    if not images or any(not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8 for t in images):
+        raise RuntimeError("crop_resize_rgb: uint8 CUDA images only (there is no CPU fallback)")
+    dev = images[0].device
+    keep = []
+    img = np.zeros(len(images), RGB_IMAGE_DTYPE)
+    for i, t in enumerate(images):
+        if t.ndim != 3 or t.shape[2] != 3 or t.device != dev:
+            raise ValueError(f"crop_resize_rgb: images are [H,W,3] on one device (image {i}: {tuple(t.shape)})")
+        if t.stride(2) != 1 or t.stride(1) != 3:
+            t = t.contiguous()
+        keep.append(t)
+        img[i] = (t.data_ptr(), t.stride(0), t.shape[1], t.shape[0])
+    src = np.asarray(src, np.int64).reshape(-1)
+    boxes = np.asarray(boxes, np.int64).reshape(-1, 4)
+    N = len(src)
+    if len(boxes) != N or N == 0:
+        raise ValueError(f"crop_resize_rgb: one box per source index, at least one (got {len(boxes)} and {N})")
+    if boxes.min() < -2 ** 31 or boxes.max() >= 2 ** 31:
+        raise ValueError("crop_resize_rgb: box coordinates must fit int32")
+    area = (boxes[:, 2] - boxes[:, 0]) * (boxes[:, 3] - boxes[:, 1])
+    order = np.argsort(-area, kind="stable")
+    crops = np.zeros(N, RGB_CROP_DTYPE)
+    crops["src"], crops["out"] = src[order], order
+    crops["x0"], crops["y0"], crops["x1"], crops["y1"] = boxes[order].T
+    ctl = torch.empty((img.nbytes + crops.nbytes,), dtype=torch.uint8, pin_memory=True)
+    c = ctl.numpy()
+    c[:img.nbytes] = img.view(np.uint8)
+    c[img.nbytes:] = crops.view(np.uint8)
+    with _on_device(dev) as stream:
+        ctl_dev = torch.empty((ctl.numel(),), dtype=torch.uint8, device=dev)
+        ctl_dev.copy_(ctl, non_blocking=True)
+        out = torch.empty((N, int(Ho), int(Wo), 3), dtype=torch.uint8, device=dev)
+        _check(L.nastar_b200_crop_resize_rgb(img.ctypes.data, ctl_dev.data_ptr(), len(img), crops.ctypes.data,
+                                             ctl_dev.data_ptr() + img.nbytes, N, int(Ho), int(Wo), out.data_ptr(),
+                                             stream), "nastar_b200_crop_resize_rgb")
+    del keep
+    return out
 
 
 # NASTAR_GIF_* (include/nastar_b200.h)

@@ -9,6 +9,7 @@ and the WarCraft `.npy` pairs (:273-282).
 """
 from __future__ import annotations
 
+import functools
 import os
 
 import numpy as np
@@ -953,6 +954,7 @@ _ZIP_DOS_DATE = (0 << 9) | (1 << 5) | 1   # 1980-01-01 00:00:00: archives do not
 _U32 = 0xFFFFFFFF
 
 
+@functools.lru_cache(maxsize=None)
 def _npy_header(dtype: np.dtype, shape) -> bytes:
     """The header np.save writes for a C-order array of this dtype and shape (format 1.0, or 2.0 when it must)."""
     import io
@@ -1018,15 +1020,38 @@ def savez_compressed_device(file, *args, **kwds) -> None:
         members[k] = a
     if not members:
         raise ValueError("savez_compressed_device: nothing to save")
-    tensors = list(members.values())
+    _savez_compressed_many([(file, members)])
+
+
+_NP_DTYPE = {}
+
+
+def _np_dtype(dtype: torch.dtype) -> np.dtype:
+    if dtype not in _NP_DTYPE:
+        _NP_DTYPE[dtype] = torch.empty(0, dtype=dtype).numpy().dtype
+    return _NP_DTYPE[dtype]
+
+
+def _savez_compressed_many(files) -> None:
+    """savez_compressed_device for many archives at once: files is a list of (file, members), members a dict of
+    member name (without ".npy") -> CUDA tensor, every tensor of every file on one device.  All members of all files
+    are deflated in one nastar_b200_deflate launch, and the host waits twice in all, once for the compressed sizes and
+    CRCs and once for exactly the compressed bytes; each archive is then finished (_zip_finish) and written.  `file`:
+    a path (".npz" is appended when missing) or a writable binary file."""
+    names, tensors, first = [], [], [0]
+    for _, members in files:
+        if not members:
+            raise ValueError("savez_compressed_device: nothing to save")
+        names += [(k + ".npy").encode() for k in members]
+        tensors += list(members.values())
+        first.append(len(tensors))
     if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in tensors):
         raise RuntimeError("savez_compressed_device: every array must be a CUDA tensor (there is no CPU fallback)")
     dev = tensors[0].device
     if any(t.device != dev for t in tensors):
         raise ValueError("savez_compressed_device: every tensor must be on one device")
-    names = [(k + ".npy").encode() for k in members]
     flat = [t.detach().contiguous().reshape(-1) for t in tensors]
-    heads = [_npy_header(torch.empty(0, dtype=t.dtype).numpy().dtype, t.shape) for t in tensors]
+    heads = [_npy_header(_np_dtype(t.dtype), tuple(t.shape)) for t in tensors]
     data = [f.view(torch.uint8) if f.numel() else f for f in flat]
     M = len(tensors)
     desc = np.zeros(M, _native.DEFLATE_DESC_DTYPE)
@@ -1035,11 +1060,12 @@ def savez_compressed_device(file, *args, **kwds) -> None:
     hoff = np.concatenate([[0], np.cumsum(hlen)])
     ctl = torch.empty((int(hoff[-1]) + desc.nbytes,), dtype=torch.uint8, pin_memory=True)
     ctl_dev = torch.empty((ctl.numel(),), dtype=torch.uint8, device=dev)
+    gaps = np.array([_zip_local_header_bytes(n) for n in names], np.int64)
     desc["head"] = ctl_dev.data_ptr() + hoff[:-1]
     desc["head_len"] = hlen
     desc["data"] = [d.data_ptr() if n else 0 for d, n in zip(data, dlen)]
     desc["data_len"] = dlen
-    desc["gap"] = [_zip_local_header_bytes(n) for n in names]
+    desc["gap"] = gaps
     desc["chunk0"] = np.concatenate([[0], np.cumsum(_native.deflate_chunk_counts(dlen))[:-1]])
     c = ctl.numpy()
     c[:hoff[-1]] = np.frombuffer(b"".join(heads), np.uint8)
@@ -1057,17 +1083,22 @@ def savez_compressed_device(file, *args, **kwds) -> None:
         torch.cuda.current_stream(dev).synchronize()   # exactly the compressed bytes, known only after the first wait
     del flat, data, ctl
     img = image.numpy()
-    tail = _zip_finish(img, names, offs, csizes, (hlen + dlen).tolist(), crcs)
-    if isinstance(file, (str, os.PathLike)):
-        file = os.fspath(file)
-        if not file.endswith(".npz"):
-            file += ".npz"
-        with open(file, "wb") as f:
-            f.write(memoryview(img))
-            f.write(tail)
-    else:
-        file.write(memoryview(img))
-        file.write(tail)
+    usizes = (hlen + dlen).tolist()
+    for f, (file, _) in enumerate(files):
+        a, b = first[f], first[f + 1]
+        start = offs[a] - int(gaps[a])   # the archive's first local header; the archives lie back to back
+        part = img[start:offs[b - 1] + csizes[b - 1]]
+        tail = _zip_finish(part, names[a:b], [o - start for o in offs[a:b]], csizes[a:b], usizes[a:b], crcs[a:b])
+        if isinstance(file, (str, os.PathLike)):
+            file = os.fspath(file)
+            if not file.endswith(".npz"):
+                file += ".npz"
+            with open(file, "wb") as fh:
+                fh.write(memoryview(part))
+                fh.write(tail)
+        else:
+            file.write(memoryview(part))
+            file.write(tail)
 
 
 def save_planning_dataset(path: str, train, valid, test) -> None:
@@ -1211,9 +1242,212 @@ def street_crop_boxes(train_files, test_files, size: int = 128, counts=(160, 20,
     return result
 
 
+SDD_LABELS = {"Pedestrian": 0, "Biker": 1, "Skater": 2, "Car": 3, "Cart": 4, "Bus": 5}
+
+
+def read_sdd_annotations(path: str):
+    """A Stanford Drone `annotations.txt`: space-separated rows `id xmin ymin xmax ymax frame lost occluded generated
+    "label"` (the label quoted).  Returns (int64 [n, 9] of the first nine columns, list of the n labels without their
+    quotes)."""
+    with open(path, "rb") as f:
+        text = f.read()
+    tok = text.split()
+    if len(tok) != 10 * sum(1 for ln in text.splitlines() if ln.strip()):
+        raise ValueError(f"{path}: every annotation row has 10 space-separated columns")
+    tok = np.array(tok).reshape(-1, 10)
+    names, which = np.unique(tok[:, 9], return_inverse=True)
+    names = np.array([n.decode().strip('"') for n in names] or [""])
+    return tok[:, :9].astype(np.int64), list(names[which.reshape(-1)])
+
+
+def sdd_sample_plan(video_dir: str, W: int = 64, min_len_ratio: float = 0.5, min_max_size: int = 128,
+                    max_step: int = 600, rng=None) -> dict:
+    """The samples planning-datasets' SDD.py (create_sample_from_dataset) makes of one Stanford Drone video directory
+    (`reference.jpg` and `annotations.txt`), planned on the host without decoding the scene (DESIGN.md §22).
+
+    Ids are visited in order of first appearance; each id's visible segments are its maximal runs of rows with
+    lost == 0, numbered 1, 2, ...  A segment longer than max_step takes a window of max_step rows starting at
+    rng.randint(0, len - max_step), drawn before the segment is judged, so rejected segments draw too.  The segment is
+    kept when its start-to-goal length is > 0, its length ratio > min_len_ratio and its larger extent > min_max_size;
+    the ROI, the resized trajectory and the ratio are the reference's float64 expressions, evaluated with the same
+    NumPy calls.  rng: a np.random.RandomState shared across videos (None: NumPy's global state, as the reference).
+
+    Returns dict(scene, video (the directory's last two components), name list of "%08d_%02d.npz", box int64 [K, 4]
+    (Image.crop's box after Python's round, half to even), traj list of float64 [n, 2] (traj_resized), label int64
+    [K], length_ratio float64 [K], start, goal int64 [K, 2] (row, column), cells list of int64 [m, 2] (row, column)
+    of the trajectory image's set cells)."""
+    from PIL import Image
+
+    rng = np.random if rng is None else rng
+    parts = os.path.normpath(os.fspath(video_dir)).split(os.sep)
+    with Image.open(os.path.join(video_dir, "reference.jpg")) as im:
+        size = im.size
+    cols, labels = read_sdd_annotations(os.path.join(video_dir, "annotations.txt"))
+    ids = cols[:, 0]
+    uniq, first = np.unique(ids, return_index=True)
+    perm = np.argsort(ids, kind="stable")   # each id's rows, in file order
+    bounds = np.searchsorted(ids[perm], uniq)
+    rows_of = {int(u): perm[b:e] for u, b, e in zip(uniq, bounds, np.append(bounds[1:], len(ids)))}
+    plan = dict(scene=parts[-2], video=parts[-1], name=[], box=[], traj=[], label=[], length_ratio=[], start=[],
+                goal=[], cells=[])
+    for id_ in uniq[np.argsort(first)]:
+        rows = rows_of[int(id_)]
+        sample = cols[rows]
+        visible = sample[:, 6] == 0
+        starts = np.flatnonzero(visible & ~np.concatenate([[False], visible[:-1]]))
+        ends = np.flatnonzero(visible & ~np.concatenate([visible[1:], [False]])) + 1
+        for vl, (a, b) in enumerate(zip(starts, ends), 1):
+            seg = sample[a:b]
+            traj = (seg[:, 1:3] + seg[:, 3:5]) / 2.
+            if len(traj) > max_step:
+                s0 = rng.randint(0, len(traj) - max_step)
+                traj = traj[s0:s0 + max_step, :]
+            max_size = np.max(traj.max(axis=0) - traj.min(axis=0), 0)
+            mean_loc = traj.min(axis=0) + (traj.max(axis=0) - traj.min(axis=0)) / 2
+            if np.all(mean_loc - max_size / 2 - 50 > 0):
+                min_loc = np.maximum(mean_loc - max_size / 2 - 50, 0)
+                max_loc = min_loc + max_size + 100
+            else:
+                max_loc = np.minimum(mean_loc + max_size / 2 + 50, size)
+                min_loc = max_loc - max_size - 100
+            all_length = np.abs(np.diff(traj, axis=0)).sum()
+            sg_length = np.abs(np.diff(traj[[0, -1]], axis=0)).sum()
+            length_ratio = sg_length / (all_length + 1e-5)
+            if not ((sg_length > 0) & (length_ratio > min_len_ratio) & (max_size > min_max_size)):
+                continue
+            label = labels[rows[0]]
+            if label not in SDD_LABELS:
+                raise ValueError(f"{video_dir}: unknown label {label!r} (id {int(id_)})")
+            tr = (traj - min_loc) / (max_size + 100) * W
+            tr[tr > W - 1] = W - 1
+            tr[tr < 0] = 0
+            dense = np.arange(len(tr) * 5)
+            knots = np.arange(0, 5 * len(tr), 5)
+            t0, t1 = np.interp(dense, knots, tr[:, 0]), np.interp(dense, knots, tr[:, 1])
+            # np.histogram2d(t1, t0, range(W + 1)) puts v in [0, W - 1] in bin floor(v)
+            cell = np.unique(np.floor(t1).astype(np.int64) * W + np.floor(t0).astype(np.int64))
+            plan["name"].append("%08d_%02d.npz" % (id_, vl))
+            plan["box"].append([round(float(v)) for v in (min_loc[0], min_loc[1], max_loc[0], max_loc[1])])
+            plan["traj"].append(tr)
+            plan["label"].append(SDD_LABELS[label])
+            plan["length_ratio"].append(length_ratio)
+            plan["start"].append([int(tr[0, 1]), int(tr[0, 0])])
+            plan["goal"].append([int(tr[-1, 1]), int(tr[-1, 0])])
+            plan["cells"].append(np.stack([cell // W, cell % W], axis=1))
+    plan["box"] = np.array(plan["box"], np.int64).reshape(-1, 4)
+    plan["label"] = np.array(plan["label"], np.int64)
+    plan["length_ratio"] = np.array(plan["length_ratio"], np.float64)
+    plan["start"] = np.array(plan["start"], np.int64).reshape(-1, 2)
+    plan["goal"] = np.array(plan["goal"], np.int64).reshape(-1, 2)
+    return plan
+
+
+def sdd_crops(scenes, boxes, size, src=None) -> torch.Tensor:
+    """RGB crops of scenes resized on the GPU, bit-equal to Pillow's np.array(scene.crop(box).resize(size)) (BICUBIC)
+    for an RGB scene: one kernel launch for all crops (include/nastar_b200.h, nastar_b200_crop_resize_rgb).
+
+    scenes: a CUDA uint8 [H,W,3] tensor or a list of them on one device (sides <= 4096); boxes: int [N, 4]
+    (left, top, right, bottom) in pixels, non-empty, sides <= 4096, past any edge allowed (those pixels are 0);
+    size: int or Pillow's (width, height), each <= 1024; src: [N] scene index of each box (None: all 0).  Returns
+    uint8 [N, height, width, 3] on the scenes' device."""
+    scenes = [scenes] if isinstance(scenes, torch.Tensor) else list(scenes)
+    Wo, Ho = (int(size), int(size)) if np.ndim(size) == 0 else (int(size[0]), int(size[1]))
+    boxes = np.asarray(boxes, np.int64).reshape(-1, 4)
+    src = np.zeros(len(boxes), np.int64) if src is None else np.asarray(src, np.int64).reshape(-1)
+    return _native.crop_resize_rgb(scenes, src, boxes, Ho, Wo)
+
+
+def _sdd_scene(video_dir: str, device) -> torch.Tensor:
+    """reference.jpg decoded by Pillow on the host and uploaded, uint8 [H, W, 3]."""
+    from PIL import Image
+
+    path = os.path.join(video_dir, "reference.jpg")
+    with Image.open(path) as im:
+        if im.mode != "RGB":
+            raise ValueError(f"{path}: the scene decodes to mode {im.mode!r}, not RGB")
+        pixels = np.array(im)
+    return torch.from_numpy(pixels).to(device)
+
+
+def _write_sdd_samples(batch, W: int, device) -> None:
+    """One batch of (plan, scene, directory) of save_sdd_samples: one crop launch, planes built on the device, one
+    deflate launch for all files."""
+    plans = [p for p, _, _ in batch]
+    K = sum(len(p["name"]) for p in plans)
+    if K == 0:
+        return
+    scenes = [s for _, s, _ in batch]
+    src = np.concatenate([np.full(len(p["name"]), i, np.int64) for i, p in enumerate(plans)])
+    images = sdd_crops(scenes, np.concatenate([p["box"] for p in plans]), W, src)
+    # start_image, goal_image and traj_image of every sample: 1.0 at the plan's cells
+    k_traj = np.concatenate([np.full(len(c), k, np.int64) for k, c in
+                             enumerate(c for p in plans for c in p["cells"])])
+    cells = np.concatenate([c for p in plans for c in p["cells"]])
+    start = np.concatenate([p["start"] for p in plans])
+    goal = np.concatenate([p["goal"] for p in plans])
+    k = np.arange(K)
+    idx = np.concatenate([np.stack([np.zeros(K, np.int64), k, start[:, 0], start[:, 1]]),
+                          np.stack([np.ones(K, np.int64), k, goal[:, 0], goal[:, 1]]),
+                          np.stack([np.full(len(cells), 2, np.int64), k_traj, cells[:, 0], cells[:, 1]])], axis=1)
+    trajs = [t for p in plans for t in p["traj"]]
+    toff = np.concatenate([[0], np.cumsum([len(t) for t in trajs])])
+    host = np.concatenate([idx.reshape(-1).view(np.float64), np.concatenate(trajs).reshape(-1),
+                           np.concatenate([p["label"] for p in plans]).view(np.float64),
+                           np.concatenate([p["length_ratio"] for p in plans])])
+    up = torch.from_numpy(host).pin_memory().to(device, non_blocking=True)
+    n_idx = idx.size
+    idx_d = up[:n_idx].view(torch.int64).view(4, -1)
+    traj_d = up[n_idx:n_idx + 2 * int(toff[-1])].view(-1, 2)
+    label_d = up[n_idx + 2 * int(toff[-1]):n_idx + 2 * int(toff[-1]) + K].view(torch.int64)
+    ratio_d = up[n_idx + 2 * int(toff[-1]) + K:]
+    planes = torch.zeros((3, K, W, W), dtype=torch.float64, device=device)
+    planes[idx_d[0], idx_d[1], idx_d[2], idx_d[3]] = 1.0
+    files, k = [], 0
+    for p, _, out_dir in batch:
+        for name in p["name"]:
+            files.append((os.path.join(out_dir, name), dict(
+                image=images[k], start_image=planes[0, k], goal_image=planes[1, k], traj_image=planes[2, k],
+                traj=traj_d[toff[k]:toff[k + 1]], label=label_d[k], length_ratio=ratio_d[k])))
+            k += 1
+    _savez_compressed_many(files)
+
+
+def save_sdd_samples(video_dirs, save_dir: str, W: int = 64, min_len_ratio: float = 0.5, min_max_size: int = 128,
+                     max_step: int = 300, rng=None, device=None, batch_samples: int = 4096) -> int:
+    """planning-datasets' SDD samples (create_sample_from_dataset over `video_dirs`, in the order given) written on the
+    GPU (DESIGN.md §22): for each video directory, `<save_dir>/<scene>/<video>/` is created (also when it gets no
+    samples) and every kept sample of sdd_sample_plan is written there as `%08d_%02d.npz` with members image (uint8
+    [W, W, 3]), start_image, goal_image, traj_image (float64 [W, W]), traj (float64 [n, 2]), label (int64) and
+    length_ratio (float64), loading equal to the reference's files.  Scenes are decoded by Pillow on the host and
+    must be RGB; the crops are resized by one kernel launch and the files deflated by one more per batch of about
+    `batch_samples` samples.  rng: a np.random.RandomState (None: RandomState(0), the generator script's
+    np.random.seed(0)).  device: a CUDA device (None: the current one).  Returns the number of files written."""
+    rng = np.random.RandomState(0) if rng is None else rng
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.type != "cuda":
+        raise RuntimeError("save_sdd_samples runs on a CUDA device (there is no CPU fallback)")
+    batch, n, total = [], 0, 0
+    for video_dir in video_dirs:
+        plan = sdd_sample_plan(video_dir, W, min_len_ratio, min_max_size, max_step, rng)
+        out_dir = os.path.join(save_dir, plan["scene"], plan["video"])
+        os.makedirs(out_dir, exist_ok=True)
+        if not plan["name"]:
+            continue
+        batch.append((plan, _sdd_scene(video_dir, dev), out_dir))
+        n += len(plan["name"])
+        if n >= batch_samples:
+            _write_sdd_samples(batch, W, dev)
+            total += n
+            batch, n = [], 0
+    _write_sdd_samples(batch, W, dev)
+    return total + n
+
+
 __all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "MazeDataset", "WarCraftDataset",
            "compute_opt_labels", "compute_weighted_opt_labels", "create_dataloader", "create_device_dataloader",
            "create_warcraft_dataloader", "draw_opt_policies", "encode_pngs", "load_map_images", "maps_from_images",
-           "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset", "save_pngs", "save_search_gifs",
+           "read_sdd_annotations", "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset",
+           "save_pngs", "save_sdd_samples", "save_search_gifs",
            "savez_compressed_device", "save_warcraft_dataset", "search_gifs",
-           "shortest_path_maps", "street_crop_boxes", "tile_maps", "visualize_results"]
+           "sdd_crops", "sdd_sample_plan", "shortest_path_maps", "street_crop_boxes", "tile_maps",
+           "visualize_results"]
