@@ -198,16 +198,22 @@ def randomise_batchnorm(ref, x: torch.Tensor, rng: np.random.RandomState) -> Non
     with torch.no_grad():
         for m in ref.encoder.model:
             if isinstance(m, nn.BatchNorm2d):
-                C = m.num_features
-                rms = x.pow(2).mean((0, 2, 3)).sqrt().clamp_min(1e-3).numpy()
-                var = 10.0 ** rng.uniform(-3, 1, C)
-                scale = (3.0 if C == 1 else 10.0 ** rng.uniform(-0.5, 0.5, C)) / rms
-                gamma = rng.choice([-1.0, 1.0], C) * scale * np.sqrt(var + m.eps)
-                m.running_var.copy_(_f32(var))
-                m.running_mean.copy_(_f32(0.5 * rms * rng.randn(C)))
-                m.weight.copy_(_f32(gamma))
-                m.bias.copy_(_f32(rng.randn(C) * 0.5))
+                randomise_one_batchnorm(m, x, rng)
             x = m(x)
+
+
+def randomise_one_batchnorm(m: nn.BatchNorm2d, x: torch.Tensor, rng: np.random.RandomState) -> None:
+    """randomise_batchnorm's statistics for one BatchNorm whose input, on the calibration batch, is x."""
+    with torch.no_grad():
+        C = m.num_features
+        rms = x.pow(2).mean((0, 2, 3)).sqrt().clamp_min(1e-3).cpu().numpy()
+        var = 10.0 ** rng.uniform(-3, 1, C)
+        scale = (3.0 if C == 1 else 10.0 ** rng.uniform(-0.5, 0.5, C)) / rms
+        gamma = rng.choice([-1.0, 1.0], C) * scale * np.sqrt(var + m.eps)
+        m.running_var.copy_(_f32(var))
+        m.running_mean.copy_(_f32(0.5 * rms * rng.randn(C)))
+        m.weight.copy_(_f32(gamma))
+        m.bias.copy_(_f32(rng.randn(C) * 0.5))
 
 
 def build_reference(ref_astar, cfg: Config, seed: int):

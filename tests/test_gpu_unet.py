@@ -54,7 +54,7 @@ def test_head_taps_16_channels():
     from neural_astar import _native
 
     torch.manual_seed(0)
-    B, H, W = 37, 32, 32                                    # ragged last 32-pixel group
+    B, H, W = 37, 31, 33                                    # P = 37851: a ragged last 32-pixel group of 27
     x = torch.randn(B, 16, H, W, device="cuda").contiguous(memory_format=torch.channels_last)
     w = np.random.RandomState(0).randn(16, 9).astype(np.float32)
     taps = _native.head_taps(x, w)
