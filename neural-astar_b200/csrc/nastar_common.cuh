@@ -68,13 +68,20 @@ __device__ __forceinline__ float f_value(float gr, float omg, float g, float h) 
     return __fadd_rn(__fmul_rn(gr, g), __fmul_rn(omg, h));
 }
 
+// sqrt(dy^2 + dx^2) as get_heuristic computes it: squares and their sum rounded to fp32 one operation at a time.  Below
+// 4 096 cells every step is exact; beyond, dx*dx exceeds 2^24 and the sum is rounded twice, which an exactly rounded
+// integer sum would not reproduce (at (dy, dx) = (7, 4281) the heuristic would come out one ulp high).
+__device__ __forceinline__ float euclid(int ady, int adx) {
+    const float fy = static_cast<float>(ady), fx = static_cast<float>(adx);
+    return __fsqrt_rn(__fadd_rn(__fmul_rn(fy, fy), __fmul_rn(fx, fx)));
+}
+
 // get_heuristic (differentiable_astar.py:26-52): chebyshev + 0.001 * euclid, all in fp32.
 __device__ __forceinline__ float heuristic(int y, int x, int gy, int gx) {
     int idy = y - gy, idx = x - gx;
     int ady = idy < 0 ? -idy : idy, adx = idx < 0 ? -idx : idx;
     float cheb = static_cast<float>(ady + adx - (ady < adx ? ady : adx));   // exact
-    float euc = __fsqrt_rn(static_cast<float>(ady * ady + adx * adx));       // exact int -> IEEE sqrt
-    return __fadd_rn(cheb, __fmul_rn(0.001f, euc));
+    return __fadd_rn(cheb, __fmul_rn(0.001f, euclid(ady, adx)));
 }
 
 // The generator's NorthEastWestSouth.get_heuristic (planning_datasets_utils/mechanism.py:124-131): manhattan +
@@ -83,8 +90,7 @@ __device__ __forceinline__ float heuristic_news(int y, int x, int gy, int gx) {
     int idy = y - gy, idx = x - gx;
     int ady = idy < 0 ? -idy : idy, adx = idx < 0 ? -idx : idx;
     float manh = static_cast<float>(ady + adx);                               // exact
-    float euc = __fsqrt_rn(static_cast<float>(ady * ady + adx * adx));       // exact int -> IEEE sqrt
-    return __fadd_rn(manh, __fmul_rn(0.001f, euc));
+    return __fadd_rn(manh, __fmul_rn(0.001f, euclid(ady, adx)));
 }
 
 // heuristic of the search's mechanism: kNews = NASTAR_FWD_NEWS / NASTAR_MECH_NEWS (4-connected), else Moore

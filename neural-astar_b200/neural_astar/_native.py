@@ -237,6 +237,21 @@ def mechanism_code(mechanism: str) -> int:
     return MECHANISMS[mechanism]
 
 
+# the loop bound reaches the library as int32_t (nastar_fwd_params.T, the T of nastar_b200_batch_steps, *T_batch)
+MAX_STEPS = 2**31 - 1
+MAX_EVAL_WIDTH = math.isqrt(MAX_STEPS)   # 46 340: the widest map whose evaluation bound W*W fits
+
+
+def check_steps(T: int, what: str = "the step bound T") -> int:
+    """int(T), or a ValueError when T does not fit the library's int32 loop bound (a silent ctypes truncation would
+    search with a wrong bound)."""
+    T = int(T)
+    if T > MAX_STEPS:
+        raise ValueError(f"{what} = {T} exceeds 2**31 - 1, the largest loop bound the search takes: the evaluation "
+                         f"bound W*W fits for W <= {MAX_EVAL_WIDTH} only")
+    return T
+
+
 class SearchCounts(tuple):
     """(n_closed [B'] i32, path_len [B'] i32): histories.sum() / paths.sum() per map, written by the kernel."""
 
@@ -246,6 +261,7 @@ def _search_params(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, 
     """Check the inputs of `forward` / `forward_coupled` and fill their FwdParams up to the outputs.  `flags` gets
     NASTAR_FWD_NEWS added for `mechanism` "news".  Returns (p, planes to keep alive, B, H, W, device)."""
     news = mechanism_code(mechanism) == MECHANISMS["news"]
+    T = check_steps(T)
     lib()
     if not cost.is_cuda:
         raise RuntimeError("neural_astar (H100): the search runs on CUDA tensors only (no CPU fallback); "
@@ -503,6 +519,7 @@ def cost_from_taps(taps: torch.Tensor, bias: float, scale: float) -> torch.Tenso
 
 def batch_steps(t_solve: torch.Tensor, n_steps: torch.Tensor, T: int) -> torch.Tensor:
     """Device-side T_batch (int32[1]); replaces the per-step host sync of differentiable_astar.py:251."""
+    T = check_steps(T)
     L = lib()
     dev = t_solve.device
     with _on_device(dev) as stream:
@@ -846,13 +863,16 @@ def pq_astar(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, map_de
     return hist, paths, status, expansions
 
 
-def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch: torch.Tensor, t_solve: torch.Tensor,
+def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch, t_solve: torch.Tensor,
              g_ratio: float, mechanism: str = "moore") -> torch.Tensor:
     """dL/dcost [B,1,H,W] from dL/dhistories (closed form of the reference's autograd, SURVEY App. B), for a forward
-    that ran with the same `mechanism`."""
+    that ran with the same `mechanism`.  `T_batch` is the replayed step count: an int32 [1] device tensor
+    (batch_steps, forward_coupled) or a Python int, which must fit int32 like the forward's bound."""
     mech = mechanism_code(mechanism)
-    L = lib()
     dev = cost.device
+    if not isinstance(T_batch, torch.Tensor):
+        T_batch = torch.full((1,), check_steps(T_batch, "T_batch"), dtype=torch.int32, device=dev)
+    L = lib()
     B, _, H, W = cost.shape
     p = BwdParams()
     keep = _set_planes(p, (("cost", cost), ("start", start), ("goal", goal), ("obst", obst)))

@@ -17,6 +17,7 @@ import torch
 import torch.nn as nn
 
 from .. import _native
+from .._native import check_steps
 
 
 class AstarOutput(NamedTuple):
@@ -235,6 +236,7 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
         T = self.num_steps(cost_maps.shape[-1])
         if T < 1:
             raise ValueError("Tmax * W * W < 1: the reference loop would not execute (:203)")
+        check_steps(T, f"the step bound int(Tmax * W * W) of a map of width W = {cost_maps.shape[-1]}")
         g_ratio = float(self.g_ratio)
         coupled = batch_coupled(g_ratio, cost_maps.shape[0])
         goal_clamped = None

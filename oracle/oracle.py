@@ -84,12 +84,23 @@ def num_steps(Tmax: float, training: bool, W: int) -> int:
     return int((Tmax if training else 1.0) * W * W)
 
 
+MAX_STEPS = 2**31 - 1   # the C oracle takes the loop bound as a C int
+
+
+def check_steps(T: int) -> int:
+    """int(T), refused with a ValueError above 2**31 - 1 rather than truncated by ctypes into a wrong bound."""
+    T = int(T)
+    if T > MAX_STEPS:
+        raise ValueError(f"step bound {T} exceeds 2**31 - 1, the largest the oracle takes (W*W fits for W <= 46340)")
+    return T
+
+
 def forward(cost, start, goal, obst, g_ratio=0.5, Tmax=1.0, training=False, mode="spec",
             want_trace=False, T=None, no_early_exit=False) -> OracleOutput:
     lib = _load()
     c, s, g, o = _planes(cost), _planes(start), _planes(goal), _planes(obst)
     B, H, W = c.shape
-    T = int(T) if T is not None else num_steps(Tmax, training, W)
+    T = check_steps(T if T is not None else num_steps(Tmax, training, W))
     gr, omg, sq = scalars(g_ratio, W)
     hist = np.zeros((B, H, W), np.float32)
     paths = np.zeros((B, H, W), np.int64)
@@ -123,10 +134,11 @@ def backward(cost, start, goal, obst, grad_hist, T_batch: int, g_ratio=0.5) -> n
     c, s, g, o, gh = _planes(cost), _planes(start), _planes(goal), _planes(obst), _planes(grad_hist)
     B, H, W = c.shape
     gr, omg, sq = scalars(g_ratio, W)
+    T_batch = check_steps(T_batch)
     out = np.zeros((B, H, W), np.float32)
     rc = lib.nastar_oracle_backward(_p(c, ctypes.c_float), _p(s, ctypes.c_float), _p(g, ctypes.c_float),
                                     _p(o, ctypes.c_float), _p(gh, ctypes.c_float), B, H, W, gr, omg, sq,
-                                    int(T_batch), _p(out, ctypes.c_float))
+                                    T_batch, _p(out, ctypes.c_float))
     if rc != 0:
         raise RuntimeError(f"oracle returned {rc}")
     return out[:, None]
