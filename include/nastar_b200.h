@@ -547,6 +547,49 @@ int nastar_b200_crop_resize_rgb(const nastar_rgb_image *src, const nastar_rgb_im
                                 const nastar_rgb_crop *crops, const nastar_rgb_crop *crops_dev, int32_t N, int32_t Ho,
                                 int32_t Wo, uint8_t *out, void *stream);
 
+/* One zip member of a nastar_b200_inflate batch.  Offsets and lengths are in bytes. */
+typedef struct nastar_inflate_desc {
+    int64_t in_off, in_len;    /* the member's stored bytes or raw deflate stream in `data` */
+    int64_t out_off, out_len;  /* its output range in `out`; out_len is its exact size (the central directory's) */
+    int32_t method;            /* the zip compression method: 0 stored, 8 deflated */
+    int32_t reserved;          /* ignored */
+} nastar_inflate_desc;
+
+/* Bytes of the workspace of nastar_b200_inflate: its queue counter. */
+#define NASTAR_INFLATE_WORKSPACE_BYTES 256
+
+/* Zip members to their bytes on the device, each with the CRC-32 of its output: the device half of reading .npz files
+ * (utils.data.load_npz_device, DESIGN.md §23), which replaces np.load's zipfile + zlib inflate on the host.  Per
+ * member: method 8 inflates the raw deflate stream (stored, fixed and dynamic Huffman blocks, with the block decoder of
+ * nastar_b200_decode_png) straight into out[out_off, out_off + out_len), which it must fill exactly; method 0 copies
+ * in_len == out_len bytes.  Writes status i32 [M]: 0, or an OR of 2 bad block type or Huffman code, 4 a distance past
+ * the start of the output, 8 the stream ends early or inflates to more or less than out_len; and crc u32 [M] (passed as
+ * int32), the CRC-32 of the output (unspecified where status is not 0), for the caller to compare with the zip's.  A
+ * corrupt stream reads and writes nothing outside its own ranges.  desc: the M descriptors in HOST memory, read for the
+ * checks; desc_dev: the same descriptors in device memory, read by the kernel.  Every check precedes the launch: null
+ * pointers, M <= 0, a method other than 0 and 8, a negative length, an input range outside data, a stored member whose
+ * lengths differ, or output ranges outside out or not in increasing, disjoint order give NASTAR_EINVAL; a workspace
+ * below NASTAR_INFLATE_WORKSPACE_BYTES gives NASTAR_EWORKSPACE.  One kernel launch (persistent one-warp CTAs taking
+ * members from a queue, so one warp inflates one member: suited to many small members, not to a few huge ones).
+ * Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_inflate(const uint8_t *data, int64_t data_bytes, const nastar_inflate_desc *desc,
+                        const nastar_inflate_desc *desc_dev, int32_t M, uint8_t *out, int64_t out_bytes,
+                        int32_t *status, uint32_t *crc, void *workspace, size_t workspace_bytes, void *stream);
+
+/* Directed Chamfer distances between two cell sets per map, replacing a host loop over
+ * scipy.ndimage.distance_transform_edt (DESIGN.md §23).  masks: uint8 [B][H*W] dense, bit 0 = the cell is in set A,
+ * bit 1 = in set B.  Writes out fp64 [B][2]: d(A -> B) and d(B -> A), d(S -> T) the mean over S's cells of the
+ * Euclidean distance, in cells, to the nearest cell of T; NaN in both columns of a map where A or B is empty.  The
+ * squared distances are exact integers (Meijster's separable transform), each square root is correctly rounded and the
+ * sums run in a fixed order, so results are the same from run to run.  Maps whose state does not fit in shared memory
+ * use one workspace slot per CTA: nastar_b200_chamfer_workspace_bytes (0 when they all fit; workspace may then be
+ * NULL).  Every check precedes the launch: null masks or out, or B, H or W <= 0 give NASTAR_EINVAL; H or W above 1024
+ * gives NASTAR_EUNSUPPORTED; a workspace below nastar_b200_chamfer_workspace_bytes gives NASTAR_EWORKSPACE.  One kernel
+ * launch, one CTA per map.  Asynchronous on `stream`.  Returns NASTAR_*. */
+int nastar_b200_chamfer(const uint8_t *masks, int32_t B, int32_t H, int32_t W, double *out, void *workspace,
+                        size_t workspace_bytes, void *stream);
+size_t nastar_b200_chamfer_workspace_bytes(int32_t B, int32_t H, int32_t W);
+
 /* Search animations (DESIGN.md §19): G GIFs over a search of B maps, layout NASTAR_GIF_EACH (one GIF per map, G = B)
  * or NASTAR_GIF_GRID (one GIF of all maps in make_grid's layout: 8 per row, 2-pixel border, none for B = 1).  GIF g
  * has T_g steps and T_g + 1 frames, numbered GIF by GIF: frame k < T_g is the closed set before step k and the cell

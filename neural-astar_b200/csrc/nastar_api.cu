@@ -11,6 +11,7 @@
 
 #include "../../include/nastar_b200.h"
 #include "nastar_bin16.cuh"
+#include "nastar_chamfer.cuh"
 #include "nastar_convhead.cuh"
 #include "nastar_crops.cuh"
 #include "nastar_deflate.cuh"
@@ -18,6 +19,7 @@
 #include "nastar_gif.cuh"
 #include "nastar_glue.cuh"
 #include "nastar_goals.cuh"
+#include "nastar_inflate.cuh"
 #include "nastar_labels.cuh"
 #include "nastar_maps.cuh"
 #include "nastar_png.cuh"
@@ -385,6 +387,35 @@ int png_enc_check(const nastar_png_enc_desc* desc, int32_t B, int64_t filt_bytes
         *bound += nastar::png_gap(i) + nastar::deflate_member_bound(0, n);
     }
     return st;
+}
+
+// ---- .npz members (nastar_inflate.cuh) --------------------------------------------------------------------------
+// NASTAR_OK or NASTAR_EINVAL for these descriptors: a known method, ranges inside data / out, output ranges in
+// increasing, disjoint order, and stored members of equal lengths
+int inflate_check(const nastar_inflate_desc* desc, int32_t M, int64_t data_bytes, int64_t out_bytes) {
+    if (!desc || M <= 0) return NASTAR_EINVAL;
+    auto inside = [](int64_t off, int64_t len, int64_t total) { return off >= 0 && len >= 0 && len <= total - off; };
+    int64_t end = 0;
+    for (int32_t i = 0; i < M; ++i) {
+        const nastar_inflate_desc& d = desc[i];
+        if ((d.method != 0 && d.method != 8) || (d.method == 0 && d.in_len != d.out_len)) return NASTAR_EINVAL;
+        if (!inside(d.in_off, d.in_len, data_bytes) || !inside(d.out_off, d.out_len, out_bytes) || d.out_off < end)
+            return NASTAR_EINVAL;
+        end = d.out_off + d.out_len;
+    }
+    return NASTAR_OK;
+}
+
+// ---- Chamfer distances (nastar_chamfer.cuh) ---------------------------------------------------------------------
+constexpr size_t kChamferWorkspaceBudget = size_t(256) << 20;   // global slots: at most this much, but one always
+
+bool chamfer_global(int32_t H, int32_t W) { return nastar::chamfer_layout(H, W).bytes > nastar::kChamferSmemMax; }
+size_t chamfer_slot_bytes(int32_t H, int32_t W) { return round256(size_t(nastar::chamfer_layout(H, W).bytes)); }
+int chamfer_grid(int32_t B, int32_t H, int32_t W) {
+    if (!chamfer_global(H, W)) return B;
+    const int64_t fit = int64_t(kChamferWorkspaceBudget / chamfer_slot_bytes(H, W));
+    const int g = capped_grid(B, 1);
+    return int(g < fit ? g : fit > 0 ? fit : 1);
 }
 
 // ---- search GIFs (nastar_gif.cuh) ------------------------------------------------------------------------------
@@ -1143,6 +1174,43 @@ int nastar_b200_crop_resize_rgb(const nastar_rgb_image* src, const nastar_rgb_im
     if (smem > kMaxDynSmem) return NASTAR_EUNSUPPORTED;
     const nastar::CropArgs a{src_dev, crops_dev, Ho, Wo, int64_t(smem), out};
     const cudaError_t e = launch_smem(nastar::crop_resize_rgb_kernel, N, nastar::kCropThreads, smem,
+                                      static_cast<cudaStream_t>(stream_v), a);
+    if (e != cudaSuccess) return cuda_fail(e);
+    return launched();
+}
+
+int nastar_b200_inflate(const uint8_t* data, int64_t data_bytes, const nastar_inflate_desc* desc,
+                        const nastar_inflate_desc* desc_dev, int32_t M, uint8_t* out, int64_t out_bytes,
+                        int32_t* status, uint32_t* crc, void* workspace, size_t workspace_bytes, void* stream_v) {
+    if (!data || !desc_dev || !out || !status || !crc) return NASTAR_EINVAL;
+    const int st = inflate_check(desc, M, data_bytes, out_bytes);
+    if (st != NASTAR_OK) return st;
+    if (!workspace || workspace_bytes < NASTAR_INFLATE_WORKSPACE_BYTES) return NASTAR_EWORKSPACE;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+    int32_t* queue = static_cast<int32_t*>(workspace);
+    const cudaError_t e = cudaMemsetAsync(queue, 0, sizeof(int32_t), stream);
+    if (e != cudaSuccess) return cuda_fail(e);
+    const nastar::InflateArgs a{data, desc_dev, M, out, status, crc, queue};
+    nastar::inflate_kernel<<<capped_grid(M, 16), nastar::kInflateThreads, 0, stream>>>(a);
+    return launched();
+}
+
+size_t nastar_b200_chamfer_workspace_bytes(int32_t B, int32_t H, int32_t W) {
+    if (B <= 0 || H <= 0 || W <= 0 || H > nastar::kChamferMaxSide || W > nastar::kChamferMaxSide) return 0;
+    return chamfer_global(H, W) ? size_t(chamfer_grid(B, H, W)) * chamfer_slot_bytes(H, W) : 0;
+}
+
+int nastar_b200_chamfer(const uint8_t* masks, int32_t B, int32_t H, int32_t W, double* out, void* workspace,
+                        size_t workspace_bytes, void* stream_v) {
+    if (!masks || !out || B <= 0 || H <= 0 || W <= 0) return NASTAR_EINVAL;
+    if (H > nastar::kChamferMaxSide || W > nastar::kChamferMaxSide) return NASTAR_EUNSUPPORTED;
+    const size_t need = nastar_b200_chamfer_workspace_bytes(B, H, W);
+    if (need && (!workspace || workspace_bytes < need)) return NASTAR_EWORKSPACE;
+    const bool global = chamfer_global(H, W);
+    const nastar::ChamferArgs a{masks, B, H, W, out, global ? static_cast<unsigned char*>(workspace) : nullptr,
+                                int64_t(chamfer_slot_bytes(H, W))};
+    const size_t smem = global ? 0 : size_t(nastar::chamfer_layout(H, W).bytes);
+    const cudaError_t e = launch_smem(nastar::chamfer_kernel, chamfer_grid(B, H, W), nastar::kChamferThreads, smem,
                                       static_cast<cudaStream_t>(stream_v), a);
     if (e != cudaSuccess) return cuda_fail(e);
     return launched();

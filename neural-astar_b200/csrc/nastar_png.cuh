@@ -231,13 +231,13 @@ __device__ __forceinline__ uint32_t png_level(const uint8_t* row, int x, int dep
     }
 }
 
-// inflate the zlib stream of `d` into raw[0, raw_len); returns the status bits
-__device__ int png_inflate(PngSmem& s, const uint8_t* src, int64_t src_len, uint8_t* raw, int64_t raw_len) {
+// the raw deflate blocks (stored, fixed and dynamic Huffman) that `br` reads from src[0, src_len), inflated into
+// raw[0, raw_len), which they must fill exactly; returns the status bits.  Matches read back from `raw`, so no other
+// buffer is needed.  Shared by the PNG decode (png_inflate adds the zlib framing) and the .npz reader
+// (nastar_inflate.cuh).  Warp-collective.
+__device__ int png_inflate_blocks(PngSmem& s, PngBits& br, const uint8_t* src, int64_t src_len, uint8_t* raw,
+                                  int64_t raw_len) {
     const int lane = threadIdx.x & 31;
-    PngBits br{src, src_len, 0, 0, 0};
-    const uint32_t cmf = br.get(8), flg = br.get(8);
-    if (br.overrun() || (cmf & 15) != 8 || (cmf >> 4) > 7 || ((cmf << 8) | flg) % 31 != 0 || (flg & 32))
-        return kPngBadHeader;
     int64_t op = 0;
     bool last = false;
     while (!last) {
@@ -343,7 +343,18 @@ __device__ int png_inflate(PngSmem& s, const uint8_t* src, int64_t src_len, uint
             op += len;
         }
     }
-    if (op != raw_len) return kPngBadLength;
+    return op != raw_len ? kPngBadLength : 0;
+}
+
+// inflate the zlib stream of `d` into raw[0, raw_len); returns the status bits
+__device__ int png_inflate(PngSmem& s, const uint8_t* src, int64_t src_len, uint8_t* raw, int64_t raw_len) {
+    const int lane = threadIdx.x & 31;
+    PngBits br{src, src_len, 0, 0, 0};
+    const uint32_t cmf = br.get(8), flg = br.get(8);
+    if (br.overrun() || (cmf & 15) != 8 || (cmf >> 4) > 7 || ((cmf << 8) | flg) % 31 != 0 || (flg & 32))
+        return kPngBadHeader;
+    const int st = png_inflate_blocks(s, br, src, src_len, raw, raw_len);
+    if (st) return st;
     br.align();
     const uint32_t b0 = br.get(8), b1 = br.get(8), b2 = br.get(8), b3 = br.get(8);
     if (br.overrun()) return kPngBadLength;

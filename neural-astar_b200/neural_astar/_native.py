@@ -117,6 +117,9 @@ _SIGNATURES = {
     "nastar_b200_png_gap": (_i64, [_i32]),
     "nastar_b200_png_encode_bound": (_i64, [_p, _i32]),
     "nastar_b200_crop_resize_rgb": (_int, [_p, _p, _i32, _p, _p] + [_i32] * 3 + [_p, _p]),
+    "nastar_b200_inflate": (_int, [_p, _i64, _p, _p, _i32, _p, _i64, _p, _p, _p, ctypes.c_size_t, _p]),
+    "nastar_b200_chamfer": (_int, [_p] + [_i32] * 3 + [_p, _p, ctypes.c_size_t, _p]),
+    "nastar_b200_chamfer_workspace_bytes": (ctypes.c_size_t, [_i32] * 3),
     "nastar_b200_gif_tables_bytes": (_i64, [ctypes.POINTER(GifParams)]),
     "nastar_b200_gif_plan": (_int, [ctypes.POINTER(GifParams), _p, _p, _p, ctypes.c_size_t, _p]),
     "nastar_b200_gif_record_bytes": (_i64, [_i64]),
@@ -1102,4 +1105,57 @@ def gif_encode(p: GifParams, nbytes: torch.Tensor, nbytes_host: np.ndarray, offs
         _check(L.nastar_b200_gif_encode(ctypes.byref(p), nbytes.data_ptr(), nb.ctypes.data, off.ctypes.data,
                                         offset_dev.data_ptr(), len(nb), out.data_ptr(), int(off[-1]), ws.data_ptr(),
                                         ws.numel(), stream), "nastar_b200_gif_encode")
+    return out
+
+
+# struct nastar_inflate_desc (include/nastar_b200.h) as a NumPy record
+INFLATE_DESC_DTYPE = np.dtype([("in_off", "<i8"), ("in_len", "<i8"), ("out_off", "<i8"), ("out_len", "<i8"),
+                               ("method", "<i4"), ("reserved", "<i4")])
+INFLATE_WORKSPACE_BYTES = 256
+# status bits of nastar_b200_inflate
+INFLATE_STATUS = {2: "bad block type or Huffman code", 4: "distance past the start of the output",
+                  8: "stream ends early or inflates to the wrong size"}
+
+
+def inflate(data: torch.Tensor, desc, desc_dev: torch.Tensor, out: torch.Tensor):
+    """Zip members to their bytes in one kernel (include/nastar_b200.h, nastar_b200_inflate): member i of `desc` (a
+    NumPy array of INFLATE_DESC_DTYPE, the host copy checked before the launch) from `data` into `out` (1-D uint8 CUDA
+    tensors); desc_dev: the same descriptors' bytes in device memory.  Returns (status int32 [M], crc int32 [M] (the
+    CRC-32's bits)) on the current stream; nothing is read back."""
+    L = lib()
+    d = np.ascontiguousarray(desc, dtype=INFLATE_DESC_DTYPE)
+    if any(not t.is_cuda or t.dtype != torch.uint8 or t.ndim != 1 for t in (data, out, desc_dev)):
+        raise RuntimeError("inflate: data, out and desc_dev must be 1-D uint8 CUDA tensors (there is no CPU fallback)")
+    if not desc_dev.is_contiguous() or desc_dev.numel() != d.nbytes or desc_dev.device != data.device:
+        raise ValueError(f"inflate: desc_dev must be {d.nbytes} contiguous uint8 bytes on the data's device")
+    dev = data.device
+    with _on_device(dev) as stream:
+        status = torch.empty((len(d),), dtype=torch.int32, device=dev)
+        crc = torch.empty((len(d),), dtype=torch.int32, device=dev)
+        ws = torch.empty((INFLATE_WORKSPACE_BYTES,), dtype=torch.uint8, device=dev)
+        _check(L.nastar_b200_inflate(data.data_ptr(), data.numel(), d.ctypes.data, desc_dev.data_ptr(), len(d),
+                                     out.data_ptr(), out.numel(), status.data_ptr(), crc.data_ptr(), ws.data_ptr(),
+                                     INFLATE_WORKSPACE_BYTES, stream), "nastar_b200_inflate")
+    return status, crc
+
+
+CHAMFER_MAX_SIDE = 1024
+
+
+def chamfer(masks: torch.Tensor) -> torch.Tensor:
+    """Directed Chamfer distances in one kernel (include/nastar_b200.h, nastar_b200_chamfer): masks is a uint8 CUDA
+    tensor [B,H,W] with bit 0 = set A and bit 1 = set B.  Returns fp64 [B,2] (d(A -> B), d(B -> A)) on the current
+    stream."""
+    L = lib()
+    if not masks.is_cuda or masks.dtype != torch.uint8 or masks.ndim != 3:
+        raise RuntimeError("chamfer: masks must be a uint8 CUDA tensor [B,H,W] (there is no CPU fallback)")
+    masks = masks.contiguous()
+    B, H, W = masks.shape
+    dev = masks.device
+    ws_bytes = int(L.nastar_b200_chamfer_workspace_bytes(B, H, W))
+    with _on_device(dev) as stream:
+        out = torch.empty((B, 2), dtype=torch.float64, device=dev)
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None
+        _check(L.nastar_b200_chamfer(masks.data_ptr(), B, H, W, out.data_ptr(), ws.data_ptr() if ws is not None else None,
+                                     ws_bytes, stream), "nastar_b200_chamfer")
     return out

@@ -1443,11 +1443,269 @@ def save_sdd_samples(video_dirs, save_dir: str, W: int = 64, min_len_ratio: floa
     return total + n
 
 
-__all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "MazeDataset", "WarCraftDataset",
-           "compute_opt_labels", "compute_weighted_opt_labels", "create_dataloader", "create_device_dataloader",
-           "create_warcraft_dataloader", "draw_opt_policies", "encode_pngs", "load_map_images", "maps_from_images",
+# the .npy dtypes load_npz_device reads: NumPy's descr -> the torch dtype of the same bytes
+_NPY_TORCH_DTYPE = {"|b1": torch.bool, "|u1": torch.uint8, "|i1": torch.int8, "<i2": torch.int16, "<i4": torch.int32,
+                    "<i8": torch.int64, "<f2": torch.float16, "<f4": torch.float32, "<f8": torch.float64}
+_NPY_MAGIC = b"\x93NUMPY"
+
+
+class NpzMember(tuple):
+    """One member of a .npz file as load_npz_device reads it: (key, method, data_off, csize, usize, crc, descr, shape,
+    header_len).  data_off / csize: the stored or deflated bytes in the file; usize: the inflated .npy size;
+    header_len: the bytes of its .npy header, after which the array's C-order bytes follow."""
+
+
+def _npz_plan(blob, name: str = "<bytes>") -> list:
+    """The members of a .npz file held in memory, parsed on the host as zipfile and np.lib.format read them: the end
+    record (ZIP64 where present), the central directory (sizes and CRC from there, with ZIP64 extras, so members
+    written with data descriptors work) and each local header's length.  Each member's .npy header (format 1, 2 or 3)
+    comes from its first bytes alone, inflated with zlib.decompressobj(-15) when it is deflated.  Returns a list of
+    NpzMember in central-directory order.  Anything load_npz_device does not read raises ValueError naming the file and
+    the member: methods other than stored (0) and deflated (8), encryption, members that are not .npy files, dtypes
+    other than |b1 |u1 |i1 <i2 <i4 <i8 <f2 <f4 <f8 (object, structured and big-endian ones among them), Fortran order,
+    and sizes that do not add up."""
+    import ast
+    import struct
+    import zlib
+
+    blob = memoryview(blob).cast("B")
+    n = len(blob)
+
+    def bad(why, member=None):
+        return ValueError(f"{name}: {why}" if member is None else f"{name}: member {member!r}: {why}")
+
+    tail = bytes(blob[max(0, n - 22 - 0xFFFF):])
+    e = tail.rfind(b"PK\x05\x06")
+    if e < 0 or len(tail) - e < 22:
+        raise bad("not a zip file (no end of central directory record)")
+    eocd = n - len(tail) + e
+    _, _, _, _, count, cd_size, cd_off, _ = struct.unpack("<IHHHHIIH", blob[eocd:eocd + 22])
+    if eocd >= 20 and bytes(blob[eocd - 20:eocd - 16]) == b"PK\x06\x07":
+        z64 = struct.unpack("<Q", blob[eocd - 12:eocd - 4])[0]
+        if z64 + 56 > n or bytes(blob[z64:z64 + 4]) != b"PK\x06\x06":
+            raise bad("corrupt ZIP64 end of central directory record")
+        count, _, cd_size, cd_off = struct.unpack("<QQQQ", blob[z64 + 24:z64 + 56])
+    if cd_off + cd_size > n:
+        raise bad("central directory outside the file")
+    members, pos = [], cd_off
+    for _ in range(count):
+        if pos + 46 > n or bytes(blob[pos:pos + 4]) != b"PK\x01\x02":
+            raise bad("corrupt central directory")
+        (_, _, _, flags, method, _, _, crc, csize, usize, nlen, elen, clen, _, _, _,
+         lh) = struct.unpack("<IHHHHHHIIIHHHHHII", blob[pos:pos + 46])
+        member = bytes(blob[pos + 46:pos + 46 + nlen]).decode("utf-8" if flags & 0x800 else "cp437")
+        extra = bytes(blob[pos + 46 + nlen:pos + 46 + nlen + elen])
+        pos += 46 + nlen + elen + clen
+        x = 0
+        while x + 4 <= len(extra):   # ZIP64 extra: the 64-bit values of the fields that hold 0xFFFFFFFF, in order
+            tag, size = struct.unpack("<HH", extra[x:x + 4])
+            if tag == 1:
+                vals = list(struct.unpack(f"<{size // 8}Q", extra[x + 4:x + 4 + size // 8 * 8]))
+                if usize == _U32 and vals:
+                    usize = vals.pop(0)
+                if csize == _U32 and vals:
+                    csize = vals.pop(0)
+                if lh == _U32 and vals:
+                    lh = vals.pop(0)
+            x += 4 + size
+        if flags & 1:
+            raise bad("encrypted members are not supported", member)
+        if method not in (0, 8):
+            raise bad(f"compression method {method} is not supported (only stored and deflated)", member)
+        if not member.endswith(".npy"):
+            raise bad("not a .npy member", member)
+        if lh + 30 > n or bytes(blob[lh:lh + 4]) != b"PK\x03\x04":
+            raise bad("corrupt local header", member)
+        lnlen, lelen = struct.unpack("<HH", blob[lh + 26:lh + 30])
+        data_off = lh + 30 + lnlen + lelen
+        if data_off + csize > n or (method == 0 and csize != usize):
+            raise bad("member data outside the file or of the wrong size", member)
+        comp = blob[data_off:data_off + csize]
+
+        def first(k):   # the member's first k inflated bytes (fewer at its end)
+            if method == 0:
+                return bytes(comp[:k])
+            try:
+                return zlib.decompressobj(-15).decompress(comp, k)
+            except zlib.error as err:
+                raise bad(f"corrupt deflate stream ({err})", member) from None
+
+        head = first(12)
+        if len(head) < 10 or head[:6] != _NPY_MAGIC or head[6] not in (1, 2, 3):
+            raise bad("not a .npy file of format 1, 2 or 3", member)
+        start = 10 if head[6] == 1 else 12
+        hl = struct.unpack("<H" if head[6] == 1 else "<I", head[8:start])[0]
+        text = first(start + hl)[start:]
+        if len(text) != hl:
+            raise bad("truncated .npy header", member)
+        try:
+            d = ast.literal_eval(text.decode("utf-8" if head[6] == 3 else "latin-1"))
+        except (ValueError, SyntaxError, UnicodeDecodeError):
+            raise bad("unreadable .npy header", member) from None
+        if not isinstance(d, dict) or set(d) != {"descr", "fortran_order", "shape"}:
+            raise bad("unreadable .npy header", member)
+        descr, shape = d["descr"], d["shape"]
+        try:
+            dt = np.dtype(descr).str if isinstance(descr, str) else None
+        except TypeError:
+            dt = None
+        if dt not in _NPY_TORCH_DTYPE:
+            raise bad(f"dtype {descr!r} is not supported (only {' '.join(_NPY_TORCH_DTYPE)})", member)
+        if d["fortran_order"]:
+            raise bad("Fortran-order arrays are not supported", member)
+        if not isinstance(shape, tuple) or not all(isinstance(v, int) and v >= 0 for v in shape):
+            raise bad(f"bad shape {shape!r}", member)
+        descr = dt
+        if start + hl + int(np.prod(shape, dtype=np.int64)) * np.dtype(descr).itemsize != usize:
+            raise bad("the .npy header does not match the member's size", member)
+        members.append(NpzMember((member[:-4], method, data_off, csize, usize, crc, descr, tuple(shape), start + hl)))
+    return members
+
+
+def load_npz_device(files, device=None) -> list:
+    """np.load for many .npz files at once, with the members inflated on the GPU (include/nastar_b200.h,
+    nastar_b200_inflate; DESIGN.md §23).  files: paths or `bytes`.  Returns one dict per file of what np.load(f) gives,
+    {member name without ".npy": CUDA tensor} with the same dtypes, shapes and values.
+
+    The host parses the zip records and each member's .npy header (_npz_plan: anything it does not read raises
+    ValueError naming the file and member before any launch), copies every member's stored or deflated bytes to
+    `device` (the current CUDA device when None) in one transfer and allocates one output buffer, each array's bytes
+    starting 64-byte aligned, so every array is a typed view of it.  One launch inflates every member of every file;
+    one synchronisation then reads the statuses and CRC-32s: a corrupt stream or a CRC-32 that differs from the zip's
+    raises ValueError naming the file and member, whose `arrays` attribute holds the result, exact for every member it
+    does not name.  One warp inflates one member, so this suits many small members
+    (such as the SDD samples), not a few huge ones."""
+    names, blobs = [], []
+    for f in files:
+        if isinstance(f, (bytes, bytearray, memoryview)):
+            names.append(f"<npz {len(names)}>")
+            blobs.append(f)
+        else:
+            names.append(os.fspath(f))
+            with open(f, "rb") as fh:
+                blobs.append(fh.read())
+    plans = [_npz_plan(b, n) for b, n in zip(blobs, names)]
+    if not blobs:
+        return []
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.type != "cuda":
+        raise RuntimeError("load_npz_device runs on a CUDA device (there is no CPU fallback)")
+    M = sum(len(p) for p in plans)
+    desc = np.zeros(M, _native.INFLATE_DESC_DTYPE)
+    head = (desc.nbytes + 63) // 64 * 64
+    total = head + sum(m[3] for p in plans for m in p)
+    buf = torch.empty((max(total, 1),), dtype=torch.uint8).pin_memory()
+    host = buf.numpy()
+    pos, out_pos, i = head, 0, 0
+    for blob, plan in zip(blobs, plans):
+        b = np.frombuffer(blob, np.uint8)
+        for key, method, off, csize, usize, _, _, _, hl in plan:
+            out_pos = (out_pos + hl + 63) // 64 * 64 - hl   # the array's bytes start 64-byte aligned
+            host[pos:pos + csize] = b[off:off + csize]
+            desc[i] = (pos, csize, out_pos, usize, method, 0)
+            pos += csize
+            out_pos += usize
+            i += 1
+    host[:desc.nbytes] = desc.view(np.uint8)
+    with torch.cuda.device(dev):
+        data = buf.to(dev, non_blocking=True)
+        out = torch.empty((max(out_pos, 1),), dtype=torch.uint8, device=dev)
+        if M:
+            status, crc = _native.inflate(data, desc, data[:desc.nbytes], out)
+            meta = torch.cat([status.to(torch.int64), crc.to(torch.int64) & _U32]).cpu().numpy().reshape(2, M)
+        else:
+            meta = np.zeros((2, 0), np.int64)
+    result, i, errors = [], 0, []
+    for name, plan in zip(names, plans):
+        arrays = {}
+        for key, _, _, _, usize, crc, descr, shape, hl in plan:
+            st, got = int(meta[0, i]), int(meta[1, i])
+            if st:
+                why = ", ".join(w for bit, w in _native.INFLATE_STATUS.items() if st & bit)
+                errors.append(f"{name}: member {key + '.npy'!r}: corrupt deflate stream ({why})")
+            elif got != crc:
+                errors.append(f"{name}: Bad CRC-32 for file {key + '.npy'!r}")
+            a = int(desc[i]["out_off"]) + hl
+            arrays[key] = out[a:a + usize - hl].view(_NPY_TORCH_DTYPE[descr]).view(shape)
+            i += 1
+        result.append(arrays)
+    if errors:
+        err = ValueError("; ".join(errors[:20]))
+        err.arrays = result   # what the call read: exact for every member the message does not name
+        raise err
+    return result
+
+
+class DeviceSDDDataset:
+    def __init__(self, root: str, scenes=None, device=None):
+        """The Stanford Drone planning samples that save_sdd_samples / tools/make_sdd_dataset.py write, read back onto
+        the GPU for training Neural A* on raw RGB images (DESIGN.md §23): every `<root>/<scene>/<video>/*.npz`, in
+        sorted (scene, video, file) order, of the given `scenes` only when given, read by one load_npz_device call.
+
+        Keeps map_designs fp32 [N,3,W,W] = (image.transpose(2, 0, 1) / 255.0).astype(np.float32) (WarCraftDataset's
+        rule), start_maps / goal_maps / traj_images fp32 [N,1,W,W] (start_image, goal_image, traj_image), label int64
+        [N], length_ratio fp64 [N], the ragged trajectories as traj fp64 [T,2] with traj_offsets int64 [N+1] (sample i
+        is traj[traj_offsets[i]:traj_offsets[i+1]]), all on the device, and per sample the host lists scene and name
+        ("<video>/<file>").  A scene that is not in the tree, or a selection without samples, raises ValueError."""
+        import glob
+
+        root = os.fspath(root)
+        present = sorted(d for d in os.listdir(root) if os.path.isdir(os.path.join(root, d)))
+        scenes = present if scenes is None else sorted(set(scenes))
+        unknown = [s for s in scenes if s not in present]
+        if unknown:
+            raise ValueError(f"{root}: no scene {unknown} (scenes: {present})")
+        files = []
+        for s in scenes:   # within a scene, the paths sort as (video, file): "/" sorts before any name character
+            files += sorted(glob.glob(os.path.join(glob.escape(root), glob.escape(s), "*", "*.npz")))
+        if not files:
+            raise ValueError(f"{root}: no samples in scenes {scenes}")
+        arrays = load_npz_device(files, device)
+        self.scene = [os.path.basename(os.path.dirname(os.path.dirname(f))) for f in files]
+        self.name = [os.path.relpath(f, os.path.dirname(os.path.dirname(f))) for f in files]
+        images = torch.stack([a["image"] for a in arrays])
+        self.device = images.device
+        self.map_designs = (images.permute(0, 3, 1, 2).double() / 255.0).float().contiguous()
+        self.start_maps, self.goal_maps, self.traj_images = (
+            torch.stack([a[k] for a in arrays])[:, None].float() for k in ("start_image", "goal_image", "traj_image"))
+        self.label = torch.stack([a["label"] for a in arrays])
+        self.length_ratio = torch.stack([a["length_ratio"] for a in arrays])
+        self.traj = torch.cat([a["traj"] for a in arrays])
+        self.traj_offsets = torch.tensor(np.concatenate([[0], np.cumsum([a["traj"].shape[0] for a in arrays])]),
+                                         dtype=torch.int64, device=self.device)
+
+    def __len__(self):
+        return self.map_designs.shape[0]
+
+    def sample(self, indices, generator: torch.Generator = None):
+        """(map_designs [B,3,W,W], start_maps, goal_maps, traj_images [B,1,W,W]) of the samples `indices` (host or
+        device), the batch PlannerModule and GraphedTrainStep take (traj_images is the target, as opt_trajs is for
+        mazes).  The samples are fixed: `generator` is accepted for DeviceDataLoader and not used."""
+        idx = torch.as_tensor(indices)
+        if idx.device.type == "cpu":
+            if idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= len(self)):
+                raise IndexError(f"indices must lie in [0, {len(self)})")
+        idx = idx.to(self.device).reshape(-1).to(torch.int64)
+        return self.map_designs[idx], self.start_maps[idx], self.goal_maps[idx], self.traj_images[idx]
+
+
+def sdd_leave_one_scene_out(root: str, test_scene: str, device=None):
+    """(train, test) DeviceSDDDatasets of the SDD sample tree at `root`: test holds the samples of `test_scene`, train
+    those of every other scene.  An unknown scene raises ValueError."""
+    root = os.fspath(root)
+    scenes = sorted(d for d in os.listdir(root) if os.path.isdir(os.path.join(root, d)))
+    if test_scene not in scenes:
+        raise ValueError(f"{root}: no scene {test_scene!r} (scenes: {scenes})")
+    return (DeviceSDDDataset(root, [s for s in scenes if s != test_scene], device),
+            DeviceSDDDataset(root, [test_scene], device))
+
+
+__all__ = ["AstarOutput", "DeviceDataLoader", "DeviceMazeDataset", "DeviceSDDDataset", "MazeDataset",
+           "WarCraftDataset", "compute_opt_labels", "compute_weighted_opt_labels", "create_dataloader",
+           "create_device_dataloader", "create_warcraft_dataloader", "draw_opt_policies", "encode_pngs",
+           "load_map_images", "load_npz_device", "maps_from_images",
            "read_sdd_annotations", "sample_device_goal_maps", "sample_goal_maps", "save_planning_dataset",
            "save_pngs", "save_sdd_samples", "save_search_gifs",
            "savez_compressed_device", "save_warcraft_dataset", "search_gifs",
-           "sdd_crops", "sdd_sample_plan", "shortest_path_maps", "street_crop_boxes", "tile_maps",
-           "visualize_results"]
+           "sdd_crops", "sdd_leave_one_scene_out", "sdd_sample_plan", "shortest_path_maps", "street_crop_boxes",
+           "tile_maps", "visualize_results"]

@@ -15,6 +15,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
+from .. import _native
 from ..planner.astar import VanillaAstar
 
 try:  # pragma: no cover - optional dependency
@@ -88,6 +89,36 @@ def path_cost_metrics(paths: torch.Tensor, cost_maps: torch.Tensor, opt_path_cos
     ratio = (cost / opt).mean()
     vals = torch.stack((p_opt, ratio)).tolist()
     return vals[0], vals[1]
+
+
+def chamfer_distances(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """Directed Chamfer distances between the cell sets of two masks, on the GPU (include/nastar_b200.h,
+    nastar_b200_chamfer; DESIGN.md §23).  a, b: CUDA tensors of one shape, [B,1,H,W] or [B,H,W], of any real,
+    integer or bool dtype; a cell belongs to a set iff its value != 0.  Returns fp64 [B,2]: the mean, over A's cells, of
+    the Euclidean distance in cells to the nearest cell of B, and the same from B to A.  A map where either set is
+    empty gets NaN in both columns.  Exact squared distances, correctly rounded square roots and a fixed summation
+    order make the result the same from run to run.  H, W <= 1024.  A metric: no autograd."""
+    if a.shape != b.shape:
+        raise ValueError(f"chamfer_distances: masks of one shape expected (got {tuple(a.shape)} and {tuple(b.shape)})")
+    if a.ndim == 4 and a.shape[1] == 1:
+        a, b = a[:, 0], b[:, 0]
+    if a.ndim != 3:
+        raise ValueError(f"chamfer_distances: masks are [B,1,H,W] or [B,H,W] (got {tuple(a.shape)})")
+    if not (a.is_cuda and b.is_cuda) or a.device != b.device:
+        raise RuntimeError("chamfer_distances runs on CUDA tensors of one device (there is no CPU fallback)")
+    if a.shape[1] > _native.CHAMFER_MAX_SIDE or a.shape[2] > _native.CHAMFER_MAX_SIDE:
+        raise ValueError(f"chamfer_distances: H, W <= {_native.CHAMFER_MAX_SIDE} (got {tuple(a.shape[1:])})")
+    if a.shape[0] == 0 or a.shape[1] == 0 or a.shape[2] == 0:
+        return torch.full((a.shape[0], 2), float("nan"), dtype=torch.float64, device=a.device)
+    a, b = a.detach(), b.detach()
+    masks = (a != 0).to(torch.uint8) | ((b != 0).to(torch.uint8) << 1)
+    return _native.chamfer(masks)
+
+
+def chamfer_distance(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """The Chamfer distance d(A -> B) + d(B -> A) per map, fp64 [B] (chamfer_distances summed): how far a planned
+    path lies from a trajectory, the metric of Neural A*'s raw-image (Stanford Drone) experiment."""
+    return chamfer_distances(a, b).sum(1)
 
 
 class GraphedTrainStep:
