@@ -9,10 +9,11 @@
 //
 // GEMM view: M = pixels, N = 256 output channels, K = 9 taps x 128 input channels, both operands K-major (the input
 // is channels-last, the folded weights are OIHW in channels-last memory = [cout][ky][kx][cin]), which is what TF32
-// wgmma requires.  Operands are TF32 (the tensor cores read the top 19 bits of each fp32), products are accumulated
-// in fp32: the precision class of cuDNN's TF32 path it replaces.  The epilogue (bias, ReLU, the 9 head products and
-// the cross-lane sums) is plain fp32 FFMA in a fixed order, so the same inputs give the same bits; there are no
-// atomics.
+// wgmma requires.  Operands are TF32: the tensor cores read the top 19 bits of each fp32 operand, i.e. truncate the
+// mantissa to 10 bits (observed on an H100 SXM for both operands, tests/test_gpu_encoder_exact.py); products are
+// accumulated in fp32: the precision class of cuDNN's TF32 path it replaces.  The epilogue (bias, ReLU, the 9 head
+// products and the cross-lane sums) is plain fp32 FFMA in a fixed order, so the same inputs give the same bits
+// wherever a map lands in the batch and whatever tile width it gets; there are no atomics.
 //
 // Tiles: a CTA computes 128 pixels x 256 channels = R image rows of Wp pixels, Wp = W rounded up to 8/16/32/64 and
 // R = 128 / Wp (4 rows at W = 32).  Columns x >= W and rows y >= H are computed on zeros and not stored.

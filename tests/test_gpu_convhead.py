@@ -1,19 +1,22 @@
 """The fused last-conv + head kernel (csrc/nastar_convhead.cuh): TF32 128 -> 256 3x3 convolution, bias, ReLU and the
-head's 9 per-pixel products in one launch.  Checked against fp64 with an error bound derived from the TF32 unit
-roundoff, against the cuDNN TF32 conv + head_taps path it replaces, for determinism, and for staying out of the fp32
-path."""
+head's 9 per-pixel products in one launch.  Checked against fp64 taps of its TF32 operands within a bound on fp32
+accumulation alone, against the cuDNN TF32 conv + head_taps path it replaces, for determinism, and for staying out of
+the fp32 path.  tests/test_gpu_encoder_exact.py checks it bit for bit."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
+import encoder_exact_oracle as eo
 from golden_util import Golden
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-# TF32 keeps 10 explicit mantissa bits: reading an fp32 operand as TF32 (truncation or rounding) changes it by less
-# than 2^-10 relatively, so each product x*w is off by less than 2^-9 |x||w|.
+# TF32 keeps 10 explicit mantissa bits: reading an fp32 operand as TF32 changes it by less than 2^-10 relatively, so
+# each product x*w is off by less than 2^-9 |x||w|.  The fused kernel's tensor cores truncate (observed on an H100 SXM,
+# test_gpu_encoder_exact.py::test_tf32_operand_conversion_mode); cuDNN's conversion is not assumed, so this bound, used
+# for cuDNN and the encoder references, covers rounding as well.
 U_TF32 = 2.0 ** -10
 PROD = 2 * U_TF32 + U_TF32 ** 2
 
@@ -62,18 +65,23 @@ def _fp64_taps_and_bound(x, w, b, hw):
 @pytest.mark.parametrize("B,H,W", [(1, 32, 32), (7, 32, 32), (100, 32, 32), (3, 64, 64), (5, 20, 27), (4, 5, 3),
                                    (100, 64, 64), (1000, 32, 32)])   # production batches: 3200 and 8000 tiles
 def test_fused_taps_within_tf32_bound_of_fp64(native, B, H, W):
+    """Against fp64 taps of the TF32 operands the tensor cores read (eo.tf32_taps_and_bound): the bound covers only
+    the fp32 accumulation, the bias add and the head sum, and is at least 10x tighter than the a-priori bound of
+    _fp64_taps_and_bound, which also has to cover the operand conversion."""
     x, w, b, hw = _problem(B, H, W, seed=B * 1000 + H * 10 + W)
     got = native.conv3x3_head_taps(x, w, b, hw)
     torch.cuda.synchronize()
-    want, bound = _fp64_taps_and_bound(x, w, b, hw)
+    want, bound = eo.tf32_taps_and_bound(x, w, b, hw)
     err = (got.double() - want).abs()
     assert got.shape == (B, H, W, 9)
     assert bool(torch.isfinite(got).all())
     worst = float((err / bound).max())
-    print(f"B={B} {H}x{W}: max error / TF32 bound = {worst:.3f}")
-    assert worst <= 1.0, f"error exceeds the TF32 bound by {worst:.3f}x"
+    tighter = float((bound / _fp64_taps_and_bound(x, w, b, hw)[1]).max())
+    print(f"B={B} {H}x{W}: max error / TF32-emulated bound = {worst:.4f}; bound / a-priori TF32 bound <= {tighter:.4f}")
+    assert worst <= 1.0, f"error exceeds the TF32-emulated bound by {worst:.3f}x"
+    assert tighter <= 0.1
     # the bound is not vacuous: it is a small fraction of the outputs it bounds
-    assert float(bound.median()) < 0.02 * float(want.abs().median())
+    assert float(bound.median()) < 0.002 * float(want.abs().median())
 
 
 def test_fused_taps_leave_the_rest_of_out_untouched(native):

@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 import torch
 
+import encoder_exact_oracle as eo
 from golden_util import Golden
 
 pytestmark = pytest.mark.gpu
@@ -232,28 +233,23 @@ def test_cost_kinds_equal_plane_search(native):
 
 @pytest.mark.parametrize("C,B,H", [(256, 7, 32), (128, 5, 12), (64, 3, 20), (32, 2, 9)])
 def test_head_taps_kernel_matches_fp32_matmul(native, C, B, H):
-    """Encoder head: per-pixel [C] x [C,9] products from the streaming kernel vs a plain PyTorch fp32 matmul of the
-    same operands (different summation order only)."""
+    """Encoder head: per-pixel [C] x [C,9] products from the streaming kernel, bit-equal to the same fp32 operation
+    sequence replayed on the CPU (eo.head_taps_replay: ascending channel, one fmaf per product)."""
     torch.manual_seed(C)
     x = torch.randn(B, C, H, H, device="cuda").contiguous(memory_format=torch.channels_last)
     w = torch.randn(C, 9, device="cuda") / C ** 0.5
-    old = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    try:
-        want = (x.permute(0, 2, 3, 1).reshape(-1, C).double() @ w.double()).view(B, H, H, 9)
-    finally:
-        torch.backends.cuda.matmul.allow_tf32 = old
+    want = eo.head_taps_replay(x.permute(0, 2, 3, 1).reshape(-1, C).cpu().numpy(), w.cpu().numpy())
     got = native.head_taps(x, w.cpu().numpy())
     assert got.shape == (B, H, H, 9)
-    assert float((got.double() - want).abs().max()) < 2e-5
+    assert np.array_equal(got.view(-1, 9).cpu().numpy(), want)
     buf = torch.empty_like(got)
     assert native.head_taps(x, w.cpu().numpy(), out=buf).data_ptr() == buf.data_ptr() and torch.equal(buf, got)
 
 
 @pytest.mark.parametrize("B,H,W", [(7, 32, 32), (3, 20, 27), (2, 64, 64), (1, 5, 3)])
 def test_conv1_marks_matches_torch_conv(native, B, H, W):
-    """First encoder layer fused with the input assembly vs torch: relu(conv2d(cat(map, start + goal), w, b)) in fp32
-    (different summation order only), channels-last result."""
+    """First encoder layer fused with the input assembly: relu(conv2d(cat(map, start + goal), w, b)), channels-last,
+    bit-equal to the kernel's fp32 operation sequence replayed on the CPU (eo.conv1_marks_replay)."""
     torch.manual_seed(B * H + W)
     maps = (torch.rand(B, 1, H, W, device="cuda") > 0.2).float()
     start = torch.zeros(B, 1, H, W, device="cuda")
@@ -263,13 +259,12 @@ def test_conv1_marks_matches_torch_conv(native, B, H, W):
         goal[b, 0, H - 1 - b % H, W - 1] = 1
     w = torch.randn(32, 2, 3, 3, device="cuda") * 0.3
     bias = torch.randn(32, device="cuda") * 0.1
-    want = torch.relu(torch.nn.functional.conv2d(torch.cat((maps, start + goal), 1).double(), w.double(), bias.double(),
-                                                 padding=1))
     wh = np.ascontiguousarray(w.permute(2, 3, 1, 0).reshape(9, 2, 32).cpu().numpy())
     bh = bias.cpu().numpy()
+    want = eo.conv1_marks_replay(maps.cpu().numpy(), start.cpu().numpy(), goal.cpu().numpy(), wh, bh)
     got = native.conv1_marks(maps, start, goal, wh, bh)
     assert got.shape == (B, 32, H, W) and got.is_contiguous(memory_format=torch.channels_last)
-    assert float((got.double() - want).abs().max()) < 1e-5
+    assert np.array_equal(got.permute(0, 2, 3, 1).cpu().numpy(), want)
     # strided one-hot planes (views into a stacked request buffer) are read in place
     stacked = torch.stack((maps, start, goal), 0)
     got2 = native.conv1_marks(stacked[0], stacked[1], stacked[2], wh, bh)
