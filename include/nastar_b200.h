@@ -182,6 +182,29 @@ int nastar_b200_backward_mech(const nastar_bwd_params *p, int32_t mechanism, voi
 size_t nastar_b200_forward_coupled_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t T);
 int nastar_b200_forward_coupled(const nastar_fwd_params *p, int32_t *T_batch, int32_t *goal_clamp, void *stream);
 
+/* Black-box backward of the search (BB-A*: the gradient of Vlastelica et al., ICLR 2020, through a non-differentiable
+ * A*).  With w the cost plane of p, g = grad_histories and lambda > 0:
+ *   w'        = fl(w + fl(lambda * g))   (two roundings, no FMA, no clamp: w' may be negative);
+ *   y'        = the closed set of the same search on w' (p->g_ratio, p->T, mechanism, start / goal / obstacle planes);
+ *   grad_cost = (y' - histories) / lambda, every cell exactly 0 or +-fl(1/lambda).
+ * Inputs: p's input fields (cost .. flags, cost_kind, workspace); its output fields are neither read nor written.
+ * `histories` are the forward's histories y(w), [B][H*W] contiguous; grad_histories [B][H*W] maps grad_stride elements
+ * apart.  Output: grad_cost [B][H*W] contiguous, overwritten.
+ * T_batch and goal_clamp both NULL: the search on w' stops each map at its solve step, like nastar_b200_forward
+ * without flags (exact for g_ratio >= 0.5 or B = 1).  One launch; w' is formed while the costs are staged and y' is
+ * compared with `histories` in the epilogue, so neither w' nor y' is ever stored.  Both non-NULL: the batch-coupled
+ * search of nastar_b200_forward_coupled with cap p->T on w', which also writes its T_batch[0] and goal_clamp[B]
+ * there; the same three launches, with the black-box prologue and epilogue in both search passes.
+ * Checks, all before the first launch: a NULL plane, histories, grad_histories or grad_cost, B, H or W <= 0, T < 1,
+ * lambda not finite or <= 0, cost_kind other than NASTAR_COST_PLANE, flags other than NASTAR_FWD_NEWS, a trace, or
+ * only one of T_batch / goal_clamp give NASTAR_EINVAL; unsupported shapes NASTAR_EUNSUPPORTED.  Workspace: coupled,
+ * nastar_b200_forward_coupled_workspace_bytes(B, H, W, T) bytes; otherwise the generic engine's state slots beyond
+ * 128x128 (nastar_b200_forward_workspace_bytes(B, H, W) covers them), else NASTAR_EWORKSPACE.  Engines 1, 4, 2 and 3;
+ * engine 5 is never used.  Asynchronous on `stream`. */
+int nastar_b200_backward_blackbox(const nastar_fwd_params *p, const float *histories, const float *grad_histories,
+                                  int64_t grad_stride, float lambda, float *grad_cost, int32_t *T_batch,
+                                  int32_t *goal_clamp, void *stream);
+
 /* T_batch[0] = min(T, 1 + max_b n_steps-style stop) computed on the device from the forward's
  * t_solve/n_steps arrays (replaces the host-synchronising torch.all(...) of :251). */
 int nastar_b200_batch_steps(const int32_t *t_solve, const int32_t *n_steps, int32_t B, int32_t T,

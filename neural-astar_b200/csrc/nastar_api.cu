@@ -2,6 +2,7 @@
 // Host side only validates, picks an engine and launches; no torch types, no CPU fallback.
 #include <cuda_runtime.h>
 #include <atomic>
+#include <cmath>
 #include <cstdio>
 
 #include <cstdlib>
@@ -158,11 +159,13 @@ int generic_slots(int B) { return capped_grid(B, kGlobalCtasPerSm); }
 // NASTAR_COST_PLANE, 4-connected for NASTAR_FWD_NEWS; the 32-wide engine runs 2B CTAs under NASTAR_FWD_PAIR.  The
 // generic engine gets one CTA per map, or one per workspace slot when its state or the backward lives in the
 // workspace.  Fills the heuristic table first where the engine reads one; the launch is left for launched().
+// kExit may carry nastar::kExitBlackbox (the black-box backward: no trace, plain cost plane, no pair).
 template <int kExit, bool kBwd>
 cudaError_t launch_search(int engine, const nastar::SearchArgs& a, cudaStream_t stream) {
     constexpr bool kMayTrace = !kBwd && (kExit == nastar::kExitEarly || kExit == nastar::kExitNone);
+    constexpr bool kBlackbox = (kExit & nastar::kExitBlackbox) != 0;
     const auto trace = flag_if<kMayTrace>(a.f.trace != nullptr);
-    const auto fused = flag_if<!kBwd>(a.f.cost_kind != NASTAR_COST_PLANE);
+    const auto fused = flag_if<!kBwd && !kBlackbox>(a.f.cost_kind != NASTAR_COST_PLANE);
     const bool news = (a.f.flags & NASTAR_FWD_NEWS) != 0;
     const int B = a.f.B;
     if (engine == 1 || engine == 4) {
@@ -318,6 +321,32 @@ __global__ void __launch_bounds__(kCoupledThreads) coupled_reduce_kernel(const n
         }
         goal_clamp[b] = (n >= 2) ? 0 : Tb;
     }
+}
+
+// the three launches of a batch-coupled search (nastar_b200_forward_coupled): pass 1 (kExitCoupled1), the reduction,
+// pass 2 (kExitCoupled2), each with the extra mode bits kMore (nastar::kExitBlackbox for the black-box backward).
+// `a` holds the problems; its records and engine-3 slots are carved from p->workspace here.
+template <int kMore>
+int run_coupled(int engine, nastar::SearchArgs a, const nastar_fwd_params* p, int32_t* T_batch, int32_t* goal_clamp,
+                cudaStream_t stream) {
+    a.T_batch = T_batch;
+    a.cw = coupled_ws(p->workspace, p->B, p->T);
+    if (engine == 2 || engine == 3) {
+        const size_t aux = coupled_aux_bytes(p->B, p->T);
+        a.f.workspace = static_cast<unsigned char*>(p->workspace) + aux;   // engine 3's slots follow the records
+        a.f.workspace_bytes = p->workspace_bytes - aux;
+    }
+    // no host round trip between the three launches
+    cudaError_t e = launch_search<nastar::kExitCoupled1 | kMore, false>(engine, a, stream);
+    if (e != cudaSuccess) return cuda_fail(e);
+    int st = launched();
+    if (st != NASTAR_OK) return st;
+    coupled_reduce_kernel<<<1, kCoupledThreads, 0, stream>>>(a.cw, p->B, p->T, T_batch, goal_clamp);
+    st = launched();
+    if (st != NASTAR_OK) return st;
+    e = launch_search<nastar::kExitCoupled2 | kMore, false>(engine, a, stream);
+    if (e != cudaSuccess) return cuda_fail(e);
+    return launched();
 }
 
 // ---- PNG decode (nastar_png.cuh) -----------------------------------------------------------------------------
@@ -641,27 +670,42 @@ int nastar_b200_forward_coupled(const nastar_fwd_params* p, int32_t* T_batch, in
     if (p->cost_kind != NASTAR_COST_PLANE && engine != 1 && engine != 4) return NASTAR_EUNSUPPORTED;
     const size_t need = nastar_b200_forward_coupled_workspace_bytes(p->B, p->H, p->W, p->T);
     if (!p->workspace || p->workspace_bytes < need) return NASTAR_EWORKSPACE;
+    nastar::SearchArgs a{};
+    a.f = *p;
+    return run_coupled<0>(engine, a, p, T_batch, goal_clamp, static_cast<cudaStream_t>(stream_v));
+}
+
+int nastar_b200_backward_blackbox(const nastar_fwd_params* p, const float* histories, const float* grad_histories,
+                                  int64_t grad_stride, float lambda, float* grad_cost, int32_t* T_batch,
+                                  int32_t* goal_clamp, void* stream_v) {
+    if (!p || !p->cost || !p->start || !p->goal || !p->obst || !histories || !grad_histories || !grad_cost)
+        return NASTAR_EINVAL;
+    if (p->B <= 0 || p->H <= 0 || p->W <= 0 || p->T < 1) return NASTAR_EINVAL;
+    if (!std::isfinite(lambda) || !(lambda > 0.f)) return NASTAR_EINVAL;
+    if (p->cost_kind != NASTAR_COST_PLANE || (p->flags & ~NASTAR_FWD_NEWS) != 0 || p->trace) return NASTAR_EINVAL;
+    if ((T_batch == nullptr) != (goal_clamp == nullptr)) return NASTAR_EINVAL;
+    const bool coupled = (T_batch != nullptr);
+    const int engine = nastar_b200_engine_for(p->H, p->W);
+    if (engine == 0) return NASTAR_EUNSUPPORTED;
+    const size_t need = coupled ? nastar_b200_forward_coupled_workspace_bytes(p->B, p->H, p->W, p->T)
+                                : (engine == 3 ? size_t(generic_slots(p->B)) * nastar::GenericLayout(p->H, p->W).slot_bytes()
+                                               : 0);
+    if (need && (!p->workspace || p->workspace_bytes < need)) return NASTAR_EWORKSPACE;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
     nastar::SearchArgs a{};
     a.f = *p;
-    a.T_batch = T_batch;
-    a.cw = coupled_ws(p->workspace, p->B, p->T);
-    if (engine == 2 || engine == 3) {
-        const size_t aux = coupled_aux_bytes(p->B, p->T);
-        a.f.workspace = static_cast<unsigned char*>(p->workspace) + aux;   // engine 3's slots follow the records
-        a.f.workspace_bytes = p->workspace_bytes - aux;
-    }
-    // pass 1 (kExitCoupled1), the reduction, pass 2 (kExitCoupled2): three launches, no host round trip
-    cudaError_t e = launch_search<nastar::kExitCoupled1, false>(engine, a, stream);
-    if (e != cudaSuccess) return cuda_fail(e);
-    int st = launched();
-    if (st != NASTAR_OK) return st;
-    coupled_reduce_kernel<<<1, kCoupledThreads, 0, stream>>>(a.cw, p->B, p->T, T_batch, goal_clamp);
-    st = launched();
-    if (st != NASTAR_OK) return st;
-    e = launch_search<nastar::kExitCoupled2, false>(engine, a, stream);
-    if (e != cudaSuccess) return cuda_fail(e);
-    return launched();
+    // the search's own outputs are never written: its closed set goes straight into dL/dw
+    a.f.histories = nullptr;
+    a.f.paths = nullptr;
+    a.f.t_solve = a.f.n_steps = a.f.n_closed = a.f.path_len = nullptr;
+    a.grad_hist = grad_histories;
+    a.grad_stride = grad_stride;
+    a.grad_cost = grad_cost;
+    a.bb_lambda = lambda;
+    a.bb_hist = histories;
+    if (coupled) return run_coupled<nastar::kExitBlackbox>(engine, a, p, T_batch, goal_clamp, stream);
+    const cudaError_t e = launch_search<nastar::kExitEarly | nastar::kExitBlackbox, false>(engine, a, stream);
+    return e == cudaSuccess ? launched() : cuda_fail(e);
 }
 
 int nastar_b200_backward(const nastar_bwd_params* p, void* stream_v) {

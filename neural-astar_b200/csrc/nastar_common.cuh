@@ -21,6 +21,11 @@ constexpr uint32_t kKeyInf = 0xFFFFFFFFu;  // "no open cell" sentinel, above eve
 //   kExitCoupled2 pass 2: maps that pass 1 stopped after more than *T_batch steps run again for exactly *T_batch
 //                 steps; every other map only finishes its counters.
 constexpr int kExitEarly = 0, kExitNone = 1, kExitCoupled1 = 2, kExitCoupled2 = 3;
+// kExitBlackbox, added to kExitEarly, kExitCoupled1 or kExitCoupled2: the black-box backward
+// (nastar_b200_backward_blackbox).  The prologue searches w' = fl(w + fl(lambda * dL/dhistories)) instead of the cost
+// plane, and the epilogue writes dL/dw = (closed(w') - histories) / lambda instead of histories and paths.  A bit of
+// the exit mode rather than a template parameter of its own, so that the other instantiations keep their names.
+constexpr int kExitBlackbox = 8;
 
 // how pass 1 of the coupled forward ended for a map (CoupledWs::end)
 constexpr int kEndCapped = 0;      // T steps executed

@@ -25,6 +25,9 @@ struct SearchArgs {
     // generic engine's forward only, nullable: per-map flags written by the bin16 engine (nastar_bin16.cuh); when
     // given, only maps with redo[b] != 0 are processed (the others were already finished on-chip)
     const int32_t* redo;
+    // black-box backward only (kExitBlackbox): grad_hist / grad_stride carry dL/dhistories and grad_cost receives dL/dw
+    float bb_lambda;            // lambda > 0
+    const float* bb_hist;       // the forward's histories y(w), [B][H*W]
 };
 
 // ---- heuristic tables -----------------------------------------------------------------------------------------
@@ -45,6 +48,18 @@ __global__ void heur_init_kernel() {
     const int i = threadIdx.x + blockIdx.x * blockDim.x;
     float* const table = (kSide == 32) ? g_heur32 : g_heur64;
     if (i < kN) table[(kNews ? kN : 0) + i] = heuristic_of<kNews>(i >> kShift, i & (kSide - 1), 0, 0);
+}
+
+// ---- black-box backward -----------------------------------------------------------------------------------------
+// cell i of w' = fl(w + fl(lambda * g)): two roundings, no FMA, no clamp (w' may be negative)
+__device__ __forceinline__ float bb_cost(const float* cost, const float* grad, int i, float lam) {
+    return __fadd_rn(__ldg(cost + i), __fmul_rn(lam, __ldg(grad + i)));
+}
+
+// dL/dw of one cell: (y' - y) / lambda, y' = closed after the search on w', y = the forward's histories; exactly 0 or
+// +-fl(1/lambda)
+__device__ __forceinline__ float bb_grad(bool closed, float y, float lam) {
+    return __fdiv_rn((closed ? 1.f : 0.f) - y, lam);
 }
 
 // ---- outputs ----------------------------------------------------------------------------------------------------

@@ -49,8 +49,12 @@ struct GenericLayout {
 // T steps) or a pass of the coupled forward, kExitCoupled1 / kExitCoupled2 (nastar_common.cuh).
 // kNews: NASTAR_FWD_NEWS / NASTAR_MECH_NEWS — only lanes 1, 3, 5, 7 (N, W, E, S) take a neighbour, and h is the
 // Manhattan heuristic.
-template <bool kGlobal, bool kTrace, bool kBwd, int kExit = kExitEarly, bool kNews = false>
+// kMode: kExit, plus kExitBlackbox for the black-box backward (nastar_common.cuh): the search reads w' (into shared
+// memory, or cell by cell when kGlobal) and writes dL/dw in place of its outputs.
+template <bool kGlobal, bool kTrace, bool kBwd, int kMode = kExitEarly, bool kNews = false>
 __global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
+    enum : int { kExit = kMode & ~kExitBlackbox };          // enumerators, as in the 32-wide engine
+    enum : bool { kBB = (kMode & kExitBlackbox) != 0 };
     constexpr bool kContinue = kBwd || (kExit != kExitEarly);
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const nastar_fwd_params& p = a.f;
@@ -118,10 +122,11 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
         const float* gStart = p.start + int64_t(b) * p.start_stride;
         const float* gGoal = p.goal + int64_t(b) * p.goal_stride;
         const float* gObst = p.obst + int64_t(b) * p.obst_stride;
+        const float* gGrad = kBB ? a.grad_hist + int64_t(b) * a.grad_stride : nullptr;
 
         // ---- prologue: cost plane -> smem (TMA), bit rows from obstacle/start/goal planes -------
         if (!kGlobal) {
-            const bool tma_ok = ((N & 3) == 0) && aligned16(gCost);
+            const bool tma_ok = !kBB && ((N & 3) == 0) && aligned16(gCost);
             if (tma_ok) {
                 if (lane == 0) {
                     fence_proxy_async();  // earlier generic-proxy accesses to sCost (previous map) are ordered
@@ -129,7 +134,7 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
                     tma_load_1d(sCost, gCost, uint32_t(N) * 4u, bar);
                 }
             } else {
-                for (int i = lane; i < N; i += 32) sCost[i] = __ldg(gCost + i);
+                for (int i = lane; i < N; i += 32) sCost[i] = kBB ? bb_cost(gCost, gGrad, i, a.bb_lambda) : __ldg(gCost + i);
             }
             (void)tma_ok;
         }
@@ -206,11 +211,13 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
         for (int i = lane; i < L.nbits; i += 32) { sOpen[i] = 0u; sClosed[i] = 0u; }
         for (int y = lane; y < H; y += 32) { sRmKey[y] = kKeyInf; sRmCol[y] = 0; }
         if (!kGlobal) {
-            if (((N & 3) == 0) && aligned16(gCost)) { mbar_wait(bar, bar_parity); bar_parity ^= 1u; }
+            if (!kBB && ((N & 3) == 0) && aligned16(gCost)) { mbar_wait(bar, bar_parity); bar_parity ^= 1u; }
         }
         __syncwarp();
         const int gy = goal_idx / W, gx = goal_idx - gy * W;
-        auto cost_at = [&](int i) -> float { return kGlobal ? __ldg(gCost + i) : sCost[i]; };
+        auto cost_at = [&](int i) -> float {
+            return kGlobal ? (kBB ? bb_cost(gCost, gGrad, i, a.bb_lambda) : __ldg(gCost + i)) : sCost[i];
+        };
 
         int ts_in = NASTAR_TS_CAPPED;
         bool blocked = false;
@@ -411,6 +418,15 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
             a.cw.first[b] = t_solve;
         }
 
+        if constexpr (kBB) {
+            // black-box backward: dL/dw = (closed cells of this search on w' - the forward's histories) / lambda
+            const float* gY = a.bb_hist + int64_t(b) * N;
+            float* gOut = a.grad_cost + int64_t(b) * N;
+            for (int i = lane; i < N; i += 32) {
+                const int y = i / W, x = i - y * W;
+                gOut[i] = bb_grad((sClosed[y * Wd + (x >> 5)] >> (x & 31)) & 1u, __ldg(gY + i), a.bb_lambda);
+            }
+        }
         if (kBwd) {
             // close the intervals of the cells still open at the end, then scale
             const float coef = -omg / a.sqrt_w;
@@ -423,7 +439,7 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
             }
             __syncwarp();
         }
-        if (!kBwd) {
+        if (!kBwd && !kBB) {
         // ---- backtrack (differentiable_astar.py:96-125): follow direction codes ---------------
         for (int i = lane; i < L.nbits; i += 32) sPath[i] = 0u;   // sPath aliases sPass
         __syncwarp();

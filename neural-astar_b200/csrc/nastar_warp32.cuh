@@ -51,8 +51,13 @@ struct __align__(16) W32Smem {
 // kFused (forward only): the prologue may have to finish the encoder (NASTAR_COST_LOGIT / NASTAR_COST_TAPS); kept out
 // of the plain instantiation so that its cold instruction footprint stays small.
 // kNews: NASTAR_FWD_NEWS / NASTAR_MECH_NEWS — 4-connected expansion (N, E, W, S) and the Manhattan heuristic.
-template <bool kTrace, bool kBwd, int kExit = kExitEarly, bool kFused = false, bool kNews = false>
+// kMode: kExit, plus kExitBlackbox for the black-box backward (forward search on w', dL/dw in place of the outputs).
+template <bool kTrace, bool kBwd, int kMode = kExitEarly, bool kFused = false, bool kNews = false>
 __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const SearchArgs a) {
+    // enumerators, not constexpr variables: the instantiations without kExitBlackbox then compile to the code they had
+    // before the black-box backward existed
+    enum : int { kExit = kMode & ~kExitBlackbox };
+    enum : bool { kBB = (kMode & kExitBlackbox) != 0 };
     constexpr bool kContinue = kBwd || (kExit != kExitEarly);   // the loop does not stop at the solve step
     __shared__ W32Smem S;
     extern __shared__ __align__(16) unsigned char bwd_raw[];  // backward only: W32Bwd
@@ -72,7 +77,7 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const SearchArgs a
     const float* gCost = vanilla_half ? gObst : (p.cost + int64_t(bi) * p.cost_stride);
     const int cost_kind = (!kFused || kBwd || vanilla_half) ? NASTAR_COST_PLANE : p.cost_kind;
     const bool cost_plane = (cost_kind == NASTAR_COST_PLANE);
-    const bool obst_is_cost = cost_plane && (gObst == gCost);
+    const bool obst_is_cost = !kBB && cost_plane && (gObst == gCost);   // w' is never the obstacle plane
     if constexpr (kExit == kExitCoupled2) {
         const int Tc = *a.T_batch;
         if (a.cw.stop[b] <= Tc) {   // pass 1's outputs stand
@@ -84,7 +89,7 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const SearchArgs a
     // ---------------- prologue: stage planes, build row masks ------------------------------
     uint32_t pass = 0u;
     int start_rc = -1, goal_rc = -1;
-    const bool tma = (W == 32) && (!cost_plane || aligned16(gCost)) && aligned16(gStart) && aligned16(gGoal) && aligned16(gObst);
+    const bool tma = !kBB && (W == 32) && (!cost_plane || aligned16(gCost)) && aligned16(gStart) && aligned16(gGoal) && aligned16(gObst);
     if (tma) {
         // flat layout == padded layout: bulk-copy whole planes (start/goal/obstacles are parked in the
         // f and {g,h} planes, which are not live yet)
@@ -134,7 +139,7 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const SearchArgs a
                 const bool ok = in && (y0 + u < H);
                 const int i = (y0 + u) * W + lane;
                 vc[u] = ok ? (kFused ? cost_value(cost_kind, gCost, y0 + u, lane, H, W, p.cost_bias, p.cost_scale)
-                                     : __ldg(gCost + i)) : 0.f;
+                                     : kBB ? bb_cost(gCost, a.grad_hist + int64_t(bi) * a.grad_stride, i, a.bb_lambda) : __ldg(gCost + i)) : 0.f;
                 vo[u] = obst_is_cost ? vc[u] : (ok ? __ldg(gObst + i) : 0.f);
                 vs[u] = ok ? __ldg(gStart + i) : 0.f;
                 vg[u] = ok ? __ldg(gGoal + i) : 0.f;
@@ -358,6 +363,19 @@ __global__ void __launch_bounds__(32, 12) astar_warp32_kernel(const SearchArgs a
         // is the same record: no step past the cap is ever read)
         a.cw.end[b] = (t_solve == NASTAR_TS_EXHAUSTED) ? kEndExhausted : ((t < T) ? kEndFixed : kEndCapped);
         a.cw.first[b] = t_solve;
+    }
+
+    if constexpr (kBB) {
+        // black-box backward: dL/dw = (closed rows of this search on w' - the forward's histories) / lambda
+        S.bits_a[lane] = closed;
+        __syncwarp();
+        const float* gY = a.bb_hist + int64_t(b) * N;
+        float* gOut = a.grad_cost + int64_t(b) * N;
+        for (int y = 0; y < H; ++y) {
+            const int i = y * W + lane;
+            if (lane < W) gOut[i] = bb_grad((S.bits_a[y] >> lane) & 1u, __ldg(gY + i), a.bb_lambda);
+        }
+        return;
     }
 
     if (kBwd) {

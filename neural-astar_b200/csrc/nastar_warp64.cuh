@@ -43,9 +43,14 @@ struct __align__(16) W64Bwd {
 // kFused (forward only): the prologue may have to finish the encoder (NASTAR_COST_LOGIT / NASTAR_COST_TAPS), as in the
 // 32-wide engine; kept out of the plain instantiations.
 // kNews: 4-connected expansion and the Manhattan heuristic, as in the 32-wide engine.
-// kExit: exit mode of the forward (kExitEarly, kExitNone, or a pass of the coupled forward), as in the 32-wide engine.
-template <bool kTrace, int kExit, bool kBwd = false, bool kFused = false, bool kNews = false>
+// kMode: exit mode of the forward (kExitEarly, kExitNone, or a pass of the coupled forward), plus kExitBlackbox for the
+// black-box backward, as in the 32-wide engine.
+template <bool kTrace, int kMode, bool kBwd = false, bool kFused = false, bool kNews = false>
 __global__ void __launch_bounds__(32) astar_warp64_kernel(const SearchArgs a) {
+    // enumerators, not constexpr variables: the instantiations without kExitBlackbox then compile to the code they had
+    // before the black-box backward existed
+    enum : int { kExit = kMode & ~kExitBlackbox };
+    enum : bool { kBB = (kMode & kExitBlackbox) != 0 };
     constexpr bool kContinue = kBwd || (kExit != kExitEarly);
     const nastar_fwd_params& p = a.f;
     extern __shared__ __align__(16) unsigned char smem64_raw[];
@@ -63,7 +68,7 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const SearchArgs a) {
     const float* gObst = p.obst + int64_t(b) * p.obst_stride;
     const int cost_kind = (kFused && !kBwd) ? p.cost_kind : NASTAR_COST_PLANE;
     const bool cost_plane = (cost_kind == NASTAR_COST_PLANE);
-    const bool obst_is_cost = cost_plane && (gObst == gCost);
+    const bool obst_is_cost = !kBB && cost_plane && (gObst == gCost);   // w' is never the obstacle plane
     if constexpr (kExit == kExitCoupled2) {
         const int Tc = *a.T_batch;
         if (a.cw.stop[b] <= Tc) {   // pass 1's outputs stand
@@ -75,7 +80,7 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const SearchArgs a) {
     // ---------------- prologue ----------------------------------------------------------------
     u64 pass[2] = {0ull, 0ull};
     int start_rc = -1, goal_rc = -1;
-    const bool tma = (W == 64) && (!cost_plane || aligned16(gCost)) && aligned16(gStart) && aligned16(gGoal) && aligned16(gObst);
+    const bool tma = !kBB && (W == 64) && (!cost_plane || aligned16(gCost)) && aligned16(gStart) && aligned16(gGoal) && aligned16(gObst);
     if (tma) {
         float* tStart = reinterpret_cast<float*>(S.key);
         float* tGoal = reinterpret_cast<float*>(sGH);
@@ -128,7 +133,7 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const SearchArgs a) {
                     const bool ok = (hf ? in1 : in0) && (y0 + u < H);
                     const int i = (y0 + u) * W + lane + 32 * hf;
                     vc[u][hf] = ok ? (kFused ? cost_value(cost_kind, gCost, y0 + u, lane + 32 * hf, H, W, p.cost_bias, p.cost_scale)
-                                             : __ldg(gCost + i)) : 0.f;
+                                             : kBB ? bb_cost(gCost, a.grad_hist + int64_t(b) * a.grad_stride, i, a.bb_lambda) : __ldg(gCost + i)) : 0.f;
                     vo[u][hf] = obst_is_cost ? vc[u][hf] : (ok ? __ldg(gObst + i) : 0.f);
                     vs[u][hf] = ok ? __ldg(gStart + i) : 0.f;
                     vg[u][hf] = ok ? __ldg(gGoal + i) : 0.f;
@@ -367,6 +372,19 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const SearchArgs a) {
         // is the same record: no step past the cap is ever read)
         a.cw.end[b] = (t_solve == NASTAR_TS_EXHAUSTED) ? kEndExhausted : ((t < T) ? kEndFixed : kEndCapped);
         a.cw.first[b] = t_solve;
+    }
+
+    if constexpr (kBB) {
+        // black-box backward: dL/dw = (closed rows of this search on w' - the forward's histories) / lambda
+        S.bits_a[lane] = closed[0];
+        S.bits_a[lane + 32] = closed[1];
+        __syncwarp();
+        const float* gY = a.bb_hist + int64_t(b) * N;
+        float* gOut = a.grad_cost + int64_t(b) * N;
+        for (int y = 0; y < H; ++y)
+            for (int x = lane; x < W; x += 32)
+                gOut[y * W + x] = bb_grad((S.bits_a[y] >> x) & 1ull, __ldg(gY + y * W + x), a.bb_lambda);
+        return;
     }
 
     if (kBwd) {

@@ -85,6 +85,7 @@ _SIGNATURES = {
     "nastar_b200_forward_coupled": (_int, [ctypes.POINTER(FwdParams), _p, _p, _p]),
     "nastar_b200_backward": (_int, [ctypes.POINTER(BwdParams), _p]),
     "nastar_b200_backward_mech": (_int, [ctypes.POINTER(BwdParams), _i32, _p]),
+    "nastar_b200_backward_blackbox": (_int, [ctypes.POINTER(FwdParams), _p, _p, _i64, ctypes.c_float, _p, _p, _p, _p]),
     "nastar_b200_batch_steps": (_int, [_p, _p, _i32, _i32, _p, _p]),
     "nastar_b200_engine_for": (_int, [_i32, _i32]),
     "nastar_b200_bin16_supported": (_int, [_i32, _i32]),
@@ -894,6 +895,62 @@ def backward(cost, start, goal, obst, grad_hist: torch.Tensor, T_batch, t_solve:
         p.workspace_bytes = ws_bytes
         _check(L.nastar_b200_backward_mech(ctypes.byref(p), mech, stream), "nastar_b200_backward_mech")
     del keep
+    return grad_cost
+
+
+def check_lambda(lam: float) -> float:
+    """The black-box backward's lambda as the fp32 value the library receives, or a ValueError when that value is not
+    finite or not > 0."""
+    with np.errstate(over="ignore"):
+        lam32 = float(np.float32(lam))
+    if not (math.isfinite(lam32) and lam32 > 0.0):
+        raise ValueError(f"the black-box lambda must be a finite float32 > 0 (got {lam!r})")
+    return lam32
+
+
+def backward_blackbox(cost: torch.Tensor, start: torch.Tensor, goal: torch.Tensor, obst: torch.Tensor,
+                      hist: torch.Tensor, grad_hist: torch.Tensor, lam: float, g_ratio: float, T: int, *,
+                      mechanism: str = "moore", coupled: bool = False) -> torch.Tensor:
+    """dL/dcost [B,1,H,W] of the black-box backward (BB-A*, include/nastar_b200.h, nastar_b200_backward_blackbox):
+    (y(w') - hist) / lam with w' = fl(cost + fl(lam * grad_hist)) and y the histories of the same search on w'.
+    `hist` [B,1,H,W] are the forward's histories for `cost`; the planes are those of `forward` (channel 0 of `cost` is
+    searched).  `coupled` = False: each map of the search on w' stops at its solve step, one launch (the forward without
+    flags, exact for g_ratio >= 0.5 or one map).  `coupled` = True: the batch-coupled search of `forward_coupled` with
+    cap `T`, its T_batch decided on the device, three launches.  Asynchronous on the current stream, no host
+    synchronisation."""
+    lam = check_lambda(lam)
+    p, keep, B, H, W, dev = _search_params(cost, start, goal, obst, g_ratio, T, 0, COST_PLANE, 1.0, 0.0, mechanism)
+    for name, t_ in (("hist", hist), ("grad_hist", grad_hist)):
+        if t_.device != dev:
+            raise RuntimeError("all planes must live on the same CUDA device")
+        if t_.shape[0] != B or t_.shape[-2:] != (H, W):
+            raise ValueError(f"{name} must be [B,1,H,W] like the search planes")
+    if hist.dtype != torch.float32:
+        raise TypeError("hist must be the forward's float32 histories")
+    hk = hist.detach().reshape(B, H * W).contiguous()
+    gk, g_ptr, g_stride = _plane(grad_hist.detach().to(torch.float32))
+    L = lib()
+    if coupled:
+        key = (B, H, W, int(T))
+        ws_bytes = _coupled_ws_cache.get(key)
+        if ws_bytes is None:
+            ws_bytes = _coupled_ws_cache[key] = int(L.nastar_b200_forward_coupled_workspace_bytes(B, H, W, int(T)))
+    else:
+        ws_bytes = _ws_cache.get((B, H, W))
+        if ws_bytes is None:
+            ws_bytes = _ws_cache[(B, H, W)] = int(L.nastar_b200_forward_workspace_bytes(B, H, W))
+    with _on_device(dev) as stream:
+        grad_cost = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
+        # coupled: the search on w' gets its own T_batch [1] and goal clamp [B] (the second is not needed here)
+        rec = torch.empty((B + 1,), dtype=torch.int32, device=dev) if coupled else None
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None
+        p.workspace = ws.data_ptr() if ws is not None else None
+        p.workspace_bytes = ws_bytes
+        _check(L.nastar_b200_backward_blackbox(ctypes.byref(p), hk.data_ptr(), g_ptr, g_stride, lam,
+                                               grad_cost.data_ptr(), rec[:1].data_ptr() if coupled else None,
+                                               rec[1:].data_ptr() if coupled else None, stream),
+               "nastar_b200_backward_blackbox")
+    del keep, hk, gk
     return grad_cost
 
 

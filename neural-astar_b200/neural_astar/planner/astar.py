@@ -23,7 +23,7 @@ import torch.nn.functional as F
 
 from .. import _native
 from . import encoder as _encoders
-from .differentiable_astar import AstarOutput, DifferentiableAstar, TakesMechanism, _mech_kw, batch_coupled
+from .differentiable_astar import AstarOutput, BlackboxAstar, DifferentiableAstar, TakesMechanism, _mech_kw, batch_coupled
 from .pq_astar import _check_semantics, pq_astar  # noqa: F401  pq_astar re-exported, like the reference module does
 
 
@@ -197,3 +197,40 @@ class NeuralAstar(VanillaAstar):
         hist, paths, _, _, _, counts = _native.forward(cost, start_maps, goal_maps, map_designs, float(self.g_ratio), T,
                                                        pair=True, want_counts=True, **kw)
         return (AstarOutput(hist[:B], paths[:B], []), AstarOutput(hist[B:], paths[B:], []), tuple(counts))
+
+
+class BBAstar(NeuralAstar):
+    """BB-A*: Neural A*'s encoder trained through a non-differentiable A*, with the black-box gradient of Vlastelica
+    et al., "Differentiation of Blackbox Combinatorial Solvers" (ICLR 2020).  The learned baseline that the Neural A*
+    paper (Yonetani et al., ICML 2021) sets against Neural A*.
+
+    The forward is NeuralAstar's, output for output.  The backward takes the incoming gradient g = dL/dhistories,
+    searches again on the perturbed costs w' = fl(w + fl(lambda * g)) (same g_ratio, step bound, mechanism and
+    obstacles; w' may be negative) and returns dL/dcost = (histories(w') - histories(w)) / lambda, every cell 0 or
+    +-fl(1/lambda); only channel 0 of a multi-channel cost gets a gradient.  Below g_ratio 0.5 a batch of more than one
+    map is searched batch-coupled in both searches, each with its own T_batch decided on the device.  The backward is
+    one search launch (three when coupled) and never synchronises with the host, so GraphedTrainStep captures it.
+
+    The default bbastar_lambda = 20.0 is the value Vlastelica et al. use in their shortest-path experiments, and the
+    formula follows the two papers.  Neither is checked against the Neural A* authors' own BB-A* code, which is not
+    part of the reference this project follows.
+
+    Args: NeuralAstar's, plus
+        bbastar_lambda: the interpolation strength lambda, a finite float32 > 0 (ValueError otherwise).
+    use_differentiable_astar=False is a ValueError: pq_astar has no black-box gradient.  The state dict is
+    NeuralAstar's key for key (lambda is not a buffer), so checkpoints load either way.
+    """
+
+    def __init__(self, g_ratio: float = 0.5, Tmax: float = 1.0, encoder_input: str = "m+", encoder_arch: str = "CNN",
+                 encoder_depth: int = 4, learn_obstacles: bool = False, const: Optional[float] = None,
+                 use_differentiable_astar: bool = True, bbastar_lambda: float = 20.0):
+        if not use_differentiable_astar:
+            raise ValueError("BBAstar needs use_differentiable_astar=True: pq_astar has no black-box gradient")
+        astar = BlackboxAstar(g_ratio=g_ratio, Tmax=Tmax, bbastar_lambda=bbastar_lambda)
+        super().__init__(g_ratio, Tmax, encoder_input, encoder_arch, encoder_depth, learn_obstacles, const,
+                         use_differentiable_astar)
+        self.astar = astar
+
+    @property
+    def bbastar_lambda(self) -> float:
+        return self.astar.bbastar_lambda

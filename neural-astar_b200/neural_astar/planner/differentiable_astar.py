@@ -127,27 +127,43 @@ class TakesMechanism(type):
         return planner
 
 
+def _search(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped, mechanism,
+            device_coupled):
+    """The search of _AstarSearch.forward: (histories, paths, t_solve, n_steps, trace, T_batch, goal_clamp).
+    goal_clamped is given only on the batch-coupled path (g_ratio < 0.5, see _coupled_steps): the search then runs
+    exactly T steps per map.  device_coupled: the same batch coupling decided on the device (_native.forward_coupled, T
+    is the cap), which returns T_batch and the goal clamp as device tensors (None otherwise)."""
+    if device_coupled:
+        hist, paths, t_solve, n_steps, T_batch, goal_clamp = _native.forward_coupled(
+            cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, **_mech_kw(mechanism))
+        return hist, paths, t_solve, n_steps, None, T_batch, goal_clamp
+    no_early_exit = goal_clamped is not None
+    hist, paths, t_solve, n_steps, trace = _native.forward(
+        cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, no_early_exit, **_mech_kw(mechanism))
+    return hist, paths, t_solve, n_steps, trace, None, None
+
+
+def _channel0_grad(grad_cost: torch.Tensor, cost: torch.Tensor) -> torch.Tensor:
+    """dL/dcost for all of `cost`'s channels from the gradient of channel 0, the only one searched (:177)."""
+    if grad_cost.shape != cost.shape:
+        full = torch.zeros_like(cost)
+        full[:, :1] = grad_cost
+        grad_cost = full
+    return grad_cost
+
+
 class _AstarSearch(torch.autograd.Function):
     """forward: libnastar_b200 search; backward: closed-form dL/dcost kernel."""
 
     @staticmethod
     def forward(ctx, cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped=None,
                 mechanism="moore", device_coupled=False):
-        # goal_clamped is given only on the batch-coupled path (g_ratio < 0.5, see _coupled_steps): the search then
-        # runs exactly T steps per map and the backward is told which goals were selected more than once.
-        # device_coupled: the same batch coupling decided on the device (_native.forward_coupled, T is the cap), which
-        # hands T_batch and the goal clamp to the backward as device tensors
-        ctx.device_T_batch = None
-        if device_coupled:
-            hist, paths, t_solve, n_steps, T_batch, goal_clamp = _native.forward_coupled(
-                cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, **_mech_kw(mechanism))
-            trace = None
-            ctx.device_T_batch = T_batch
-        else:
-            no_early_exit = goal_clamped is not None
-            hist, paths, t_solve, n_steps, trace = _native.forward(
-                cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, no_early_exit,
-                **_mech_kw(mechanism))
+        # goal_clamped (host-coupled) and device_coupled: see _search.  The backward is told which goals were selected
+        # more than once, and on the device route gets T_batch and the goal clamp as device tensors
+        hist, paths, t_solve, n_steps, trace, T_batch, goal_clamp = _search(
+            cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped, mechanism,
+            device_coupled)
+        ctx.device_T_batch = T_batch
         ctx.g_ratio = g_ratio
         ctx.mechanism = mechanism
         ctx.T = T
@@ -178,11 +194,40 @@ class _AstarSearch(torch.autograd.Function):
                 T_batch = _native.batch_steps(t_solve, n_steps, ctx.T)
             grad_cost = _native.backward(cost, start, goal, obst, grad_hist.contiguous(), T_batch, t_solve, ctx.g_ratio,
                                          **_mech_kw(ctx.mechanism))
-            if grad_cost.shape != cost.shape:  # cost had extra channels: only channel 0 is searched (:177)
-                full = torch.zeros_like(cost)
-                full[:, :1] = grad_cost
-                grad_cost = full
+            grad_cost = _channel0_grad(grad_cost, cost)
         return grad_cost, None, None, None, None, None, None, None, None, None
+
+
+class _BlackboxSearch(torch.autograd.Function):
+    """forward: _AstarSearch's search call, also keeping its histories; backward: the black-box gradient of Vlastelica
+    et al. (ICLR 2020), (y(w + lam * dL/dhistories) - y(w)) / lam, from one more search on the perturbed costs
+    (_native.backward_blackbox).  `T_cap` is the search's step bound; the forward's own T is T_batch on the host-coupled
+    path.  `coupled`: the search on the perturbed costs is batch-coupled too, with its own T_batch decided on the
+    device."""
+
+    @staticmethod
+    def forward(ctx, cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped, mechanism,
+                device_coupled, lam, T_cap, coupled):
+        hist, paths, t_solve, n_steps, trace, _, _ = _search(
+            cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped, mechanism,
+            device_coupled)
+        ctx.lam, ctx.g_ratio, ctx.mechanism, ctx.T_cap, ctx.coupled = lam, g_ratio, mechanism, T_cap, coupled
+        ctx.save_for_backward(cost_maps, start_maps, goal_maps, obstacles_maps, hist)
+        ctx.mark_non_differentiable(paths, t_solve, n_steps)
+        if trace is not None:
+            ctx.mark_non_differentiable(trace)
+        return hist, paths, t_solve, n_steps, trace
+
+    @staticmethod
+    def backward(ctx, grad_hist, *_unused):
+        cost, start, goal, obst, hist = ctx.saved_tensors
+        grad_cost = None
+        if ctx.needs_input_grad[0]:
+            grad_cost = _native.backward_blackbox(cost, start, goal, obst, hist, grad_hist.contiguous(), ctx.lam,
+                                                  ctx.g_ratio, ctx.T_cap, coupled=ctx.coupled,
+                                                  **_mech_kw(ctx.mechanism))
+            grad_cost = _channel0_grad(grad_cost, cost)
+        return (grad_cost,) + (None,) * 12
 
 
 class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
@@ -240,13 +285,14 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
         g_ratio = float(self.g_ratio)
         coupled = batch_coupled(g_ratio, cost_maps.shape[0])
         goal_clamped = None
+        T_cap = T
         if coupled and cost_maps.is_cuda and torch.cuda.is_current_stream_capturing():
             # under CUDA-graph capture the host decision below cannot happen: decide T_batch on the device instead
             # (_native.forward_coupled, the same outputs and gradient); frames need the host procedure's trace
             if store_intermediate_results:
                 raise ValueError("store_intermediate_results needs a host sync and cannot be captured")
-            hist, paths, _, _, _ = _AstarSearch.apply(
-                cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, False, None, self.mechanism, True)
+            hist, paths, _, _, _ = self._apply_search(
+                cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, False, None, True, T, coupled)
             return AstarOutput(hist, paths, [])
         if coupled:
             # For g_ratio < 0.5 a solved map does not necessarily keep re-selecting its goal (SURVEY App. A.4),
@@ -256,9 +302,9 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
             # synchronises every step.)
             T, goal_clamped = _coupled_steps(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T,
                                              self.mechanism)
-        hist, paths, t_solve, n_steps, trace = _AstarSearch.apply(
+        hist, paths, t_solve, n_steps, trace = self._apply_search(
             cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, bool(store_intermediate_results), goal_clamped,
-            self.mechanism)
+            False, T_cap, coupled)
 
         intermediate_results: List[dict] = []
         if store_intermediate_results and _recording.get() is not None:
@@ -268,6 +314,16 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
                                                        T_batch=T if coupled else None)
         return AstarOutput(hist, paths, intermediate_results)
 
+
+    def _apply_search(self, cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped,
+                      device_coupled, T_cap, coupled):
+        """The autograd search of forward(): T is the step count the search runs (T_batch on the host-coupled path),
+        T_cap the step bound int(Tmax * W * W), `coupled` whether the batch is searched batch-coupled."""
+        if device_coupled:
+            return _AstarSearch.apply(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace,
+                                      goal_clamped, self.mechanism, True)
+        return _AstarSearch.apply(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped,
+                                  self.mechanism)
 
     def search_from_taps(self, taps: torch.Tensor, bias: float, scale: float, start_maps: torch.Tensor,
                          goal_maps: torch.Tensor, obstacles_maps: torch.Tensor,
@@ -296,6 +352,21 @@ class DifferentiableAstar(nn.Module, metaclass=TakesMechanism):
         elif store_intermediate_results:
             frames = _materialise_frames(hist, paths, goal_maps, t_solve, n_steps, trace, T)
         return AstarOutput(hist, paths, frames)
+
+
+class BlackboxAstar(DifferentiableAstar):
+    """DifferentiableAstar whose gradient is the black-box one of BB-A* (_BlackboxSearch): the same forward, and in the
+    backward one more search on the costs perturbed by `bbastar_lambda` times the incoming gradient.  Its state dict
+    is DifferentiableAstar's; lambda is an attribute, not a buffer."""
+
+    def __init__(self, g_ratio: float = 0.5, Tmax: float = 1.0, bbastar_lambda: float = 20.0):
+        super().__init__(g_ratio=g_ratio, Tmax=Tmax)
+        self.bbastar_lambda = _native.check_lambda(bbastar_lambda)
+
+    def _apply_search(self, cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace, goal_clamped,
+                      device_coupled, T_cap, coupled):
+        return _BlackboxSearch.apply(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio, T, want_trace,
+                                     goal_clamped, self.mechanism, device_coupled, self.bbastar_lambda, T_cap, coupled)
 
 
 def _coupled_steps(cost_maps, start_maps, goal_maps, obstacles_maps, g_ratio: float, T: int, mechanism: str = "moore"):
