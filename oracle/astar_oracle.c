@@ -9,7 +9,7 @@
  *   src/neural_astar/planner/differentiable_astar.py
  *     :26-52   get_heuristic          -> heuristic_plus_cost()
  *     :55-74   _st_softmax_noexp      -> select_literal()
- *     :77-93   expand (3x3 stencil)   -> the 8-neighbour loops below
+ *     :77-93   expand (3x3 stencil)   -> the neighbour loops over kDy / kDx below
  *     :96-125  backtrack              -> backtrack_literal() / backtrack_spec()
  *     :187-252 state machine          -> nastar_oracle_forward_literal()
  *   (autograd of the above; closed form SURVEY.md App. B) -> nastar_oracle_backward()
@@ -24,8 +24,13 @@
  *            values into equal softmax weights (measured: 0 in 141k vanilla
  *            selections; see DESIGN.md "selection semantics").
  *
+ * Mechanism (NASTAR_MECH_*, include/nastar_b200.h), as DifferentiableAstar(mechanism=) takes it:
+ *   MOORE  the 8 neighbours, h = Chebyshev + 0.001 * Euclid (the reference's own search);
+ *   NEWS   N, E, W, S only, h = Manhattan + 0.001 * Euclid (the planning-datasets generator's
+ *          NorthEastWestSouth, mechanism.py:113-131; get_news_heuristic's fp32 operation order).
+ *
  * Parity pinning: both restatements are checked against golden vectors produced by
- * running the reference's own Python (tests/golden/make_golden.py) on this box.
+ * running the reference's own Python (tests/golden/make_golden.py, make_golden_news.py).
  *
  * Arithmetic: IEEE fp32, one rounding per op (compile with -ffp-contract=off).
  */
@@ -36,6 +41,8 @@
 #ifdef _OPENMP
 #include <omp.h>
 #endif
+
+#include "nastar_b200.h"
 
 #define NASTAR_ORACLE_OK 0
 #define NASTAR_ORACLE_EINVAL 1
@@ -51,18 +58,24 @@ static int argmax_first(const float *x, int n)
     return best;
 }
 
-/* differentiable_astar.py:26-52 followed by :192 (h = heuristic + cost) */
-static void heuristic_plus_cost(const float *cost, int H, int W, int goal, float *h)
+/* the moves as (dy, dx): N, E, W, S, NE, NW, SE, SW (mechanism.py:58, :140-149); NEWS takes the first 4 */
+static const int kDy[8] = {-1, 0, 0, +1, -1, -1, +1, +1};
+static const int kDx[8] = {0, +1, -1, 0, +1, -1, +1, -1};
+
+static int mech_ok(int mech) { return mech == NASTAR_MECH_MOORE || mech == NASTAR_MECH_NEWS; }
+static int num_moves(int mech) { return mech == NASTAR_MECH_NEWS ? 4 : 8; }
+
+/* differentiable_astar.py:26-52 (Moore) or get_news_heuristic (NEWS), followed by :192 (h = heuristic + cost) */
+static void heuristic_plus_cost(const float *cost, int H, int W, int goal, int mech, float *h)
 {
     const float gy = (float)(goal / W), gx = (float)(goal % W);
     for (int y = 0; y < H; ++y) {
         for (int x = 0; x < W; ++x) {
             float dy = fabsf((float)y - gy), dx = fabsf((float)x - gx);
-            float cheb = (dy + dx) - fminf(dy, dx);
-            float ey = (float)y - gy, ex = (float)x - gx;
-            float euc = sqrtf(ey * ey + ex * ex);
+            float dist = (mech == NASTAR_MECH_NEWS) ? dy + dx : (dy + dx) - fminf(dy, dx);
+            float euc = sqrtf(dy * dy + dx * dx);
             float t = 0.001f * euc;
-            float heur = cheb + t;
+            float heur = dist + t;
             h[y * W + x] = heur + cost[y * W + x];
         }
     }
@@ -98,7 +111,7 @@ typedef struct {
 /* one loop iteration of differentiable_astar.py:206-249 for one map; returns 1 if
  * this map is "unsolved" after the step (is_unsolved, :220). */
 static int literal_step(lit_map_t *m, const float *cost, const float *obst, const float *goalmap,
-                        int H, int W, float gr, float omg, float sqrtw, int t, int32_t *trace_out)
+                        int H, int W, int nmoves, float gr, float omg, float sqrtw, int t, int32_t *trace_out)
 {
     const int N = H * W;
     float s = 0.0f;
@@ -120,22 +133,19 @@ static int literal_step(lit_map_t *m, const float *cost, const float *obst, cons
     /* :222-225 */
     m->hist[ind] = fminf(fmaxf(m->hist[ind] + 1.0f, 0.0f), 1.0f);
     m->open[ind] = fminf(fmaxf(m->open[ind] - unsolved * 1.0f, 0.0f), 1.0f);
-    /* :228-249 — only the 8 neighbours of ind have neighbor_nodes != 0 */
+    /* :228-249 — only the neighbours of ind under the filter have neighbor_nodes != 0 */
     const int r = ind / W, c = ind % W;
     const float g2 = m->g[ind] + cost[ind];            /* :234 (g+cost)*sel through the stencil */
-    for (int dr = -1; dr <= 1; ++dr) {
-        for (int dc = -1; dc <= 1; ++dc) {
-            if (!dr && !dc) continue;
-            int y = r + dr, x = c + dc;
-            if (y < 0 || y >= H || x < 0 || x >= W) continue; /* zero padding, :91 */
-            int n = y * W + x;
-            float nbr = 1.0f * obst[n];                /* :229 */
-            float gt = (m->g[n] > g2) ? 1.0f : 0.0f;
-            float idx = ((1.0f - m->open[n]) * (1.0f - m->hist[n]) + m->open[n] * gt) * nbr; /* :235-236 */
-            m->g[n] = g2 * idx + m->g[n] * (1.0f - idx);                  /* :238 */
-            m->open[n] = fminf(fmaxf(m->open[n] + idx, 0.0f), 1.0f);     /* :242 */
-            m->parents[n] = (float)ind * idx + m->parents[n] * (1.0f - idx); /* :249 */
-        }
+    for (int k = 0; k < nmoves; ++k) {
+        int y = r + kDy[k], x = c + kDx[k];
+        if (y < 0 || y >= H || x < 0 || x >= W) continue; /* zero padding, :91 */
+        int n = y * W + x;
+        float nbr = 1.0f * obst[n];                /* :229 */
+        float gt = (m->g[n] > g2) ? 1.0f : 0.0f;
+        float idx = ((1.0f - m->open[n]) * (1.0f - m->hist[n]) + m->open[n] * gt) * nbr; /* :235-236 */
+        m->g[n] = g2 * idx + m->g[n] * (1.0f - idx);                  /* :238 */
+        m->open[n] = fminf(fmaxf(m->open[n] + idx, 0.0f), 1.0f);     /* :242 */
+        m->parents[n] = (float)ind * idx + m->parents[n] * (1.0f - idx); /* :249 */
     }
     return unsolved != 0.0f;
 }
@@ -157,16 +167,16 @@ static void backtrack_literal(const float *parents, int goal, int N, int current
  * T = number of loop iterations allowed (int(Tmax_eff*W*W), :200-202).
  * Outputs: hist [B][N] fp32, paths [B][N] int64, t_solve [B] (first step the goal was
  * selected, -1 if never), trace [B][T] int32 selected index per executed step (or NULL),
- * *T_batch = number of executed loop iterations.
+ * *T_batch = number of executed loop iterations.  mech: NASTAR_MECH_MOORE or NASTAR_MECH_NEWS.
  */
 int nastar_oracle_forward_literal(const float *cost, const float *start, const float *goal,
                                   const float *obst, int B, int H, int W, float g_ratio,
                                   float one_minus_g_ratio, float sqrt_w, int T,
                                   float *hist, int64_t *paths, int32_t *t_solve, int32_t *trace,
-                                  int32_t *T_batch)
+                                  int32_t *T_batch, int mech)
 {
-    if (B <= 0 || H <= 0 || W <= 0 || T <= 0) return NASTAR_ORACLE_EINVAL;
-    const int N = H * W;
+    if (B <= 0 || H <= 0 || W <= 0 || T <= 0 || !mech_ok(mech)) return NASTAR_ORACLE_EINVAL;
+    const int N = H * W, nm = num_moves(mech);
     lit_map_t *maps = (lit_map_t *)calloc((size_t)B, sizeof(lit_map_t));
     float *pool = (float *)calloc((size_t)B * N * 6, sizeof(float));
     for (int b = 0; b < B; ++b) {
@@ -177,7 +187,7 @@ int nastar_oracle_forward_literal(const float *cost, const float *start, const f
         m->goal = argmax_first(goal + (size_t)b * N, N);   /* :197 */
         m->start = argmax_first(start + (size_t)b * N, N);
         m->solved_at = -1;
-        heuristic_plus_cost(cost + (size_t)b * N, H, W, m->goal, m->h); /* :191-192 */
+        heuristic_plus_cost(cost + (size_t)b * N, H, W, m->goal, mech, m->h); /* :191-192 */
         memcpy(m->open, start + (size_t)b * N, sizeof(float) * N);       /* :187 */
         for (int i = 0; i < N; ++i) m->parents[i] = (float)m->goal;      /* :195-198 */
     }
@@ -194,7 +204,7 @@ int nastar_oracle_forward_literal(const float *cost, const float *start, const f
             int t = 0;
             for (t = 0; t < T; ++t) {
                 int uns = literal_step(&maps[b], cost + (size_t)b * N, obst + (size_t)b * N, goal + (size_t)b * N,
-                                       H, W, g_ratio, one_minus_g_ratio, sqrt_w, t,
+                                       H, W, nm, g_ratio, one_minus_g_ratio, sqrt_w, t,
                                        trace ? trace + (size_t)b * T + t : NULL);
                 if (!uns) { ++t; break; }
             }
@@ -204,7 +214,7 @@ int nastar_oracle_forward_literal(const float *cost, const float *start, const f
 #pragma omp parallel for schedule(dynamic, 1)
         for (int b = 0; b < B; ++b) {
             for (int t = done[b]; t < tb; ++t)
-                literal_step(&maps[b], cost + (size_t)b * N, obst + (size_t)b * N, goal + (size_t)b * N, H, W,
+                literal_step(&maps[b], cost + (size_t)b * N, obst + (size_t)b * N, goal + (size_t)b * N, H, W, nm,
                              g_ratio, one_minus_g_ratio, sqrt_w, t, trace ? trace + (size_t)b * T + t : NULL);
         }
         free(done);
@@ -216,7 +226,7 @@ int nastar_oracle_forward_literal(const float *cost, const float *start, const f
 #pragma omp parallel for schedule(static) reduction(| : any_unsolved)
             for (int b = 0; b < B; ++b)
                 any_unsolved |= literal_step(&maps[b], cost + (size_t)b * N, obst + (size_t)b * N,
-                                             goal + (size_t)b * N, H, W, g_ratio, one_minus_g_ratio, sqrt_w, t,
+                                             goal + (size_t)b * N, H, W, nm, g_ratio, one_minus_g_ratio, sqrt_w, t,
                                              trace ? trace + (size_t)b * T + t : NULL);
             tb = t + 1;
             if (!any_unsolved) break;
@@ -263,20 +273,18 @@ static int spec_select(const spec_map_t *m, int N, float gr, float omg)
     return best;
 }
 
-static void spec_expand(spec_map_t *m, const float *cost, const float *obst, int H, int W, int ind)
+static void spec_expand(spec_map_t *m, const float *cost, const float *obst, int H, int W, int nmoves, int ind)
 {
     const int r = ind / W, c = ind % W;
     const float g2 = m->g[ind] + cost[ind];
-    for (int dr = -1; dr <= 1; ++dr)
-        for (int dc = -1; dc <= 1; ++dc) {
-            if (!dr && !dc) continue;
-            int y = r + dr, x = c + dc;
-            if (y < 0 || y >= H || x < 0 || x >= W) continue;
-            int n = y * W + x;
-            if (obst[n] == 0.0f) continue;
-            int upd = (!m->open[n] && !m->closed[n]) || (m->open[n] && m->g[n] > g2);
-            if (upd) { m->g[n] = g2; m->open[n] = 1; m->parent[n] = ind; }
-        }
+    for (int k = 0; k < nmoves; ++k) {
+        int y = r + kDy[k], x = c + kDx[k];
+        if (y < 0 || y >= H || x < 0 || x >= W) continue;
+        int n = y * W + x;
+        if (obst[n] == 0.0f) continue;
+        int upd = (!m->open[n] && !m->closed[n]) || (m->open[n] && m->g[n] > g2);
+        if (upd) { m->g[n] = g2; m->open[n] = 1; m->parent[n] = ind; }
+    }
 }
 
 /*
@@ -288,10 +296,10 @@ static void spec_expand(spec_map_t *m, const float *cost, const float *obst, int
 int nastar_oracle_forward_spec(const float *cost, const float *start, const float *goal,
                                const float *obst, int B, int H, int W, float g_ratio,
                                float one_minus_g_ratio, int T, int no_early_exit, float *hist, int64_t *paths,
-                               int32_t *t_solve, int32_t *n_steps, int32_t *trace)
+                               int32_t *t_solve, int32_t *n_steps, int32_t *trace, int mech)
 {
-    if (B <= 0 || H <= 0 || W <= 0 || T <= 0) return NASTAR_ORACLE_EINVAL;
-    const int N = H * W;
+    if (B <= 0 || H <= 0 || W <= 0 || T <= 0 || !mech_ok(mech)) return NASTAR_ORACLE_EINVAL;
+    const int N = H * W, nm = num_moves(mech);
 #pragma omp parallel for schedule(dynamic, 1)
     for (int b = 0; b < B; ++b) {
         spec_map_t m;
@@ -303,7 +311,7 @@ int nastar_oracle_forward_spec(const float *cost, const float *start, const floa
         const float *cb = cost + (size_t)b * N, *ob = obst + (size_t)b * N;
         const int gi = argmax_first(goal + (size_t)b * N, N);
         const int si = argmax_first(start + (size_t)b * N, N);
-        heuristic_plus_cost(cb, H, W, gi, m.h);
+        heuristic_plus_cost(cb, H, W, gi, mech, m.h);
         for (int i = 0; i < N; ++i) m.parent[i] = gi;
         m.open[si] = 1;
         int ts = -1, steps = 0;
@@ -314,7 +322,7 @@ int nastar_oracle_forward_spec(const float *cost, const float *start, const floa
             steps = t + 1;
             m.closed[ind] = 1;
             if (ind != gi) m.open[ind] = 0;       /* the goal, once selected, stays open */
-            spec_expand(&m, cb, ob, H, W, ind);
+            spec_expand(&m, cb, ob, H, W, nm, ind);
             if (ind == gi && ts < 0) ts = t;
             if (ind == gi && !no_early_exit) break;   /* no_early_exit: exactly T steps, like the batch loop */
         }
@@ -345,15 +353,15 @@ int nastar_oracle_forward_spec(const float *cost, const float *start, const floa
  *   dL/dcost[p] = sum_t  -(1-g_ratio)/sqrt_w * y_t[p] * ( Gh[p] - <Gh, y_t> )
  * with y_t = softmax over the open set of -f/sqrt_w and Gh = G with the goal cell zeroed
  * when the map was solved before step T_batch-1 (clamp blocks the gradient there,
- * differentiable_astar.py:222-223).  Accumulation in double.
+ * differentiable_astar.py:222-223).  Accumulation and output in double: the caller rounds once.
  */
 int nastar_oracle_backward(const float *cost, const float *start, const float *goal,
                            const float *obst, const float *grad_hist, int B, int H, int W,
                            float g_ratio, float one_minus_g_ratio, float sqrt_w, int T_batch,
-                           float *grad_cost)
+                           double *grad_cost, int mech)
 {
-    if (B <= 0 || H <= 0 || W <= 0 || T_batch <= 0) return NASTAR_ORACLE_EINVAL;
-    const int N = H * W;
+    if (B <= 0 || H <= 0 || W <= 0 || T_batch <= 0 || !mech_ok(mech)) return NASTAR_ORACLE_EINVAL;
+    const int N = H * W, nm = num_moves(mech);
 #pragma omp parallel for schedule(dynamic, 1)
     for (int b = 0; b < B; ++b) {
         spec_map_t m;
@@ -370,7 +378,7 @@ int nastar_oracle_backward(const float *cost, const float *start, const float *g
         const float *G = grad_hist + (size_t)b * N;
         const int gi = argmax_first(goal + (size_t)b * N, N);
         const int si = argmax_first(start + (size_t)b * N, N);
-        heuristic_plus_cost(cb, H, W, gi, m.h);
+        heuristic_plus_cost(cb, H, W, gi, mech, m.h);
         m.open[si] = 1;
         int blocked_goal = 0;
         for (int t = 0; t < T_batch; ++t) {
@@ -400,14 +408,14 @@ int nastar_oracle_backward(const float *cost, const float *start, const float *g
             if (m.closed[ind]) blocked_goal = 1;   /* hist+sel == 2 before the clamp */
             m.closed[ind] = 1;
             if (ind != gi) m.open[ind] = 0;
-            spec_expand(&m, cb, ob, H, W, ind);
+            spec_expand(&m, cb, ob, H, W, nm, ind);
         }
         const double Gg = blocked_goal ? 0.0 : (double)G[gi];
         const double coef = -(double)one_minus_g_ratio / (double)sqrt_w;
-        float *out = grad_cost + (size_t)b * N;
+        double *out = grad_cost + (size_t)b * N;
         for (int i = 0; i < N; ++i) {
             double Gi = (i == gi) ? Gg : (double)G[i];
-            out[i] = (float)(coef * (acc_y[i] * Gi - acc_yd[i] - acc_yg[i] * Gg));
+            out[i] = coef * (acc_y[i] * Gi - acc_yd[i] - acc_yg[i] * Gg);
         }
         free(m.g); free(m.h); free(m.open); free(m.closed); free(m.parent);
         free(acc_y); free(acc_yd); free(acc_yg); free(y);

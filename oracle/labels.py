@@ -14,11 +14,14 @@ import subprocess
 
 import numpy as np
 
+from .oracle import mechanism_code
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, "labels_oracle.c")
 _LIB_PATH = os.path.join(_HERE, "liblabels_oracle.so")
 # same compiler and flags as oracle/Makefile (the image's default CC lacks libgomp.spec)
-_CC = ["/usr/bin/gcc", "-O2", "-fPIC", "-fopenmp", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-std=c11"]
+_CC = ["/usr/bin/gcc", "-O2", "-fPIC", "-fopenmp", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-std=c11",
+       "-I" + os.path.join(os.path.dirname(_HERE), "include")]
 _lib = None
 
 # build output, git-ignored like the rest of oracle/_ref: the generator's modules, byte for byte, imported as the
@@ -57,7 +60,7 @@ def _load():
         lib.nastar_oracle_opt_labels.argtypes = [ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int32),
                                                  ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                  ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_uint8),
-                                                 ctypes.POINTER(ctypes.c_int8)]
+                                                 ctypes.POINTER(ctypes.c_int8), ctypes.c_int]
         lib.nastar_oracle_opt_labels.restype = ctypes.c_int
         _lib = lib
     return _lib
@@ -67,9 +70,11 @@ def _p(a, ty):
     return a.ctypes.data_as(ctypes.POINTER(ty))
 
 
-def opt_labels(maps, goal_idx):
+def opt_labels(maps, goal_idx, mechanism="moore"):
     """Labels of the planning-datasets generator for maps [B,H,W] or [B,1,H,W] (passable iff != 0) and flat goal
-    indices [B]: (dists float32 [B,1,H,W], act_mask uint8 [B,1,H,W], action int8 [B,1,H,W]), see labels_oracle.c."""
+    indices [B]: (dists float32 [B,1,H,W], act_mask uint8 [B,1,H,W], action int8 [B,1,H,W]), see labels_oracle.c.
+    mechanism "moore" has 8 actions, "news" the 4 actions N, E, W, S."""
+    mech = mechanism_code(mechanism)
     lib = _load()
     m = np.asarray(maps, dtype=np.float32)
     if m.ndim == 4:
@@ -81,7 +86,7 @@ def opt_labels(maps, goal_idx):
     mask = np.empty((B, 1, H, W), np.uint8)
     action = np.empty((B, 1, H, W), np.int8)
     rc = lib.nastar_oracle_opt_labels(_p(m, ctypes.c_float), _p(g, ctypes.c_int32), B, H, W, _p(dists, ctypes.c_float),
-                                      _p(mask, ctypes.c_uint8), _p(action, ctypes.c_int8))
+                                      _p(mask, ctypes.c_uint8), _p(action, ctypes.c_int8), mech)
     if rc != 0:
         raise RuntimeError(f"labels oracle returned {rc}")
     return dists, mask, action

@@ -19,6 +19,14 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "libastar_oracle.so")
 _lib = None
+MECHANISMS = {"moore": 0, "news": 1}   # NASTAR_MECH_MOORE / NASTAR_MECH_NEWS (include/nastar_b200.h)
+
+
+def mechanism_code(mechanism: str) -> int:
+    """The NASTAR_MECH_* value of "moore" or "news"; anything else is a ValueError."""
+    if mechanism not in MECHANISMS:
+        raise ValueError(f"mechanism must be one of {sorted(MECHANISMS)} (got {mechanism!r})")
+    return MECHANISMS[mechanism]
 
 
 def build(force: bool = False) -> str:
@@ -39,14 +47,15 @@ def _load():
         lp = ctypes.POINTER(ctypes.c_int64)
         lib.nastar_oracle_forward_literal.argtypes = [fp, fp, fp, fp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                       ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int,
-                                                      fp, lp, ip, ip, ip]
+                                                      fp, lp, ip, ip, ip, ctypes.c_int]
         lib.nastar_oracle_forward_literal.restype = ctypes.c_int
         lib.nastar_oracle_forward_spec.argtypes = [fp, fp, fp, fp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                    ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_int,
-                                                   fp, lp, ip, ip, ip]
+                                                   fp, lp, ip, ip, ip, ctypes.c_int]
         lib.nastar_oracle_forward_spec.restype = ctypes.c_int
         lib.nastar_oracle_backward.argtypes = [fp, fp, fp, fp, fp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                               ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int, fp]
+                                               ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int,
+                                               ctypes.POINTER(ctypes.c_double), ctypes.c_int]
         lib.nastar_oracle_backward.restype = ctypes.c_int
         lib.nastar_oracle_num_threads.restype = ctypes.c_int
         lib.nastar_oracle_set_threads.argtypes = [ctypes.c_int]
@@ -96,7 +105,10 @@ def check_steps(T: int) -> int:
 
 
 def forward(cost, start, goal, obst, g_ratio=0.5, Tmax=1.0, training=False, mode="spec",
-            want_trace=False, T=None, no_early_exit=False) -> OracleOutput:
+            want_trace=False, T=None, no_early_exit=False, mechanism="moore") -> OracleOutput:
+    """The search of DifferentiableAstar(mechanism=mechanism): "moore" (8 neighbours, Chebyshev heuristic) or "news"
+    (N, E, W, S, Manhattan heuristic), in the LITERAL or SPEC form of astar_oracle.c."""
+    mech = mechanism_code(mechanism)
     lib = _load()
     c, s, g, o = _planes(cost), _planes(start), _planes(goal), _planes(obst)
     B, H, W = c.shape
@@ -113,14 +125,14 @@ def forward(cost, start, goal, obst, g_ratio=0.5, Tmax=1.0, training=False, mode
         rc = lib.nastar_oracle_forward_literal(_p(c, ctypes.c_float), _p(s, ctypes.c_float), _p(g, ctypes.c_float),
                                                _p(o, ctypes.c_float), B, H, W, gr, omg, sq, T,
                                                _p(hist, ctypes.c_float), _p(paths, ctypes.c_int64),
-                                               _p(ts, ctypes.c_int32), tp, ctypes.byref(tb))
+                                               _p(ts, ctypes.c_int32), tp, ctypes.byref(tb), mech)
         T_batch = int(tb.value)
         ns[:] = T_batch
     elif mode == "spec":
         rc = lib.nastar_oracle_forward_spec(_p(c, ctypes.c_float), _p(s, ctypes.c_float), _p(g, ctypes.c_float),
                                             _p(o, ctypes.c_float), B, H, W, gr, omg, T, int(bool(no_early_exit)),
                                             _p(hist, ctypes.c_float), _p(paths, ctypes.c_int64),
-                                            _p(ts, ctypes.c_int32), _p(ns, ctypes.c_int32), tp)
+                                            _p(ts, ctypes.c_int32), _p(ns, ctypes.c_int32), tp, mech)
         T_batch = int(ns.max())
     else:
         raise ValueError(mode)
@@ -129,19 +141,23 @@ def forward(cost, start, goal, obst, g_ratio=0.5, Tmax=1.0, training=False, mode
     return OracleOutput(hist[:, None], paths[:, None], ts, ns, T_batch, trace)
 
 
-def backward(cost, start, goal, obst, grad_hist, T_batch: int, g_ratio=0.5) -> np.ndarray:
+def backward(cost, start, goal, obst, grad_hist, T_batch: int, g_ratio=0.5, dtype=np.float32,
+             mechanism="moore") -> np.ndarray:
+    """Closed-form dL/dcost [B,1,H,W] for dL/dhistories = grad_hist.  The sums run in double; dtype=np.float64 returns
+    them unrounded, np.float32 rounds each once."""
+    mech = mechanism_code(mechanism)
     lib = _load()
     c, s, g, o, gh = _planes(cost), _planes(start), _planes(goal), _planes(obst), _planes(grad_hist)
     B, H, W = c.shape
     gr, omg, sq = scalars(g_ratio, W)
     T_batch = check_steps(T_batch)
-    out = np.zeros((B, H, W), np.float32)
+    out = np.zeros((B, H, W), np.float64)
     rc = lib.nastar_oracle_backward(_p(c, ctypes.c_float), _p(s, ctypes.c_float), _p(g, ctypes.c_float),
                                     _p(o, ctypes.c_float), _p(gh, ctypes.c_float), B, H, W, gr, omg, sq,
-                                    T_batch, _p(out, ctypes.c_float))
+                                    T_batch, _p(out, ctypes.c_double), mech)
     if rc != 0:
         raise RuntimeError(f"oracle returned {rc}")
-    return out[:, None]
+    return out[:, None].astype(dtype)
 
 
 def set_threads(n: int) -> None:

@@ -10,11 +10,14 @@ import subprocess
 
 import numpy as np
 
+from .oracle import mechanism_code
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_HERE, "wlabels_oracle.c")
 _LIB_PATH = os.path.join(_HERE, "libwlabels_oracle.so")
 # the flags of oracle/labels.py: no FMA contraction, so every float add of the fold is rounded once
-_CC = ["/usr/bin/gcc", "-O2", "-fPIC", "-fopenmp", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-std=c11"]
+_CC = ["/usr/bin/gcc", "-O2", "-fPIC", "-fopenmp", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra", "-std=c11",
+       "-I" + os.path.join(os.path.dirname(_HERE), "include")]
 _lib = None
 
 
@@ -30,7 +33,8 @@ def _load():
     if _lib is None:
         build()
         lib = ctypes.CDLL(_LIB_PATH)
-        lib.nastar_oracle_weighted_labels.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 7
+        lib.nastar_oracle_weighted_labels.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 7 + [
+            ctypes.c_int]
         lib.nastar_oracle_weighted_labels.restype = ctypes.c_int
         _lib = lib
     return _lib
@@ -43,10 +47,12 @@ def _maps(x):
     return np.ascontiguousarray(a)
 
 
-def weighted_labels(cost, goal_idx, passable=None, start_idx=None):
+def weighted_labels(cost, goal_idx, passable=None, start_idx=None, mechanism="moore"):
     """Labels of cost maps [B,H,W] or [B,1,H,W] with flat goal (and optional start) indices [B], passable iff != 0
-    (None: every cell).  Returns a dict of dists f32, hops i32, act_mask u8, action i8 (each [B,1,H,W]) and status
-    i32 [B]; with starts also path_maps f32 [B,1,H,W] and path_costs f32 [B].  See wlabels_oracle.c."""
+    (None: every cell), with the 8 moves of "moore" or the 4 moves N, E, W, S of "news".  Returns a dict of dists f32,
+    hops i32, act_mask u8, action i8 (each [B,1,H,W]) and status i32 [B]; with starts also path_maps f32 [B,1,H,W]
+    and path_costs f32 [B].  See wlabels_oracle.c."""
+    mech = mechanism_code(mechanism)
     lib = _load()
     c = _maps(cost)
     B, H, W = c.shape
@@ -67,7 +73,7 @@ def weighted_labels(cost, goal_idx, passable=None, start_idx=None):
 
     rc = lib.nastar_oracle_weighted_labels(ptr(c), ptr(p), ptr(g), ptr(s), B, H, W, ptr(out["dists"]),
                                            ptr(out["hops"]), ptr(out["act_mask"]), ptr(out["action"]),
-                                           ptr(out.get("path_maps")), ptr(out.get("path_costs")), ptr(out["status"]))
+                                           ptr(out.get("path_maps")), ptr(out.get("path_costs")), ptr(out["status"]), mech)
     if rc != 0:
         raise RuntimeError(f"weighted labels oracle returned {rc}")
     return out

@@ -1,7 +1,8 @@
 /*
  * wlabels_oracle.c -- CPU oracle of the vertex-weighted shortest-path labels (TEST INFRASTRUCTURE ONLY; the product
  * package never links it).  Checks nastar_b200_weighted_labels (neural-astar_b200/csrc/nastar_wlabels.cuh), but is
- * written from the semantics (DESIGN.md §11), not from the kernel:
+ * written from the semantics (DESIGN.md §11), not from the kernel.  Moves are the 8 actions of Moore or the first 4
+ * (N, E, W, S) of NEWS:
  *   cost-to-go  Dijkstra from the goal with a binary heap of (D, cell), lazy deletion.  Settling u relaxes every
  *               in-grid passable neighbour v != goal (the move v->u charges c[u]): fl(D[u] + c[u]).  Compiled with
  *               -ffp-contract=off on an SSE target, every float add is rounded once.  The fold x -> fl(x + c) is
@@ -16,7 +17,9 @@
 #include <stdlib.h>
 #include <string.h>
 
-static const int kDy[8] = {-1, 0, 0, +1, -1, -1, +1, +1};   /* N, E, W, S, NE, NW, SE, SW */
+#include "nastar_b200.h"
+
+static const int kDy[8] = {-1, 0, 0, +1, -1, -1, +1, +1};   /* N, E, W, S, NE, NW, SE, SW; NEWS takes the first 4 */
 static const int kDx[8] = {0, +1, -1, 0, +1, -1, +1, -1};
 
 typedef struct {
@@ -56,7 +59,7 @@ typedef struct {
     const uint8_t *pas;
     const float *D;
     const int32_t *hop;
-    int H, W, goal;
+    int H, W, goal, nmoves;
 } Map;
 
 /* the move v -> t is allowed: t on the grid and passable or the goal (v's own passability is the caller's) */
@@ -70,14 +73,15 @@ static int target(const Map *m, int v, int a) {
 static unsigned policy(const Map *m, int v) {
     if (v == m->goal || m->hop[v] < 0) return 0;
     unsigned mask = 0;
-    for (int a = 0; a < 8; ++a) {
+    for (int a = 0; a < m->nmoves; ++a) {
         const int t = target(m, v, a);
         if (t >= 0 && m->hop[t] == m->hop[v] - 1 && m->D[t] + m->c[t] == m->D[v]) mask |= 1u << a;
     }
     return mask;
 }
 
-static int one_map(const float *c, const float *passable, int goal, const int32_t *start, int H, int W, float *D,
+static int one_map(const float *c, const float *passable, int goal, const int32_t *start, int H, int W, int nmoves,
+                   float *D,
                    uint8_t *pas, Item *heap, int32_t *queue, float *dists, int32_t *hop, uint8_t *act_mask,
                    int8_t *action, float *path, float *path_cost) {
     const int N = H * W;
@@ -92,7 +96,7 @@ static int one_map(const float *c, const float *passable, int goal, const int32_
         D[i] = INFINITY;
         hop[i] = -1;
     }
-    Map m = {c, pas, D, hop, H, W, goal};
+    Map m = {c, pas, D, hop, H, W, goal, nmoves};
     if (status == 0) {
         int n = 0;
         D[goal] = 0.0f;
@@ -103,7 +107,7 @@ static int one_map(const float *c, const float *passable, int goal, const int32_
             if (it.d != D[u]) continue;   /* stale entry */
             const float via = D[u] + c[u];
             const int uy = u / W, ux = u % W;
-            for (int a = 0; a < 8; ++a) {   /* v = u - move(a): the cells whose move a enters u */
+            for (int a = 0; a < nmoves; ++a) {   /* v = u - move(a): the cells whose move a enters u */
                 const int vy = uy - kDy[a], vx = ux - kDx[a];
                 if (vy < 0 || vy >= H || vx < 0 || vx >= W) continue;
                 const int v = vy * W + vx;
@@ -121,7 +125,7 @@ static int one_map(const float *c, const float *passable, int goal, const int32_
             const int u = queue[head++];
             const float via = D[u] + c[u];
             const int uy = u / W, ux = u % W;
-            for (int a = 0; a < 8; ++a) {
+            for (int a = 0; a < nmoves; ++a) {
                 const int vy = uy - kDy[a], vx = ux - kDx[a];
                 if (vy < 0 || vy >= H || vx < 0 || vx >= W) continue;
                 const int v = vy * W + vx;
@@ -160,15 +164,18 @@ static int one_map(const float *c, const float *passable, int goal, const int32_
 }
 
 /* cost, passable (or NULL): [B][H*W] fp32; goal_idx, start_idx (or NULL): [B]; outputs [B][H*W] (path_maps) and
- * [B] (path_costs, status).  Returns 0, or 1 on bad arguments / allocation failure. */
+ * [B] (path_costs, status); mech: NASTAR_MECH_MOORE or NASTAR_MECH_NEWS.  Returns 0, or 1 on bad arguments /
+ * allocation failure. */
 int nastar_oracle_weighted_labels(const float *cost, const float *passable, const int32_t *goal_idx,
                                   const int32_t *start_idx, int B, int H, int W, float *dists, int32_t *hops,
                                   uint8_t *act_mask, int8_t *action, float *path_maps, float *path_costs,
-                                  int32_t *status) {
+                                  int32_t *status, int mech) {
     if (!cost || !goal_idx || !dists || !hops || !act_mask || !action || !status || B <= 0 || H <= 0 || W <= 0)
         return 1;
     if (start_idx && (!path_maps || !path_costs)) return 1;
+    if (mech != NASTAR_MECH_MOORE && mech != NASTAR_MECH_NEWS) return 1;
     const int64_t N = (int64_t)H * W;
+    const int nmoves = mech == NASTAR_MECH_NEWS ? 4 : 8;
     int fail = 0;
 #pragma omp parallel reduction(| : fail)
     {
@@ -183,7 +190,7 @@ int nastar_oracle_weighted_labels(const float *cost, const float *passable, cons
                 continue;
             }
             status[b] = one_map(cost + b * N, passable ? passable + b * N : NULL, goal_idx[b],
-                                start_idx ? start_idx + b : NULL, H, W, D, pas, heap, queue, dists + b * N,
+                                start_idx ? start_idx + b : NULL, H, W, nmoves, D, pas, heap, queue, dists + b * N,
                                 hops + b * N, act_mask + b * N, action + b * N, start_idx ? path_maps + b * N : NULL,
                                 start_idx ? path_costs + b : NULL);
         }

@@ -2,7 +2,7 @@
 costs w and on the perturbed costs w' = fl(w + fl(lambda * g)), the latter formed in float32 NumPy with two rounded
 operations, and dL/dw = (y(w') - y(w)) / lambda.
 
-Moore searches go through oracle/oracle.py, NEWS searches through tests/news_search_oracle.py.  Per-map early exit
+Both mechanisms' searches go through oracle/oracle.py.  Per-map early exit
 (the spec oracles) or, for a batch-coupled search, the reference's batch-synchronous loop (the literal oracles) with the
 step bound T as its cap; each search gets its own T_batch."""
 from __future__ import annotations
@@ -11,8 +11,7 @@ from typing import NamedTuple
 
 import numpy as np
 
-import news_search_oracle
-from oracle import oracle as moore_oracle
+from oracle import oracle
 
 F32 = np.float32
 
@@ -34,8 +33,8 @@ def perturbed_costs(cost, grad_hist, lam: float) -> np.ndarray:
 def search(cost, start, goal, obst, g_ratio: float, T: int, mechanism: str = "moore",
            coupled: bool = False) -> np.ndarray:
     """The histories y(cost) of the search that the planner runs: per-map early exit, or batch-coupled."""
-    mod = news_search_oracle if mechanism == "news" else moore_oracle
-    out = mod.forward(cost, start, goal, obst, g_ratio, T=T, mode="literal" if coupled else "spec")
+    out = oracle.forward(cost, start, goal, obst, g_ratio, T=T, mode="literal" if coupled else "spec",
+                         mechanism=mechanism)
     return np.asarray(out.histories, F32)
 
 

@@ -8,7 +8,7 @@ planning-datasets generator's NorthEastWestSouth pieces, exactly as a user of th
     astar.neighbor_filter.data = NorthEastWestSouth.get_neighbor_filter()     (mechanism.py:113-121)
     astar.get_heuristic        = NorthEastWestSouth.get_heuristic             (mechanism.py:123-131)
 mechanism.py is loaded by file path (it imports only numpy and torch).  Every stored output comes from the reference;
-the CPU NEWS label oracle (tests/news_labels_oracle.py) is only used to draw starts that can reach the goal over
+the CPU label oracle in NEWS mode (oracle/labels.py) is only used to draw starts that can reach the goal over
 4-connected moves (4-connectivity splits regions that Moore joins, and an unreachable goal makes the reference raise
 IndexError).  Files, under tests/golden/news/ (all square: the generator's heuristic reads size = shape[-1]):
   news_mazes032_vanilla   mazes_032 test split (100 maps), shipped goals, VanillaAstar: engine 1
@@ -40,7 +40,7 @@ import torch  # noqa: E402
 from neural_astar.planner import VanillaAstar  # noqa: E402  (the reference's)
 from neural_astar.planner.differentiable_astar import DifferentiableAstar  # noqa: E402
 
-import news_labels_oracle  # noqa: E402
+from oracle import labels as label_oracle  # noqa: E402
 
 # a directory of their own: tests/golden/*.npz are Moore search vectors that golden_util.all_names() hands to every
 # Moore parity test
@@ -80,7 +80,7 @@ def run_news(cost, start, goal, obst, g_ratio=0.5, Tmax=1.0, training=False, gra
 def news_starts(maps, goal_idx, seed):
     """One start per map, uniform over the cells that reach the goal over 4-connected moves (goal excluded)."""
     rng = np.random.RandomState(seed)
-    dists = news_labels_oracle.opt_labels(maps, goal_idx)[0]
+    dists = label_oracle.opt_labels(maps, goal_idx, mechanism="news")[0]
     B, _, H, W = maps.shape
     start = np.zeros((B, 1, H, W), np.float32)
     for b in range(B):

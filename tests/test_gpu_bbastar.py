@@ -21,8 +21,8 @@ def _native():
 
 def _problem(seed, B, H, W, far=None):
     """Random maps, 90 % passable (goals stay reachable, which the coupled oracle's literal loop needs), one start and
-    one goal per map, learned-looking costs in [0.1, 1.1).  `far` bounds |start - goal| per axis (keeps the NumPy NEWS
-    oracle quick on large maps)."""
+    one goal per map, learned-looking costs in [0.1, 1.1).  `far` bounds |start - goal| per axis (keeps the CPU oracle
+    quick on large maps)."""
     rng = np.random.RandomState(seed)
     maps = (rng.rand(B, 1, H, W) > 0.1).astype(F32)
     start = np.zeros_like(maps)

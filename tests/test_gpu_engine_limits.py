@@ -1,5 +1,5 @@
-"""The search engines at the edges of the shapes they accept, against the SPEC oracle (oracle/astar_oracle.c, and
-tests/news_search_oracle.py for NEWS), and the shapes just outside them.
+"""The search engines at the edges of the shapes they accept, against the SPEC oracle (oracle/astar_oracle.c, either
+mechanism), and the shapes just outside them.
 
 The edges are asked of the library (tests/test_engine_limits_cpu.py, which checks them against the layouts), so these
 shapes follow a layout change:
@@ -31,13 +31,6 @@ def native():
 
     _native.lib()
     return _native
-
-
-@pytest.fixture(scope="module")
-def news_oracle():
-    import news_search_oracle
-
-    return news_search_oracle
 
 
 def _dev(x):
@@ -94,8 +87,7 @@ def _near_problem(rng, B, H, W, p_obst, dist):
     return obst, start, goal
 
 
-def _search_exact(native, oracle, planes, T, launches, *, aliased=False, g_ratio=0.5, mechanism="moore",
-                  news_oracle=None, label=""):
+def _search_exact(native, oracle, planes, T, launches, *, aliased=False, g_ratio=0.5, mechanism="moore", label=""):
     """native.forward against the SPEC oracle, bit for bit with the per-map counts, and its launch count.  `aliased`
     passes one device tensor as cost and obstacles (what sends a binary map to engine 5).  Returns the device outputs
     (histories, t_solve, n_steps) and the oracle's output."""
@@ -110,10 +102,7 @@ def _search_exact(native, oracle, planes, T, launches, *, aliased=False, g_ratio
         *dev, g_ratio, T, want_counts=True, mechanism=mechanism))
     assert native.launch_count() - before == launches
     t0 = time.perf_counter()
-    if mechanism == "news":
-        ref = news_oracle.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="spec", T=T)
-    else:
-        ref = oracle.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="spec", T=T)
+    ref = oracle.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="spec", T=T, mechanism=mechanism)
     print(f"{label} {mechanism} T={T}: gpu {t_gpu:.3f} s, oracle {time.perf_counter() - t0:.2f} s, "
           f"t_solve {ref.t_solve.tolist()[:4]}")
     np.testing.assert_array_equal(ts.cpu().numpy(), ref.t_solve)
@@ -224,7 +213,7 @@ def _learned_problem(rng, H, W, dist):
 
 @pytest.mark.parametrize("mechanism", ["moore", "news"])
 @pytest.mark.parametrize("case", list(ENGINE3_SHAPES))
-def test_engine3_at_its_edges_vs_oracle(native, oracle, news_oracle, case, mechanism):
+def test_engine3_at_its_edges_vs_oracle(native, oracle, case, mechanism):
     """Learned-style costs (uniform(0.1, 1), 10 % obstacles) on engine 3's largest shapes.  Evaluation (T = W * W,
     start and goal a short way apart, or at 11 621 x 32 far apart with the bound capping it) bit-exact; training with
     a small Tmax (T = 256) with start and goal 400 cells apart, capped, bit-exact, and its backward within TOL of the
@@ -237,8 +226,7 @@ def test_engine3_at_its_edges_vs_oracle(native, oracle, news_oracle, case, mecha
     far = W < 64
     dist = 0 if far else (3000 if mechanism == "moore" else 500) if W > 40000 else 20
     planes = _learned_problem(rng, H, W, dist)
-    _, _, ref = _search_exact(native, oracle, planes, W * W, 1, mechanism=mechanism, news_oracle=news_oracle,
-                              label=f"{H}x{W} eval")
+    _, _, ref = _search_exact(native, oracle, planes, W * W, 1, mechanism=mechanism, label=f"{H}x{W} eval")
     assert (ref.t_solve == -1).all() if far else (ref.t_solve >= 0).all()   # capped by W * W = 1024, or solved
 
     astar = DifferentiableAstar(Tmax=0.25 if far else 256.5 / (W * W), mechanism=mechanism).train()
@@ -248,7 +236,7 @@ def test_engine3_at_its_edges_vs_oracle(native, oracle, news_oracle, case, mecha
     # exp(-f / sqrt(W)) stay representable in fp32, as in the reference
     planes = _learned_problem(rng, H, W, 400)
     (hist, _, ts, ns), dev, ref = _search_exact(native, oracle, planes, T, 1, mechanism=mechanism,
-                                                news_oracle=news_oracle, label=f"{H}x{W} train")
+                                                label=f"{H}x{W} train")
     assert (ref.t_solve == -1).all()
     G = rng.randn(*planes[0].shape).astype(np.float32)
     Tb = native.batch_steps(ts, ns, T)
@@ -257,7 +245,7 @@ def test_engine3_at_its_edges_vs_oracle(native, oracle, news_oracle, case, mecha
     gc, t_gpu = _clock(lambda: native.backward(*dev, _dev(G), Tb, ts, 0.5, mechanism=mechanism))
     assert native.launch_count() - before == 1
     t0 = time.perf_counter()
-    want = (news_oracle if mechanism == "news" else oracle).backward(*planes, G, T)
+    want = oracle.backward(*planes, G, T, mechanism=mechanism)
     print(f"{H}x{W} backward {mechanism}: gpu {t_gpu:.3f} s, oracle {time.perf_counter() - t0:.2f} s")
     gc = gc.cpu().numpy()
     assert np.isfinite(gc).all()
@@ -329,7 +317,7 @@ def test_open_strip_rule_vs_oracle(native, oracle):
 
 
 @pytest.mark.parametrize("mechanism", ["moore", "news"])
-def test_open_strip_at_the_widest_bound(native, oracle, news_oracle, mechanism):
+def test_open_strip_at_the_widest_bound(native, oracle, mechanism):
     """1 x 46 340: the evaluation bound W * W = 2 147 395 600 just fits.  The search runs W steps and the answer is the
     strip rule.  In training (T = 2 147 steps) toward a goal at x = 3 000 it is capped, bit-exact against the oracle,
     and its gradient, zero in closed form on one row, is zero to within TOL of one step's scale."""
@@ -353,12 +341,11 @@ def test_open_strip_at_the_widest_bound(native, oracle, news_oracle, mechanism):
     goal = np.zeros_like(plane)
     goal[0, 0, 0, 3000] = 1   # beyond the T steps, near enough that exp(-f / sqrt(W)) stays an fp32 number
     planes = (cost, start, goal, plane)
-    (_, _, ts, ns), devp, ref = _search_exact(native, oracle, planes, T, 1, mechanism=mechanism,
-                                              news_oracle=news_oracle, label="strip train")
+    (_, _, ts, ns), devp, ref = _search_exact(native, oracle, planes, T, 1, mechanism=mechanism, label="strip train")
     assert ref.t_solve.tolist() == [-1]
     G = np.random.RandomState(4).randn(*plane.shape).astype(np.float32)
     gc = native.backward(*devp, _dev(G), native.batch_steps(ts, ns, T), ts, 0.5, mechanism=mechanism).cpu().numpy()
-    want = (news_oracle if mechanism == "news" else oracle).backward(*planes, G, T)
+    want = oracle.backward(*planes, G, T, mechanism=mechanism)
     # one row: the one open cell takes the whole softmax at every step, so each step's term y * (G - <G, y>) is zero
     # and so is the gradient; the engine's running sums leave rounding residue, bounded against one step's scale
     assert not want.any()

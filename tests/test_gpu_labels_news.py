@@ -11,7 +11,7 @@ import pytest
 import torch
 
 import labels_golden
-import news_labels_oracle
+from oracle import labels as label_oracle
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -40,7 +40,7 @@ def _kernel(maps, goal_idx, dev, mechanism="news"):
 
 def _assert_matches_oracle(maps, goal_idx, dev):
     d, m, a = _kernel(maps, goal_idx, dev)
-    od, om, oa = news_labels_oracle.opt_labels(maps, goal_idx)
+    od, om, oa = label_oracle.opt_labels(maps, goal_idx, mechanism="news")
     assert np.array_equal(d, od), f"distances differ on {int((d != od).sum())} cells"
     assert np.array_equal(m, om), f"max-set masks differ on {int((m != om).sum())} cells"
     assert np.array_equal(a, oa), "first-max actions differ"

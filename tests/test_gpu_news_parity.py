@@ -1,10 +1,9 @@
 """The 4-connected (NEWS) search checked like the 8-connected one: the Moore checks of test_gpu_forward_parity.py,
-test_gpu_backward_parity.py and test_gpu_engine_schedules.py with mechanism="news", against the NumPy NEWS oracle
-(tests/news_search_oracle.py; its LITERAL form equals the reference on tests/golden/news/, test_news_oracle_cpu.py).
+test_gpu_backward_parity.py and test_gpu_engine_schedules.py with mechanism="news", against the C oracle's NEWS
+mode (oracle/astar_oracle.c; its LITERAL form equals the reference on tests/golden/news/, test_news_oracle_cpu.py).
 
 Every shape asserts the engine it is meant to reach (nastar_b200_engine_for): 1 (32-wide), 4 (64-wide), 2 (generic,
-state in shared memory) and 3 (generic, HBM workspace).  Engine 5 is Moore-only.  The oracle is per-step Python, so
-batches are small; the matrix of g_ratio, flags, shapes and edge cases is not.
+state in shared memory) and 3 (generic, HBM workspace).  Engine 5 is Moore-only.
 """
 import os
 import subprocess
@@ -14,8 +13,9 @@ import numpy as np
 import pytest
 import torch
 
-import news_search_oracle as nso
 from golden_util import Golden
+from oracle import oracle
+from search_steps import MOVES, SpecMachine
 from test_gpu_backward_parity import _assert_grad
 from test_news_oracle_cpu import problems
 
@@ -59,8 +59,8 @@ def _fwd_vs_spec(native, planes, T, g_ratio=0.5, dev=None, trace=True, no_early_
             dev[3] = dev[0]
     hist, paths, ts, ns, tr, (ncl, plen) = native.forward(*dev, g_ratio, T, trace, no_early_exit, want_counts=True,
                                                           mechanism="news", **kw)
-    ref = nso.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="spec", want_trace=trace, T=T,
-                      no_early_exit=no_early_exit)
+    ref = oracle.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="spec", want_trace=trace, T=T,
+                         no_early_exit=no_early_exit, mechanism="news")
     what = (cost.shape, g_ratio, T, no_early_exit)
     np.testing.assert_array_equal(_np(ts), ref.t_solve, err_msg=str(what))
     np.testing.assert_array_equal(_np(ns), ref.n_steps, err_msg=str(what))
@@ -79,7 +79,7 @@ def _bwd_vs_oracle(native, planes, dev, ts, ns, T, G, g_ratio=0.5, T_batch=None)
     Tb = native.batch_steps(ts, ns, T) if T_batch is None else torch.full((1,), T_batch, dtype=torch.int32,
                                                                           device="cuda")
     gc = _np(native.backward(*dev, _cu(G), Tb, ts, g_ratio, mechanism="news"))
-    want = nso.backward(cost, start, goal, obst, G, int(Tb.item()), g_ratio=g_ratio)
+    want = oracle.backward(cost, start, goal, obst, G, int(Tb.item()), g_ratio=g_ratio, mechanism="news")
     _assert_grad(gc, want, G, (cost.shape, g_ratio, T, int(Tb.item())))
     return int(Tb.item())
 
@@ -89,13 +89,11 @@ def _max_f_over_sqrt_w(planes, g_ratio, T):
     g of an opened cell is g + cost of a closed one.  Kept below 80 so that exp(-f / sqrt(W)) stays a normal fp32
     number, in the oracle's softmax as in the reference's."""
     cost, start, goal, obst = planes
-    c, H, W = nso._planes(cost)
-    s, g, o = nso._planes(start)[0], nso._planes(goal)[0], nso._planes(obst)[0]
-    gr, omg, sqw = nso._scalars(g_ratio, W)
+    gr, omg, sqw = oracle.scalars(g_ratio, cost.shape[-1])
     worst = 0.0
-    for b in range(c.shape[0]):
-        gi = int(g[b].argmax())
-        m = nso._Spec(c[b], o[b], H, W, int(s[b].argmax()), gi)
+    for b in range(cost.shape[0]):
+        gi = int(goal[b].argmax())
+        m = SpecMachine(cost[b, 0], obst[b, 0], int(start[b].argmax()), gi, "news")
         gmax = 0.0
         for _ in range(T):
             ind = m.select(gr, omg)
@@ -140,7 +138,7 @@ def _edge_problems(rs, kinds, H, W, p_obst=0.15):
         else:
             raise ValueError(kind)
         obst[b, 0, sy, sx] = obst[b, 0, gy, gx] = 1
-        for dy, dx in nso.MOVES:
+        for dy, dx in MOVES["news"]:
             if kind == "walled" and 0 <= sy + dy < H and 0 <= sx + dx < W:
                 obst[b, 0, sy + dy, sx + dx] = 0
             if kind == "enclosed" and 0 <= gy + dy < H and 0 <= gx + dx < W:
@@ -190,7 +188,7 @@ def test_no_early_exit_vs_spec(native, H, W, engine, B):
     rs = np.random.RandomState(H * 3 + W)
     planes = problems(rs, B, H, W, 0.15, True)
     for g_ratio in (0.0, 0.3, 0.5):
-        ts = nso.forward(*planes, g_ratio=g_ratio, mode="spec", T=W * W).t_solve
+        ts = oracle.forward(*planes, g_ratio=g_ratio, mode="spec", T=W * W, mechanism="news").t_solve
         assert (ts > 0).all()
         for T in (int(ts.min()), int(ts.max()) + 40):
             _fwd_vs_spec(native, planes, T, g_ratio, no_early_exit=True)
@@ -234,7 +232,8 @@ def test_coupled_module_vs_literal(native, H, W, engine, B, g_ratio, train):
     cost = cost * np.float32(10.0)
     G = rs.randn(B, 1, H, W).astype(np.float32)
     T = int((0.25 if train else 1.0) * W * W)
-    lit = nso.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="literal", want_trace=True, T=T)
+    lit = oracle.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="literal", want_trace=True, T=T,
+                         mechanism="news")
     astar = DifferentiableAstar(g_ratio=g_ratio, Tmax=0.25, mechanism="news").cuda().train(train)
     c = _cu(cost).requires_grad_(True)
     out = astar(c, _cu(start), _cu(goal), _cu(obst), store_intermediate_results=True)
@@ -244,7 +243,7 @@ def test_coupled_module_vs_literal(native, H, W, engine, B, g_ratio, train):
     sel = torch.stack([f["paths"].reshape(B, -1).argmax(1) for f in out.intermediate_results[:-1]], 1)
     np.testing.assert_array_equal(_np(sel), lit.trace[:, :lit.T_batch])
     (out.histories * _cu(G)).sum().backward()
-    want = nso.backward(cost, start, goal, obst, G, lit.T_batch, g_ratio=g_ratio)
+    want = oracle.backward(cost, start, goal, obst, G, lit.T_batch, g_ratio=g_ratio, mechanism="news")
     _assert_grad(_np(c.grad), want, G, (H, W, g_ratio, train, lit.T_batch))
 
 
@@ -344,7 +343,8 @@ def test_backward_every_engine(native, H, W, engine, B, g_ratio):
                 one = tuple(x[i:i + 1] for x in planes)
                 dev = [_cu(x) for x in one]
                 ts, ns, ref = _fwd_vs_spec(native, one, T, g_ratio, dev=dev, trace=False)
-                lit = nso.forward(*one, g_ratio=g_ratio, mode="literal", T=T) if ref.t_solve[0] != -2 else None
+                lit = (oracle.forward(*one, g_ratio=g_ratio, mode="literal", T=T, mechanism="news")
+                       if ref.t_solve[0] != -2 else None)
                 Tb = _bwd_vs_oracle(native, one, dev, ts, ns, T, G[i:i + 1], g_ratio)
                 if lit is not None:
                     assert lit.T_batch == Tb
@@ -403,13 +403,13 @@ def test_event_based_backward_single_map(native, H, W, engine, g_ratio):
         G = rs.randn(1, 1, H, W).astype(np.float32)
         for T in (W * W, W * W // 8):
             assert _max_f_over_sqrt_w(planes, g_ratio, T) < 80
-            lit = nso.forward(*planes, g_ratio=g_ratio, mode="literal", T=T)
+            lit = oracle.forward(*planes, g_ratio=g_ratio, mode="literal", T=T, mechanism="news")
             dev = [_cu(x) for x in planes]
             hist, paths, ts, ns, _ = native.forward(*dev, g_ratio, T, mechanism="news")
             Tb = native.batch_steps(ts, ns, T)
             assert int(Tb.item()) == lit.T_batch
             gc = _np(native.backward(*dev, _cu(G), Tb, ts, g_ratio, mechanism="news"))
-            want = nso.backward(*planes, G, lit.T_batch, g_ratio=g_ratio)
+            want = oracle.backward(*planes, G, lit.T_batch, g_ratio=g_ratio, mechanism="news")
             _assert_grad(gc, want, G, (H, W, g_ratio, T, trial))
 
 
@@ -562,7 +562,7 @@ def test_pair_launch_with_counts(native, H, W, engine):
                                                           mechanism="news")
     assert tr is None
     for half, cst in ((slice(0, 6), cost), (slice(6, 12), obst)):
-        ref = nso.forward(cst, start, goal, obst, mode="spec", T=W * W)
+        ref = oracle.forward(cst, start, goal, obst, mode="spec", T=W * W, mechanism="news")
         np.testing.assert_array_equal(_np(hist[half]), ref.histories)
         np.testing.assert_array_equal(_np(paths[half]), ref.paths)
         np.testing.assert_array_equal(_np(ts[half]), ref.t_solve)
@@ -587,7 +587,7 @@ def test_neural_astar_fused_forward_equals_encode_then_search(native, H, W):
         cost = na.encode(m, s, g)
         plain = na.astar(cost, s, g, m)
     assert torch.equal(fused.histories, plain.histories) and torch.equal(fused.paths, plain.paths)
-    ref = nso.forward(_np(cost), start, goal, maps, mode="spec")
+    ref = oracle.forward(_np(cost), start, goal, maps, mode="spec", mechanism="news")
     np.testing.assert_array_equal(_np(fused.histories), ref.histories)
     np.testing.assert_array_equal(_np(fused.paths), ref.paths)
 
@@ -597,7 +597,6 @@ _FIRST_USE = r"""
 import sys
 sys.path[:0] = [{root!r}, {pkg!r}, {tests!r}]
 import numpy as np, torch
-import news_search_oracle as nso
 from test_news_oracle_cpu import problems
 from neural_astar import _native
 from oracle import oracle
@@ -611,7 +610,7 @@ for H, W, engine in ((32, 32, 1), (64, 64, 4)):
         with torch.cuda.stream(stream or torch.cuda.default_stream()):
             hist, paths, ts, ns, tr = _native.forward(*dev, 0.5, W * W, True, mechanism=mech)
         torch.cuda.synchronize()
-        ref = (nso if mech == "news" else oracle).forward(*planes, mode="spec", want_trace=True, T=W * W)
+        ref = oracle.forward(*planes, mode="spec", want_trace=True, T=W * W, mechanism=mech)
         for got, want in ((hist, ref.histories), (paths, ref.paths), (ts, ref.t_solve), (tr, ref.trace)):
             assert np.array_equal(got.cpu().numpy(), want), (H, W, mech)
 print("first use ok")

@@ -1,14 +1,14 @@
 """The 4-connected (NEWS) search on the GPU: every engine it runs on (1, 4, 2, 3; engine 5 is Moore-only) against the
-reference's own outputs (tests/golden/news/) and against the NumPy NEWS oracle's SPEC form, the backward, the fused
+reference's own outputs (tests/golden/news/) and against the C oracle's NEWS SPEC form, the backward, the fused
 cost hand-offs, the pair launch, the batch-coupled path, the graphed and pipelined planners, and optimal paths on
 maps labelled with the NEWS mechanism."""
 import numpy as np
 import pytest
 import torch
 
-import news_labels_oracle
-import news_search_oracle as nso
 from golden_util import Golden
+from oracle import labels as label_oracle
+from oracle import oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -35,7 +35,7 @@ def _problems(B, H, W, seed, learned=True, p_obst=0.25):
         while True:
             free = np.flatnonzero(maps[b, 0].reshape(-1))
             gi = int(free[rs.randint(len(free))])
-            d = news_labels_oracle.opt_labels(maps[b:b + 1], np.array([gi]))[0].reshape(-1)
+            d = label_oracle.opt_labels(maps[b:b + 1], np.array([gi]), mechanism="news")[0].reshape(-1)
             cand = np.flatnonzero((d > -(H * W)) & (d < 0))
             if len(cand):
                 break
@@ -120,7 +120,7 @@ def test_random_vs_spec_oracle(H, W, learned):
     obst = c if not learned else _cu(maps)
     hist, paths, ts, ns, trace = _native.forward(c, _cu(start), _cu(goal), obst, 0.5, T, want_trace=True,
                                                  mechanism="news")
-    ref = nso.forward(cost, start, goal, maps, mode="spec", want_trace=True, T=T)
+    ref = oracle.forward(cost, start, goal, maps, mode="spec", want_trace=True, T=T, mechanism="news")
     np.testing.assert_array_equal(hist.cpu().numpy(), ref.histories)
     np.testing.assert_array_equal(paths.cpu().numpy(), ref.paths)
     np.testing.assert_array_equal(ts.cpu().numpy(), ref.t_solve)
@@ -142,10 +142,10 @@ def test_backward_vs_oracle(H, W, engine):
     out = astar(c, _cu(start), _cu(goal), _cu(maps))
     (out.histories * _cu(G)).sum().backward()
     T = int(0.25 * W * W)
-    ref = nso.forward(cost, start, goal, maps, mode="spec", T=T)
+    ref = oracle.forward(cost, start, goal, maps, mode="spec", T=T, mechanism="news")
     np.testing.assert_array_equal(out.histories.detach().cpu().numpy(), ref.histories)
     T_batch = T if (ref.t_solve < 0).any() else int(ref.t_solve.max()) + 1
-    want = nso.backward(cost, start, goal, maps, G, T_batch)
+    want = oracle.backward(cost, start, goal, maps, G, T_batch, mechanism="news")
     assert _relerr(c.grad.cpu().numpy(), want) < 1e-5
 
 
@@ -206,7 +206,7 @@ def test_binary_256_skips_engine_5():
         before = _native.launch_count()
         out = planner(m, s, g)
         assert _native.launch_count() - before == 1
-    ref = nso.forward(maps, start, goal, maps, mode="spec")
+    ref = oracle.forward(maps, start, goal, maps, mode="spec", mechanism="news")
     np.testing.assert_array_equal(out.histories.cpu().numpy(), ref.histories)
     np.testing.assert_array_equal(out.paths.cpu().numpy(), ref.paths)
 

@@ -1,5 +1,5 @@
 """GPU tests of the NEWS (4-connected) vertex-weighted shortest-path kernel (nastar_wlabels.cuh, kNews): bit-exact
-against the NumPy NEWS oracle (tests/news_wlabels_oracle.py) on the label fixtures, on the NEWS goldens' learned costs
+against the C oracle's NEWS mode (oracle/wlabels_oracle.c) on the label fixtures, on the NEWS goldens' learned costs
 and on seeded random cost maps; the Moore case of the new entry point against the old one; NEWS planner paths against
 the NEWS optimum; determinism, launch count and dataset round trips."""
 import ctypes
@@ -12,8 +12,8 @@ import pytest
 import torch
 
 import labels_golden
-import news_wlabels_oracle
 from golden_util import Golden
+from oracle import wlabels
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -48,7 +48,7 @@ def _kernel(cost, goal_idx, dev, passable=None, start_idx=None, mechanism="news"
 
 def _assert_matches_oracle(cost, goal_idx, dev, passable=None, start_idx=None):
     k = _kernel(cost, goal_idx, dev, passable, start_idx)
-    o = news_wlabels_oracle.weighted_labels(cost, goal_idx, passable, start_idx, mechanism="news")
+    o = wlabels.weighted_labels(cost, goal_idx, passable, start_idx, mechanism="news")
     for key in KEYS:
         if key not in o:
             assert k[key] is None

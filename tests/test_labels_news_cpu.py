@@ -1,4 +1,4 @@
-"""CPU tests of the NEWS (4-action) shortest-path labels: the NumPy oracle (tests/news_labels_oracle.py) against the
+"""CPU tests of the NEWS (4-action) shortest-path labels: the C oracle's NEWS mode (oracle/labels_oracle.c) against the
 generator's own dijkstra_dist and extract_policy and against a scipy graph search, 4-action dataset files, the dataset
 tool's file names, and argument checks at the C ABI (no GPU needed)."""
 import ctypes
@@ -11,7 +11,7 @@ import pytest
 import torch
 
 import labels_golden
-import news_labels_oracle
+from oracle import labels as label_oracle
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -21,8 +21,6 @@ MECH_MOORE, MECH_NEWS = 0, 1
 
 
 def _staged():
-    from oracle import labels as label_oracle
-
     return all(os.path.exists(os.path.join(label_oracle.REF_STAGE, f)) for f in label_oracle.REF_FILES)
 
 
@@ -69,10 +67,9 @@ def test_news_oracle_matches_the_generator(case):
     """Distances equal dijkstra_dist(maze, NorthEastWestSouth(), goal); masks equal extract_policy's maximal sets, whose
     lowest member is the action."""
     from labels_sweep import extract_policy_max_sets, generator_news_dists
-    from oracle import labels as label_oracle
 
     maps, goal_idx = next((m, g) for n, m, g in _cases() if n == case)
-    d, mask, act = news_labels_oracle.opt_labels(maps, goal_idx)
+    d, mask, act = label_oracle.opt_labels(maps, goal_idx, mechanism="news")
     ref = generator_news_dists((maps, goal_idx, label_oracle.REF_STAGE))
     assert np.array_equal(d[:, 0], ref), f"distances differ on {int((d[:, 0] != ref).sum())} cells"
     for i in range(len(maps)):
@@ -113,7 +110,7 @@ def test_news_oracle_matches_a_graph_search(H, W):
     from labels_sweep import extract_policy_max_sets
 
     maps, goal_idx = _random_maps(8, H, W, 7 * H + W)
-    d, mask, _ = news_labels_oracle.opt_labels(maps, goal_idx)
+    d, mask, _ = label_oracle.opt_labels(maps, goal_idx, mechanism="news")
     for i in range(len(maps)):
         ref = _grid_bfs(maps[i], int(goal_idx[i]))
         assert np.array_equal(d[i, 0], ref)
@@ -124,12 +121,10 @@ def test_news_oracle_matches_a_graph_search(H, W):
 
 def test_news_distances_are_4_connected():
     """On an open map the NEWS distance is the Manhattan distance, the Moore one the Chebyshev distance."""
-    from oracle import labels as label_oracle
-
     H, W, g = 9, 13, 4 * 13 + 5
     maps = np.ones((1, H, W), np.float32)
     y, x = np.mgrid[0:H, 0:W]
-    news, _, _ = news_labels_oracle.opt_labels(maps, [g])
+    news, _, _ = label_oracle.opt_labels(maps, [g], mechanism="news")
     moore, _, _ = label_oracle.opt_labels(maps, [g])
     assert np.array_equal(news[0, 0], -(np.abs(y - 4) + np.abs(x - 5)).astype(np.float32))
     assert np.array_equal(moore[0, 0], -np.maximum(np.abs(y - 4), np.abs(x - 5)).astype(np.float32))
@@ -139,7 +134,7 @@ def test_news_oracle_without_a_goal_and_with_an_obstacle_goal():
     """An index outside the grid reaches nothing; an obstacle goal is still the source of the search."""
     maps = np.ones((3, 4, 5), np.float32)
     maps[2, 1, 2] = 0.0
-    d, mask, act = news_labels_oracle.opt_labels(maps, [-1, 20, 7])
+    d, mask, act = label_oracle.opt_labels(maps, [-1, 20, 7], mechanism="news")
     assert (d[0] == -20).all() and (d[1] == -20).all()
     assert d[2, 0, 1, 2] == 0 and d[2, 0, 0, 2] == -1 and d[2, 0, 0, 0] == -3
     assert (mask[:2] == 15).all() and (act[:2] == 0).all()     # all targets equal: every action is maximal
@@ -154,7 +149,7 @@ def test_four_action_dataset_rolls_out_in_maze_dataset(tmp_path):
     B, H, W = maps.shape
     goals = np.zeros((B, 1, H, W), np.float32)
     goals.reshape(B, -1)[np.arange(B), goal_idx] = 1
-    d, _, act = news_labels_oracle.opt_labels(maps, goal_idx)
+    d, _, act = label_oracle.opt_labels(maps, goal_idx, mechanism="news")
     pol = np.zeros((B, 4, 1, H, W), np.float32)
     np.put_along_axis(pol, act[:, None].astype(np.int64), 1.0, axis=1)
     split = (maps, goals, pol, d)

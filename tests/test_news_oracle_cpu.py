@@ -1,4 +1,5 @@
-"""The NumPy NEWS oracle (tests/news_search_oracle.py) checked where the GPU tests trust it, without a GPU:
+"""The C oracle's NEWS mode (oracle/astar_oracle.c, mechanism="news") checked where the GPU tests trust it, without a
+GPU:
 
   * against the reference's own outputs on the goldens above 32x32, at g_ratio 0.3 and 0.8, and with gradients
     (tests/golden/news/, made by tests/golden/make_golden_news.py);
@@ -11,9 +12,10 @@ import numpy as np
 import pytest
 import torch
 
-import news_labels_oracle
-import news_search_oracle as nso
 from golden_util import Golden
+from oracle import labels as label_oracle
+from oracle import oracle
+from search_steps import MOVES, SpecMachine, heuristic
 
 F32 = np.float32
 
@@ -23,7 +25,7 @@ def _relerr(a, b):
 
 
 def _forward(g, mode, **kw):
-    return nso.forward(g.cost, g.start, g.goal, g.obst, g_ratio=g.g_ratio, mode=mode, **kw)
+    return oracle.forward(g.cost, g.start, g.goal, g.obst, g_ratio=g.g_ratio, mode=mode, mechanism="news", **kw)
 
 
 def _assert_masks(o, g, hist_key="hist_bits", path_key="path_bits"):
@@ -54,7 +56,8 @@ def test_all064_learned_eval_and_training_gradient():
         assert o.T_batch == int(g.z["train_T_batch"])
     lit = _forward(g, "literal", T=T_train, want_trace=True)
     np.testing.assert_array_equal(lit.trace[:, :lit.T_batch], g.z["train_trace"])
-    gc = nso.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), int(g.z["train_T_batch"]), g_ratio=g.g_ratio)
+    gc = oracle.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), int(g.z["train_T_batch"]),
+                         g_ratio=g.g_ratio, mechanism="news")
     assert _relerr(gc, g.plane("train_grad_cost")) < 1e-5
 
 
@@ -83,7 +86,8 @@ def test_all064_low_g_ratio_batch_coupled():
     np.testing.assert_array_equal(s.trace, g.z["trace"])
     reselected = (g.z["trace"] == g.z["goal_idx"][:, None]).sum(1) >= 2
     assert reselected.any() and not reselected.all()
-    gc = nso.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), T_batch, g_ratio=g.g_ratio)
+    gc = oracle.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), T_batch, g_ratio=g.g_ratio,
+                         mechanism="news")
     assert _relerr(gc, g.plane("rand_grad_cost")) < 1e-5
 
 
@@ -115,7 +119,8 @@ def test_mazes032_g_ratio_08_with_gradient():
         n = int(spec.n_steps[b])
         np.testing.assert_array_equal(spec.trace[b, :n], g.z["trace"][b, :n])
         assert (g.z["trace"][b, n:] == g.z["goal_idx"][b]).all()
-    gc = nso.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), int(g.z["T_batch"]), g_ratio=g.g_ratio)
+    gc = oracle.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), int(g.z["T_batch"]), g_ratio=g.g_ratio,
+                         mechanism="news")
     assert _relerr(gc, g.plane("rand_grad_cost")) < 1e-5
 
 
@@ -131,13 +136,13 @@ def problems(rs, B, H, W, p_obst, learned):
         gi = int(rs.randint(H * W))
         plane[gi] = 1
         while True:
-            d = news_labels_oracle.opt_labels(maps[b:b + 1], np.array([gi]))[0].reshape(-1)
+            d = label_oracle.opt_labels(maps[b:b + 1], np.array([gi]), mechanism="news")[0].reshape(-1)
             cand = np.flatnonzero((d > -(H * W)) & (d < 0))
             if len(cand) or H * W == 1:
                 break
             # walled-in goal: open one of its 4-neighbours
             r, c = divmod(gi, W)
-            nb = [(r + dr) * W + c + dc for dr, dc in nso.MOVES if 0 <= r + dr < H and 0 <= c + dc < W]
+            nb = [(r + dr) * W + c + dc for dr, dc in MOVES["news"] if 0 <= r + dr < H and 0 <= c + dc < W]
             plane[nb[rs.randint(len(nb))]] = 1
         goal[b, 0].reshape(-1)[gi] = 1
         start[b, 0].reshape(-1)[int(cand[rs.randint(len(cand))])] = 1
@@ -152,9 +157,8 @@ def near_tie(cost, start, goal, obst, b, g_ratio, k, a_spec, a_lit):
     """True when step k of map b is a near tie that the two forms resolve differently (DESIGN.md "Selection
     semantics"): SPEC takes the strictly smaller f, while the two cells' fp32 softmax values are equal, so the
     reference's first argmax takes the lower flat index."""
-    c, H, W = nso._planes(cost)
-    m = nso._Spec(c[b], nso._planes(obst)[0][b], H, W, int(start[b].argmax()), int(goal[b].argmax()))
-    gr, omg, sqw = nso._scalars(g_ratio, W)
+    m = SpecMachine(cost[b, 0], obst[b, 0], int(start[b].argmax()), int(goal[b].argmax()), "news")
+    gr, omg, sqw = oracle.scalars(g_ratio, cost.shape[-1])
     for _ in range(k):
         m.close_and_expand(m.select(gr, omg))
     f = m.f(gr, omg)
@@ -180,13 +184,13 @@ def test_spec_equals_literal_on_random_problems(H, W, learned):
         for T in (W * W, max(N // 8, 1)):
             for g_ratio in (0.5, 0.8, 1.0, 0.0, 0.3):
                 what = (p_obst, T, g_ratio)
-                lit = nso.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="literal", want_trace=True, T=T)
+                kw = dict(g_ratio=g_ratio, want_trace=True, mechanism="news")
+                lit = oracle.forward(cost, start, goal, obst, mode="literal", T=T, **kw)
                 if g_ratio >= 0.5:
-                    spec = nso.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="spec", want_trace=True, T=T)
+                    spec = oracle.forward(cost, start, goal, obst, mode="spec", T=T, **kw)
                     assert spec.T_batch == lit.T_batch, what
                 else:
-                    spec = nso.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="spec", want_trace=True,
-                                       T=lit.T_batch, no_early_exit=True)
+                    spec = oracle.forward(cost, start, goal, obst, mode="spec", T=lit.T_batch, no_early_exit=True, **kw)
                 for b in range(8):
                     n = int(spec.n_steps[b])
                     diff = np.flatnonzero(spec.trace[b, :n] != lit.trace[b, :n])
@@ -222,8 +226,8 @@ def test_news_near_tie_spec_vs_literal(news_near_tie):
     step takes the other one, so the two traces differ by one swap and every output agrees; the Moore near-tie vector
     (adversarial_neartie) is the same rule with a different outcome."""
     cost, start, goal, obst = news_near_tie
-    lit = nso.forward(cost, start, goal, obst, g_ratio=0.8, mode="literal", want_trace=True)
-    spec = nso.forward(cost, start, goal, obst, g_ratio=0.8, mode="spec", want_trace=True)
+    lit = oracle.forward(cost, start, goal, obst, g_ratio=0.8, mode="literal", want_trace=True, mechanism="news")
+    spec = oracle.forward(cost, start, goal, obst, g_ratio=0.8, mode="spec", want_trace=True, mechanism="news")
     diff = np.flatnonzero(spec.trace[0, :spec.T_batch] != lit.trace[0, :spec.T_batch])
     assert diff.tolist() == [358, 359]
     assert spec.trace[0, 358:360].tolist() == [173, 35] and lit.trace[0, 358:360].tolist() == [35, 173]
@@ -249,7 +253,7 @@ def autograd_grad(cost, start, goal, obst, G, g_ratio, T):
     o = obst.reshape(B, N).astype(F32)
     gr, omg = F32(g_ratio), F32(1 - g_ratio)
     sqw = F32(math.sqrt(W))
-    heur = np.stack([nso.heuristic(H, W, gi[b]) for b in range(B)])
+    heur = np.stack([heuristic(H, W, gi[b], "news") for b in range(B)])
     h32 = heur + c32
     g32 = np.zeros((B, N), F32)
     open32 = np.zeros((B, N), F32)
@@ -283,7 +287,7 @@ def autograd_grad(cost, start, goal, obst, G, g_ratio, T):
                 open32[b, k] = 0
             g2 = g32[b, k] + c32[b, k]
             r, cc = divmod(k, W)
-            for dr, dc in nso.MOVES:
+            for dr, dc in MOVES["news"]:
                 y_, x_ = r + dr, cc + dc
                 if not (0 <= y_ < H and 0 <= x_ < W):
                     continue
@@ -303,7 +307,7 @@ def autograd_grad(cost, start, goal, obst, G, g_ratio, T):
 @pytest.mark.parametrize("g_ratio", [0.0, 0.3, 0.5, 0.8])
 @pytest.mark.parametrize("H,W,T", [(12, 12, None), (16, 16, None), (10, 14, None), (16, 16, 12), (9, 13, 8)])
 def test_closed_form_backward_equals_fp64_autograd(H, W, T, g_ratio):
-    """nso.backward for the loop's T_batch against autograd, 1e-9 relative.  T = None is the eval loop (W*W steps);
+    """oracle.backward for the loop's T_batch against autograd, 1e-9 relative.  T = None is the eval loop (W*W steps);
     the short loops leave maps step-capped.  Each case asserts that it contains what it is meant to: a capped map in
     the short loops, and in the eval loops a map whose goal is selected more than once (its goal gradient blocked)."""
     rs = np.random.RandomState(H * 31 + W + int(10 * g_ratio) + (T or 0))
@@ -313,12 +317,12 @@ def test_closed_form_backward_equals_fp64_autograd(H, W, T, g_ratio):
     G = rs.randn(B, 1, H, W).astype(F32)
     T = T if T is not None else W * W
     got, T_batch, hits = autograd_grad(cost, start, goal, obst, G, g_ratio, T)
-    lit = nso.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="literal", T=T)
+    lit = oracle.forward(cost, start, goal, obst, g_ratio=g_ratio, mode="literal", T=T, mechanism="news")
     assert lit.T_batch == T_batch
     if T < W * W:
         assert (lit.t_solve == -1).any() and T_batch == T
     else:
         assert (hits >= 2).any()
-    want = nso.backward(cost, start, goal, obst, G, T_batch, g_ratio=g_ratio, dtype=np.float64)
+    want = oracle.backward(cost, start, goal, obst, G, T_batch, g_ratio=g_ratio, dtype=np.float64, mechanism="news")
     assert np.abs(want).max() > 0
     assert _relerr(want, got) < 1e-9

@@ -1,4 +1,4 @@
-"""The 4-connected (NEWS) search without a GPU: the NumPy NEWS oracle (tests/news_search_oracle.py) against the reference's own outputs
+"""The 4-connected (NEWS) search without a GPU: the C oracle's NEWS mode (oracle/astar_oracle.c) against the reference's own outputs
 (tests/golden/news/, made by tests/golden/make_golden_news.py), the NEWS heuristic, the planners' `mechanism` keyword
 and the C ABI's rejection of an unknown mechanism."""
 import ctypes
@@ -10,8 +10,8 @@ import numpy as np
 import pytest
 import torch
 
-import news_search_oracle as nso
 from golden_util import Golden
+from oracle import oracle
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -26,7 +26,7 @@ def _relerr(a, b):
 
 
 def _forward(g, mode, **kw):
-    return nso.forward(g.cost, g.start, g.goal, g.obst, g_ratio=g.g_ratio, mode=mode, **kw)
+    return oracle.forward(g.cost, g.start, g.goal, g.obst, g_ratio=g.g_ratio, mode=mode, mechanism="news", **kw)
 
 
 def spec_batch_coupled(g):
@@ -74,8 +74,8 @@ def test_news_training_mode_and_gradient():
         np.testing.assert_array_equal(o.histories != 0, g.bits("train_hist_bits") != 0)
         np.testing.assert_array_equal(o.paths != 0, g.bits("train_path_bits") != 0)
         assert o.T_batch == int(g.z["train_T_batch"])
-    gc = nso.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), int(g.z["train_T_batch"]),
-                         g_ratio=g.g_ratio)
+    gc = oracle.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), int(g.z["train_T_batch"]),
+                         g_ratio=g.g_ratio, mechanism="news")
     assert _relerr(gc, g.plane("train_grad_cost")) < 1e-5
 
 
@@ -90,7 +90,8 @@ def test_news_batch_coupled_low_g_ratio():
     assert T_batch == int(g.z["T_batch"])
     np.testing.assert_array_equal(s.histories != 0, g.bits("hist_bits") != 0)
     np.testing.assert_array_equal(s.trace, g.z["trace"])
-    gc = nso.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), T_batch, g_ratio=g.g_ratio)
+    gc = oracle.backward(g.cost, g.start, g.goal, g.obst, g.plane("rand_G"), T_batch, g_ratio=g.g_ratio,
+                         mechanism="news")
     assert _relerr(gc, g.plane("rand_grad_cost")) < 1e-5
 
 

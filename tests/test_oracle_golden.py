@@ -153,3 +153,28 @@ def test_backward_random_upstream(oracle, name, T_key, G_key, out_key):
     g = Golden(name)
     gc = oracle.backward(g.cost, g.start, g.goal, g.obst, g.plane(G_key), int(g.z[T_key]), g_ratio=g.g_ratio)
     assert _relerr(gc, g.plane(out_key)) < 1e-5
+
+
+def test_mechanism_codes_match_the_header():
+    """The bindings' mechanism codes are NASTAR_MECH_MOORE / NASTAR_MECH_NEWS of include/nastar_b200.h, and a name
+    outside them is a ValueError in every binding."""
+    import os
+    import re
+
+    from oracle import labels, wlabels
+    from oracle import oracle as search
+
+    header = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include",
+                               "nastar_b200.h")).read()
+    defined = {m.lower(): int(v) for m, v in re.findall(r"#define NASTAR_MECH_(\w+)\s+(\d+)", header)}
+    assert search.MECHANISMS == defined == {"moore": 0, "news": 1}
+    plane = np.zeros((1, 1, 3, 3), np.float32)
+    plane[0, 0, 0, 0] = 1
+    with pytest.raises(ValueError, match="mechanism"):
+        search.forward(plane, plane, plane, plane, mechanism="hex")
+    with pytest.raises(ValueError, match="mechanism"):
+        search.backward(plane, plane, plane, plane, plane, 1, mechanism="hex")
+    with pytest.raises(ValueError, match="mechanism"):
+        labels.opt_labels(plane, [0], mechanism="hex")
+    with pytest.raises(ValueError, match="mechanism"):
+        wlabels.weighted_labels(plane, [0], mechanism="hex")

@@ -5,7 +5,7 @@ is run on seeded problems: non-square maps, every engine's shape range, g_ratio 
 single maps and batches (batch-coupled below g_ratio 0.5) and the edge cases listed with `CASES`.  For NEWS it is given
 the generator's NorthEastWestSouth filter and heuristic (oracle/_ref/planning_datasets/mechanism.py), as a user of the
 reference configures it.  Checked per case:
-  forward   the LITERAL oracle (oracle/astar_oracle.c, tests/news_search_oracle.py) equals the reference in fp32 bit
+  forward   the LITERAL oracle (oracle/astar_oracle.c, either mechanism) equals the reference in fp32 bit
             for bit: histories, paths, T_batch and the selected cell of every step;
   spec      SPEC (arg-min of (f, index), what the engines do) differs from LITERAL only by the documented
             exp-collision: two distinct f with equal fl(exp(-f / sqrt(W)));
@@ -31,14 +31,15 @@ import pytest
 import scipy.ndimage
 import torch
 
-import news_search_oracle as nso
+from oracle import oracle
+from search_steps import machines
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_PLANNER = os.path.join(ROOT, "oracle", "_ref", "neural_astar", "planner")
 REF_MECHANISM = os.path.join(ROOT, "oracle", "_ref", "planning_datasets", "mechanism.py")
 
 # Element-wise bound of a gradient against the fp64 reference: |got - want| <= ATOL * max|G| + RTOL * |want|.
-# The worst |got - want| / bound over the whole matrix is 0.52 for oracle.backward / news_search_oracle.backward
+# The worst |got - want| / bound over the whole matrix is 0.52 for oracle.backward
 # (test_backward_tolerance_is_tight); the largest |got - want| measured is 5.8e-8 * max|G|.
 RTOL = 1e-6
 ATOL = 2e-8
@@ -296,41 +297,12 @@ def problem(case: Case) -> Problem:
     return p
 
 
-class _MooreSpec(nso._Spec):
-    """news_search_oracle's per-map SPEC state machine with the 8 Moore moves and the Chebyshev heuristic."""
-
-    def __init__(self, cost, obst, H, W, si, gi):
-        super().__init__(cost, obst, H, W, si, gi)
-        ys, xs = np.divmod(np.arange(H * W), W)
-        gy, gx = divmod(int(gi), W)
-        dy, dx = np.abs(ys - gy).astype(np.float32), np.abs(xs - gx).astype(np.float32)
-        self.h = ((dy + dx) - np.minimum(dy, dx)) + np.float32(0.001) * np.sqrt(dy * dy + dx * dx) + cost
-
-    def close_and_expand(self, ind):
-        self.closed[ind] = True
-        if ind != self.gi:
-            self.open[ind] = False
-        g2 = self.g[ind] + self.cost[ind]
-        r, c = divmod(int(ind), self.W)
-        for y in range(max(r - 1, 0), min(r + 2, self.H)):
-            for x in range(max(c - 1, 0), min(c + 2, self.W)):
-                n = y * self.W + x
-                if n == ind or self.obst[n] == 0:
-                    continue
-                if (not self.open[n] and not self.closed[n]) or (self.open[n] and self.g[n] > g2):
-                    self.g[n], self.open[n] = g2, True
-
-
 def max_f_over_sqrt_w(p: Problem) -> float:
     """max over steps and open cells of f / sqrt(W), replaying SPEC for the loop bound with no early exit (so that the
     post-solve steps of a batch-coupled loop are covered too)."""
-    c, H, W = nso._planes(p.cost[:, :1])
-    s, g, o = nso._planes(p.start)[0], nso._planes(p.goal)[0], nso._planes(p.obst)[0]
-    gr, omg, sqw = nso._scalars(p.g_ratio, W)
-    spec = _MooreSpec if p.mechanism == "moore" else nso._Spec
+    gr, omg, sqw = oracle.scalars(p.g_ratio, p.start.shape[-1])
     worst = 0.0
-    for b in range(p.B):
-        m = spec(c[b], o[b], H, W, int(s[b].argmax()), int(g[b].argmax()))
+    for m in machines(p.cost, p.start, p.goal, p.obst, p.mechanism):
         for _ in range(p.T):
             ind = m.select(gr, omg)
             if ind < 0:
@@ -341,35 +313,30 @@ def max_f_over_sqrt_w(p: Problem) -> float:
 
 
 # ------------------------------------------------------------------------------------------------- the oracles
-def _oracle_module(p):
-    from oracle import oracle
-
-    return oracle if p.mechanism == "moore" else nso
-
-
 def oracle_literal(p: Problem, want_trace=True):
-    return _oracle_module(p).forward(p.cost[:, :1], p.start, p.goal, p.obst, g_ratio=p.g_ratio, Tmax=p.Tmax,
-                                     training=p.train, mode="literal", want_trace=want_trace)
+    return oracle.forward(p.cost[:, :1], p.start, p.goal, p.obst, g_ratio=p.g_ratio, Tmax=p.Tmax, training=p.train,
+                          mode="literal", want_trace=want_trace, mechanism=p.mechanism)
 
 
 def oracle_spec(p: Problem):
     """SPEC: each map's own search, or below g_ratio 0.5 with B > 1 the batch-coupled one (every map stepped with no
     early exit, stopped after the first step at which all maps select their goal).  Returns (output, T_batch)."""
-    o = _oracle_module(p)
     args = (p.cost[:, :1], p.start, p.goal, p.obst)
+    kw = dict(g_ratio=p.g_ratio, mode="spec", want_trace=True, mechanism=p.mechanism)
     if p.g_ratio < 0.5 and p.B > 1:
-        full = o.forward(*args, g_ratio=p.g_ratio, mode="spec", want_trace=True, T=p.T, no_early_exit=True)
+        full = oracle.forward(*args, **kw, T=p.T, no_early_exit=True)
         goal_idx = p.goal.reshape(p.B, -1).argmax(1)
         at_goal = (full.trace == goal_idx[:, None]).all(0)
         T_batch = int(np.argmax(at_goal)) + 1 if at_goal.any() else p.T
-        out = o.forward(*args, g_ratio=p.g_ratio, mode="spec", want_trace=True, T=T_batch, no_early_exit=True)
+        out = oracle.forward(*args, **kw, T=T_batch, no_early_exit=True)
         return out, T_batch
-    out = o.forward(*args, g_ratio=p.g_ratio, Tmax=p.Tmax, training=p.train, mode="spec", want_trace=True)
+    out = oracle.forward(*args, **kw, Tmax=p.Tmax, training=p.train)
     return out, int(out.T_batch)
 
 
 def oracle_backward(p: Problem, T_batch: int) -> np.ndarray:
-    return _oracle_module(p).backward(p.cost[:, :1], p.start, p.goal, p.obst, p.G, T_batch, g_ratio=p.g_ratio)
+    return oracle.backward(p.cost[:, :1], p.start, p.goal, p.obst, p.G, T_batch, g_ratio=p.g_ratio,
+                           mechanism=p.mechanism)
 
 
 def assert_exp_collisions(p: Problem, spec, lit):
@@ -378,10 +345,8 @@ def assert_exp_collisions(p: Problem, spec, lit):
     lower index where SPEC takes the smaller f.  The searches then go on from different states: adjacent selections
     swapped, or one cell more or less in histories (test_oracle_golden.py has both on the reference's own vectors).
     Returns the maps that differ."""
-    c, H, W = nso._planes(p.cost[:, :1])
-    o = nso._planes(p.obst)[0]
-    gr, omg, sqw = nso._scalars(p.g_ratio, W)
-    machine = _MooreSpec if p.mechanism == "moore" else nso._Spec
+    gr, omg, sqw = oracle.scalars(p.g_ratio, p.start.shape[-1])
+    maps = machines(p.cost, p.start, p.goal, p.obst, p.mechanism)
     differ = []
     for b in range(p.B):
         n = min(int(spec.n_steps[b]), int(lit.T_batch))
@@ -390,7 +355,7 @@ def assert_exp_collisions(p: Problem, spec, lit):
             continue
         differ.append(b)
         k = int(diff[0]) if len(diff) else n
-        m = machine(c[b], o[b], H, W, int(p.start[b].argmax()), int(p.goal[b].argmax()))
+        m = maps[b]
         for t in range(k):
             m.close_and_expand(int(lit.trace[b, t]))
         a, z = int(spec.trace[b, k]), int(lit.trace[b, k])

@@ -1,7 +1,7 @@
-"""CPU tests of the NEWS (4-connected) vertex-weighted shortest-path labels: the NumPy restatement
-tests/news_wlabels_oracle.py with the Moore moves against the C oracle, and with the NEWS moves against scipy's
-Dijkstra on the 4-connected move graph and against the NEWS unit-cost labels; its roll-outs (absorbed and zero costs
-included), status and edge cases; argument checks at the C ABI (no GPU needed)."""
+"""CPU tests of the NEWS (4-connected) vertex-weighted shortest-path labels: the C oracle's NEWS mode
+(oracle/wlabels_oracle.c) against scipy's Dijkstra on the 4-connected move graph and against the NEWS unit-cost labels;
+its roll-outs (absorbed and zero costs included), status and edge cases; argument checks at the C ABI (no GPU
+needed)."""
 import os
 import subprocess
 import sys
@@ -11,8 +11,8 @@ import pytest
 import torch
 
 import labels_golden
-import news_labels_oracle
-import news_wlabels_oracle
+from oracle import labels as label_oracle
+from oracle import wlabels
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -29,7 +29,7 @@ def built_lib():
 
 
 def _oracle(*args, **kw):
-    return news_wlabels_oracle.weighted_labels(*args, mechanism="news", **kw)
+    return wlabels.weighted_labels(*args, mechanism="news", **kw)
 
 
 def _random_costs(B, H, W, seed, zero_frac=0.0, block_frac=0.2):
@@ -73,8 +73,6 @@ def _scipy_dists(cost, passable, goal):
 def test_news_oracle_matches_scipy_dijkstra(H, W):
     """Positive costs: the fp32 fold is within H*W * 2^-24 (relative) of the float64 4-connected optimum, both agree
     on which cells reach the goal, and it is never below the Moore optimum of the same map."""
-    from oracle import wlabels
-
     B = 4
     cost, passable, goal = _random_costs(B, H, W, seed=H * 1000 + W + 1)
     o = _oracle(cost, goal, passable)
@@ -172,7 +170,7 @@ def test_news_oracle_reduces_to_news_unit_labels_on_fixtures():
         keep = maps.reshape(B, -1)[np.arange(B), goal_idx] != 0
         maps, goal_idx = maps[keep], goal_idx[keep]
         B, H, W = maps.shape
-        ud, um, ua = news_labels_oracle.opt_labels(maps, goal_idx)
+        ud, um, ua = label_oracle.opt_labels(maps, goal_idx, mechanism="news")
         o = _oracle((maps != 0).astype(np.float32), goal_idx, maps)
         assert (o["status"] == 0).all()
         reach = np.isfinite(o["dists"])
@@ -214,62 +212,9 @@ def test_news_oracle_status_and_edge_cases():
     reach6 = o["hops"][6, 0] >= 0
     assert reach6.sum() == 1 and reach6[1, 3]                               # only the goal itself
     # the Moore labels reach map 6's goal diagonally
-    from oracle import wlabels
-
     assert wlabels.weighted_labels(cost, goal, passable, starts)["status"][6] == 0
     with pytest.raises(ValueError):
-        news_wlabels_oracle.weighted_labels(cost, goal, passable, starts, mechanism="hex")
-
-
-def _edge_problem(B, H, W, seed):
-    """random costs with zero, absorbed and 1e4 cells, obstacles, random starts, and maps 0-4 made into edge cases:
-    a goal that is not passable, start == goal, a negative cost, no goal, a NaN cost on an obstacle"""
-    rs = np.random.RandomState(seed)
-    N = H * W
-    cost = rs.uniform(0.01, 5.0, size=(B, H, W)).astype(np.float32)
-    cost[rs.rand(B, H, W) < 0.1] = 0.0
-    cost[rs.rand(B, H, W) < 0.05] = 1e-9
-    cost[rs.rand(B, H, W) < 0.05] = 1e4
-    passable = (rs.rand(B, H, W) >= 0.25).astype(np.float32)
-    goal = rs.randint(0, N, size=B).astype(np.int32)
-    start = rs.randint(0, N, size=B).astype(np.int32)
-    passable.reshape(B, -1)[np.arange(B), start] = 1.0
-    passable.reshape(B, -1)[np.arange(B), goal] = 1.0
-    passable.reshape(B, -1)[0, goal[0]] = 0.0
-    start[1] = goal[1]
-    cost[2].reshape(-1)[start[2]] = -1.0
-    goal[3] = N + 3
-    blocked = np.flatnonzero(passable[4].ravel() == 0)
-    if len(blocked):
-        cost[4].reshape(-1)[blocked[0]] = np.nan
-    return cost, passable, goal, start
-
-
-@pytest.mark.parametrize("H,W", [(1, 1), (12, 12), (5, 40), (33, 31), (64, 64)])
-def test_restatement_with_moore_moves_equals_the_c_oracle(H, W):
-    """With the 8 Moore moves, the NumPy restatement gives the C oracle's output bit for bit, with and without starts
-    and passable planes: it states every rule of the weighted labels but the move set the same way."""
-    from oracle import wlabels
-
-    cost, passable, goal, start = _edge_problem(12, H, W, seed=H * 100 + W)
-    for pas, st in ((passable, start), (passable, None), (None, start)):
-        ref = wlabels.weighted_labels(cost, goal, pas, st)
-        got = news_wlabels_oracle.weighted_labels(cost, goal, pas, st, mechanism="moore")
-        assert sorted(got) == sorted(ref)
-        for k in ref:
-            assert got[k].shape == ref[k].shape and got[k].dtype == ref[k].dtype, k
-            assert np.array_equal(got[k].view(np.uint8), ref[k].view(np.uint8)), k
-
-
-def test_restatement_with_moore_moves_equals_the_c_oracle_on_fixtures():
-    from oracle import wlabels
-
-    maps, goal_idx, _, _ = labels_golden.load("mazes032_test")
-    cost = (maps != 0).astype(np.float32) + np.random.RandomState(1).rand(*maps.shape).astype(np.float32)
-    ref = wlabels.weighted_labels(cost, goal_idx, maps)
-    got = news_wlabels_oracle.weighted_labels(cost, goal_idx, maps, mechanism="moore")
-    for k in ref:
-        assert np.array_equal(got[k].view(np.uint8), ref[k].view(np.uint8)), k
+        wlabels.weighted_labels(cost, goal, passable, starts, mechanism="hex")
 
 
 def test_weighted_labels_mech_rejects_bad_arguments_without_a_gpu(built_lib):

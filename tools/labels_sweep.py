@@ -6,7 +6,7 @@ the 10 .npz files under planning-datasets/data/{mpd,street} (16 000 maps).  For 
   policy mismatches  cells whose shipped one-hot action is NOT in the oracle's maximal-action set
 
 Both must be 0.  The shipped files are all Moore datasets.  With --mechanism news the same maps and goals pin the
-NEWS oracle (tests/news_labels_oracle.py) to the generator's own code instead of to shipped arrays:
+oracle's NEWS mode to the generator's own code instead of to shipped arrays:
 
   dist mismatches     cells whose oracle NEWS distance differs from dijkstra_dist(maze, NorthEastWestSouth(), goal)
                       (the generator's dijkstra.py / mechanism.py, staged into oracle/_ref by build())
@@ -104,10 +104,8 @@ def sweep_news(data_dir: str = DEFAULT_DATA, chunk: int = 50, workers: int = 0) 
     """The NEWS oracle's labels against the generator's NEWS code on every shipped map with its shipped goal."""
     import multiprocessing
 
-    for p in (ROOT, os.path.join(ROOT, "tests")):
-        if p not in sys.path:
-            sys.path.insert(0, p)
-    import news_labels_oracle
+    if ROOT not in sys.path:
+        sys.path.insert(0, ROOT)
     from oracle import labels as label_oracle
 
     if not label_oracle.stage_reference():
@@ -128,7 +126,7 @@ def sweep_news(data_dir: str = DEFAULT_DATA, chunk: int = 50, workers: int = 0) 
                 jobs = [(maps[i:i + chunk], goal_idx[i:i + chunk], label_oracle.REF_STAGE)
                         for i in range(0, B, chunk)]
                 ref = np.concatenate(pool.map(generator_news_dists, jobs))
-                d, mask, _ = news_labels_oracle.opt_labels(maps, goal_idx)
+                d, mask, _ = label_oracle.opt_labels(maps, goal_idx, mechanism="news")
                 bad = d[:, 0] != ref
                 row["dist_mismatch_cells"] += int(bad.sum())
                 row["dist_mismatch_maps"] += int(bad.reshape(B, -1).any(1).sum())
