@@ -196,6 +196,34 @@ __device__ __forceinline__ void bwd_track(int lane, int n, VAt v_at, GhAt gh_at,
     else Smax = fmax(Smax, s);
 }
 
+// The prefix sums A = sum 1/S and B = sum D/S^2 only grow, and a cell's term is v * (Gh * (A - a0) - (B - b0)): a
+// difference of two prefix sums with an fp64 error of ~1e-16 x A.  When S grows over a search (low g_ratio, where f
+// falls as the search nears the goal) the early steps' 1/S dwarf the late ones, and a late interval loses the ratio
+// S_late / S_early of its precision (up to e^45 corner to corner at 2048 wide, g_ratio 0).  Whenever A exceeds kRebaseAbove x this
+// step's 1/S, every open cell's partial term is folded into its acc and A, B and the cells' a0, b0 restart from 0,
+// which leaves every interval's difference within 1e-16 x kRebaseAbove of a single step's term.  While S stays level
+// that happens once per kRebaseAbove steps; each rebase is O(N).
+constexpr double kRebaseAbove = 65536.0;
+
+// Fold the open cells lane, lane + 32, ... < n into acc and restart the prefix sums.  Warp-uniform; syncs the warp
+// before and after.
+template <class GhAt>
+__device__ __forceinline__ void bwd_rebase(int lane, int n, const float* v, GhAt gh_at, double* acc, double* a0,
+                                           double* b0, double& A, double& B) {
+    __syncwarp();
+    for (int i = lane; i < n; i += 32) {
+        const float vi = v[i];
+        if (vi != 0.f) {
+            acc[i] += double(vi) * (double(gh_at(i)) * (A - a0[i]) - (B - b0[i]));
+            a0[i] = 0.0;
+            b0[i] = 0.0;
+        }
+    }
+    __syncwarp();
+    A = 0.0;
+    B = 0.0;
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

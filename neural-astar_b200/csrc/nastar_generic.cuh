@@ -233,6 +233,7 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
         // A / B = prefix sums of 1/S and D/S^2 over the steps executed so far
         double Ssum = 0.0, Slo = 0.0, Dsum = 0.0, Dlo = 0.0, Acum = 0.0, Bcum = 0.0;   // (Ssum,Slo), (Dsum,Dlo): double-double
         double Smax = 0.0;   // largest S since the last resum (bwd_track)
+        bool s_zero = false;   // a step at which every open numerator underflowed to 0: the map's gradient is NaN
         auto gh_at = [&](int i) -> float { return (blocked && i == goal_idx) ? 0.f : __ldg(gG + i); };
         if (start_idx >= 0 && lane == 0) {
             const int sy = start_idx / W, sx = start_idx - sy * W;
@@ -270,7 +271,9 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
             if (kBwd) {
                 bwd_track(lane, N, [&](int i) { return V[i]; }, gh_at, Ssum, Slo, Dsum, Dlo, Smax);
                 const double inv = 1.0 / (Ssum + Slo);
+                s_zero |= (Ssum + Slo == 0.0);
                 const double a_t = inv, b_t = (Dsum + Dlo) * inv * inv;
+                if (Acum > kRebaseAbove * a_t) bwd_rebase(lane, N, V, gh_at, ACC, A0, B0, Acum, Bcum);
                 const bool last = stationary_ok && (ts_in >= 0) && (t == ts_in + 1);
                 if (last) {
                     // the map is solved and re-selects its goal with a frozen open set until step T_batch-1
@@ -435,7 +438,7 @@ __global__ void __launch_bounds__(32) astar_generic_kernel(const SearchArgs a) {
                 double acc = ACC[i];
                 const float v = V[i];
                 if (v != 0.f) acc += double(v) * (double(gh_at(i)) * (Acum - A0[i]) - (Bcum - B0[i]));
-                gOut[i] = float(double(coef) * acc);
+                gOut[i] = s_zero ? __int_as_float(0x7fc00000) : float(double(coef) * acc);
             }
             __syncwarp();
         }

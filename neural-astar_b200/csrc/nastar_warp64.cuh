@@ -194,6 +194,7 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const SearchArgs a) {
     // backward state: running sums replicated in every lane
     double Ssum = 0.0, Slo = 0.0, Dsum = 0.0, Dlo = 0.0, Acum = 0.0, Bcum = 0.0;   // (Ssum,Slo), (Dsum,Dlo): double-double
     double Smax = 0.0;   // largest S since the last resum (bwd_track)
+    bool s_zero = false;   // a step at which every open numerator underflowed to 0: the map's gradient is NaN
     int Tb = 0, ts_in = NASTAR_TS_CAPPED;
     if (kBwd) {
         Tb = *a.T_batch;
@@ -239,7 +240,10 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const SearchArgs a) {
             bwd_track(lane, kCells64, [&](int i) { return Bw.v[i]; }, [&](int i) { return Bw.gh[i]; }, Ssum, Slo, Dsum,
                       Dlo, Smax);
             const double inv = 1.0 / (Ssum + Slo);
+            s_zero |= (Ssum + Slo == 0.0);
             const double a_t = inv, b_t = (Dsum + Dlo) * inv * inv;
+            if (Acum > kRebaseAbove * a_t)
+                bwd_rebase(lane, kCells64, Bw.v, [&](int i) { return Bw.gh[i]; }, Bw.acc, Bw.a0, Bw.b0, Acum, Bcum);
             if (stationary_ok && (ts_in >= 0) && (t == ts_in + 1)) {
                 // solved: the goal is re-selected with a frozen open set until step T_batch-1
                 Acum += double(Tb - t) * a_t;
@@ -397,7 +401,7 @@ __global__ void __launch_bounds__(32) astar_warp64_kernel(const SearchArgs a) {
                 double acc = Bw.acc[i];
                 const float v = Bw.v[i];
                 if (v != 0.f) acc += double(v) * (double(Bw.gh[i]) * (Acum - Bw.a0[i]) - (Bcum - Bw.b0[i]));
-                gOut[y * W + x] = float(coef * acc);
+                gOut[y * W + x] = s_zero ? __int_as_float(0x7fc00000) : float(coef * acc);
             }
         }
         return;

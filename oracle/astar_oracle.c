@@ -354,71 +354,169 @@ int nastar_oracle_forward_spec(const float *cost, const float *start, const floa
  * with y_t = softmax over the open set of -f/sqrt_w and Gh = G with the goal cell zeroed
  * when the map was solved before step T_batch-1 (clamp blocks the gradient there,
  * differentiable_astar.py:222-223).  Accumulation and output in double: the caller rounds once.
+ *
+ * backward_map() does one map.  bound == NULL is nastar_oracle_backward's arithmetic exactly; otherwise it also
+ * writes the per-cell bound M of nastar_oracle_backward_bound (derivation there), and model != 0 computes the
+ * softmax numerators as the engines do, v = expf(fl32(-f / sqrt_w)) in fp32, instead of in double.
  */
+static void backward_map(const float *cb, const float *sb, const float *gb, const float *ob, const float *G,
+                         int H, int W, int mech, float g_ratio, float one_minus_g_ratio, float sqrt_w, int T_batch,
+                         int model, double *out, double *bound)
+{
+    const int N = H * W, nm = num_moves(mech);
+    spec_map_t m;
+    m.g = (float *)calloc((size_t)N, sizeof(float));
+    m.h = (float *)malloc(sizeof(float) * N);
+    m.open = (uint8_t *)calloc((size_t)N, 1);
+    m.closed = (uint8_t *)calloc((size_t)N, 1);
+    m.parent = (int32_t *)malloc(sizeof(int32_t) * N);
+    double *acc_y = (double *)calloc((size_t)N, sizeof(double));   /* sum_t y_t[p] */
+    double *acc_yd = (double *)calloc((size_t)N, sizeof(double));  /* sum_t y_t[p]*<G,y_t> (goal-free part) */
+    double *acc_yg = (double *)calloc((size_t)N, sizeof(double));  /* sum_t y_t[p]*y_t[goal] */
+    double *y = (double *)malloc(sizeof(double) * N);
+    /* bound only: exact softmax ye, relative numerator error e, and M under both goal hypotheses (Gg = G[goal] or 0;
+     * which one holds is known only after the last step) */
+    double *ye = NULL, *e = NULL, *Mh = NULL;
+    if (bound) {
+        ye = (double *)malloc(sizeof(double) * N);
+        e = (double *)calloc((size_t)N, sizeof(double));
+        Mh = (double *)calloc((size_t)N * 2, sizeof(double));
+    }
+    const int gi = argmax_first(gb, N);
+    const int si = argmax_first(sb, N);
+    heuristic_plus_cost(cb, H, W, gi, mech, m.h);
+    m.open[si] = 1;
+    int blocked_goal = 0;
+    for (int t = 0; t < T_batch; ++t) {
+        /* softmax over the open set */
+        double s = 0.0, se = 0.0;
+        int ind = -1;
+        float bf = 0.0f;
+        for (int i = 0; i < N; ++i) {
+            y[i] = 0.0;
+            if (bound) ye[i] = 0.0;
+            if (!m.open[i]) continue;
+            float f = spec_f(g_ratio, one_minus_g_ratio, m.g[i], m.h[i]);
+            if (ind < 0 || f < bf) { ind = i; bf = f; }
+            const double v = exp(-(double)f / (double)sqrt_w);
+            y[i] = model ? (double)expf((-f) / sqrt_w) : v;
+            s += y[i];
+            if (bound) {
+                const double x = fabs((double)((-f) / sqrt_w));   /* the engines' rounded quotient */
+                ye[i] = v;
+                se += v;
+                e[i] = (x > 128.0) ? 0x1p-147 / v
+                                   : 0x1p-24 * x * (1.0 + 0x1p-17) + (1.0 + 0x1p-16) * fmax(0x1p-22, 0x1p-148 / v);
+            }
+        }
+        if (ind < 0) break;
+        double dot_nogoal = 0.0;
+        for (int i = 0; i < N; ++i) {
+            y[i] /= s;
+            if (i != gi) dot_nogoal += (double)G[i] * y[i];
+        }
+        for (int i = 0; i < N; ++i) {
+            acc_y[i] += y[i];
+            acc_yd[i] += y[i] * dot_nogoal;
+            acc_yg[i] += y[i] * y[gi];
+        }
+        if (bound) {
+            double eb = 0.0, d0 = 0.0;   /* e-bar_t = sum y e; the goal-free parts of d_t and a_t */
+            for (int i = 0; i < N; ++i) {
+                if (ye[i] == 0.0) continue;
+                ye[i] /= se;
+                eb += ye[i] * e[i];
+                if (i != gi) d0 += (double)G[i] * ye[i];
+            }
+            double a0 = 0.0;
+            for (int i = 0; i < N; ++i)
+                if (ye[i] != 0.0 && i != gi) a0 += fabs((double)G[i]) * ye[i] * (e[i] + eb);
+            const double inv = 1.0 / (1.0 - eb);
+            for (int k = 0; k < 2; ++k) {
+                const double Gg = k ? 0.0 : (double)G[gi];
+                const double d = d0 + Gg * ye[gi];
+                const double a = a0 + ((ye[gi] != 0.0) ? fabs(Gg) * ye[gi] * (e[gi] + eb) : 0.0);
+                double *M = Mh + (size_t)k * N;
+                for (int i = 0; i < N; ++i) {
+                    if (ye[i] == 0.0) continue;
+                    const double Gi = (i == gi) ? Gg : (double)G[i];
+                    M[i] += (eb < 1.0) ? ye[i] * inv * ((e[i] + eb) * fabs(Gi - d) + (1.0 + e[i]) * a * inv) : INFINITY;
+                }
+            }
+        }
+        if (m.closed[ind]) blocked_goal = 1;   /* hist+sel == 2 before the clamp */
+        m.closed[ind] = 1;
+        if (ind != gi) m.open[ind] = 0;
+        spec_expand(&m, cb, ob, H, W, nm, ind);
+    }
+    const double Gg = blocked_goal ? 0.0 : (double)G[gi];
+    const double coef = -(double)one_minus_g_ratio / (double)sqrt_w;
+    for (int i = 0; i < N; ++i) {
+        double Gi = (i == gi) ? Gg : (double)G[i];
+        out[i] = coef * (acc_y[i] * Gi - acc_yd[i] - acc_yg[i] * Gg);
+    }
+    if (bound) {
+        const double *M = Mh + (size_t)blocked_goal * N;
+        for (int i = 0; i < N; ++i) {
+            const double m0 = fabs(coef) * M[i];
+            bound[i] = m0 + 0x1p-24 * (fabs(out[i]) + m0) + 0x1p-150;   /* + the fp32 rounding of the output */
+        }
+        free(ye); free(e); free(Mh);
+    }
+    free(m.g); free(m.h); free(m.open); free(m.closed); free(m.parent);
+    free(acc_y); free(acc_yd); free(acc_yg); free(y);
+}
+
 int nastar_oracle_backward(const float *cost, const float *start, const float *goal,
                            const float *obst, const float *grad_hist, int B, int H, int W,
                            float g_ratio, float one_minus_g_ratio, float sqrt_w, int T_batch,
                            double *grad_cost, int mech)
 {
     if (B <= 0 || H <= 0 || W <= 0 || T_batch <= 0 || !mech_ok(mech)) return NASTAR_ORACLE_EINVAL;
-    const int N = H * W, nm = num_moves(mech);
+    const size_t N = (size_t)H * W;
 #pragma omp parallel for schedule(dynamic, 1)
-    for (int b = 0; b < B; ++b) {
-        spec_map_t m;
-        m.g = (float *)calloc((size_t)N, sizeof(float));
-        m.h = (float *)malloc(sizeof(float) * N);
-        m.open = (uint8_t *)calloc((size_t)N, 1);
-        m.closed = (uint8_t *)calloc((size_t)N, 1);
-        m.parent = (int32_t *)malloc(sizeof(int32_t) * N);
-        double *acc_y = (double *)calloc((size_t)N, sizeof(double));   /* sum_t y_t[p] */
-        double *acc_yd = (double *)calloc((size_t)N, sizeof(double));  /* sum_t y_t[p]*<G,y_t> (goal-free part) */
-        double *acc_yg = (double *)calloc((size_t)N, sizeof(double));  /* sum_t y_t[p]*y_t[goal] */
-        double *y = (double *)malloc(sizeof(double) * N);
-        const float *cb = cost + (size_t)b * N, *ob = obst + (size_t)b * N;
-        const float *G = grad_hist + (size_t)b * N;
-        const int gi = argmax_first(goal + (size_t)b * N, N);
-        const int si = argmax_first(start + (size_t)b * N, N);
-        heuristic_plus_cost(cb, H, W, gi, mech, m.h);
-        m.open[si] = 1;
-        int blocked_goal = 0;
-        for (int t = 0; t < T_batch; ++t) {
-            /* softmax over the open set */
-            double s = 0.0;
-            int ind = -1;
-            float bf = 0.0f;
-            for (int i = 0; i < N; ++i) {
-                y[i] = 0.0;
-                if (!m.open[i]) continue;
-                float f = spec_f(g_ratio, one_minus_g_ratio, m.g[i], m.h[i]);
-                if (ind < 0 || f < bf) { ind = i; bf = f; }
-                y[i] = exp(-(double)f / (double)sqrt_w);
-                s += y[i];
-            }
-            if (ind < 0) break;
-            double dot_nogoal = 0.0;
-            for (int i = 0; i < N; ++i) {
-                y[i] /= s;
-                if (i != gi) dot_nogoal += (double)G[i] * y[i];
-            }
-            for (int i = 0; i < N; ++i) {
-                acc_y[i] += y[i];
-                acc_yd[i] += y[i] * dot_nogoal;
-                acc_yg[i] += y[i] * y[gi];
-            }
-            if (m.closed[ind]) blocked_goal = 1;   /* hist+sel == 2 before the clamp */
-            m.closed[ind] = 1;
-            if (ind != gi) m.open[ind] = 0;
-            spec_expand(&m, cb, ob, H, W, nm, ind);
-        }
-        const double Gg = blocked_goal ? 0.0 : (double)G[gi];
-        const double coef = -(double)one_minus_g_ratio / (double)sqrt_w;
-        double *out = grad_cost + (size_t)b * N;
-        for (int i = 0; i < N; ++i) {
-            double Gi = (i == gi) ? Gg : (double)G[i];
-            out[i] = coef * (acc_y[i] * Gi - acc_yd[i] - acc_yg[i] * Gg);
-        }
-        free(m.g); free(m.h); free(m.open); free(m.closed); free(m.parent);
-        free(acc_y); free(acc_yd); free(acc_yg); free(y);
-    }
+    for (int b = 0; b < B; ++b)
+        backward_map(cost + b * N, start + b * N, goal + b * N, obst + b * N, grad_hist + b * N, H, W, mech,
+                     g_ratio, one_minus_g_ratio, sqrt_w, T_batch, 0, grad_cost + b * N, NULL);
+    return NASTAR_ORACLE_OK;
+}
+
+/*
+ * The closed form of nastar_oracle_backward (model == 0) or of the engines' rounding (model != 0, see backward_map),
+ * and next to it a per-cell bound M on how far an engine's fp32 gradient may lie from the fp64 closed form.
+ *
+ * The engines' only unavoidable deviation is the fp32 rounding of each softmax numerator.  They use the same fp32 f
+ * and sqrt_w as this oracle and compute v'_q = expf(fl32(-f_q / sqrt_w)).  With x_q = f_q / sqrt_w, |delta| <= 2^-24
+ * the quotient's rounding, u = |x_q| 2^-24 and |eta| <= the error of expf:
+ *   |v'_q / v_q - 1| = |e^(-x_q delta) (1 + eta) - 1| <= (e^u - 1) + e^u |eta|
+ *                   <= u (1 + 2^-17) + (1 + 2^-16) |eta|                 for |x_q| <= 128 (u <= 2^-17),
+ * and |eta| <= max(2^-22, 2^-148 / v_q): expf is accurate to 2 ulp over its whole range (CUDA C++ Programming Guide,
+ * "Mathematical Functions", single precision; the library is built without fast math, so subnormals are kept), which
+ * is 2^-22 relative for a normal result and 2^-148 absolute for a subnormal result or one flushed to zero.  That sum
+ * is e_q.  Beyond x_q = 128 (v_q < 2^-184) the quotient is above 127.99, so the result is 0 or a subnormal of at most
+ * 2 ulp, |v'_q - v_q| <= 2^-148 + v_q <= 2^-147 and e_q = 2^-147 / v_q.
+ * S' = sum v'_q is exact in the engines (a double-double sum of fp32 values), so with e-bar_t = sum_q y_q e_q:
+ *   |y'_p - y_p| <= y_p (e_p + e-bar_t) / (1 - e-bar_t),   y'_p <= y_p (1 + e_p) / (1 - e-bar_t),
+ *   |d'_t - d_t| <= a_t / (1 - e-bar_t),   d_t = sum_q Gh_q y_q,   a_t = sum_q |Gh_q| y_q (e_q + e-bar_t),
+ * and the step's term y'_p (Gh_p - d'_t) - y_p (Gh_p - d_t) = (y'_p - y_p)(Gh_p - d_t) - y'_p (d'_t - d_t) gives
+ *   M0[p] = |coef| sum_t y_t[p] / (1 - e-bar_t) * [ (e_p + e-bar_t) |Gh_p - d_t| + (1 + e_p) a_t / (1 - e-bar_t) ].
+ * The fp32 output adds at most 2^-24 |got| <= 2^-24 (|want| + M0), or 2^-150 below the normal range:
+ *   M[p] = M0[p] + 2^-24 (|want_p| + M0[p]) + 2^-150.
+ * e-bar_t >= 1 (every open numerator underflows in fp32) makes M infinite on that step's open cells.  The engines' fp64
+ * arithmetic (prefix sums, events, the division by S) is left out of M on purpose: it is meant to be negligible, and
+ * tests/test_grad_bound_cpu.py and the GPU tests check that claim.  M costs O(N) per step.
+ * grad_cost and bound are [B][N] double.
+ */
+int nastar_oracle_backward_bound(const float *cost, const float *start, const float *goal,
+                                 const float *obst, const float *grad_hist, int B, int H, int W,
+                                 float g_ratio, float one_minus_g_ratio, float sqrt_w, int T_batch, int model,
+                                 double *grad_cost, double *bound, int mech)
+{
+    if (B <= 0 || H <= 0 || W <= 0 || T_batch <= 0 || !mech_ok(mech) || !bound) return NASTAR_ORACLE_EINVAL;
+    const size_t N = (size_t)H * W;
+#pragma omp parallel for schedule(dynamic, 1)
+    for (int b = 0; b < B; ++b)
+        backward_map(cost + b * N, start + b * N, goal + b * N, obst + b * N, grad_hist + b * N, H, W, mech,
+                     g_ratio, one_minus_g_ratio, sqrt_w, T_batch, model, grad_cost + b * N, bound + b * N);
     return NASTAR_ORACLE_OK;
 }

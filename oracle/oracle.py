@@ -57,6 +57,11 @@ def _load():
                                                ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int,
                                                ctypes.POINTER(ctypes.c_double), ctypes.c_int]
         lib.nastar_oracle_backward.restype = ctypes.c_int
+        lib.nastar_oracle_backward_bound.argtypes = [fp, fp, fp, fp, fp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                     ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int,
+                                                     ctypes.c_int, ctypes.POINTER(ctypes.c_double),
+                                                     ctypes.POINTER(ctypes.c_double), ctypes.c_int]
+        lib.nastar_oracle_backward_bound.restype = ctypes.c_int
         lib.nastar_oracle_num_threads.restype = ctypes.c_int
         lib.nastar_oracle_set_threads.argtypes = [ctypes.c_int]
         _lib = lib
@@ -158,6 +163,29 @@ def backward(cost, start, goal, obst, grad_hist, T_batch: int, g_ratio=0.5, dtyp
     if rc != 0:
         raise RuntimeError(f"oracle returned {rc}")
     return out[:, None].astype(dtype)
+
+
+def backward_with_bound(cost, start, goal, obst, grad_hist, T_batch: int, g_ratio=0.5, mechanism="moore",
+                        model=False):
+    """(want, M), both [B,1,H,W] float64: the closed-form dL/dcost of `backward`, unrounded, and per cell the bound M
+    on |engine - want| from the fp32 rounding of the softmax numerators (derivation in astar_oracle.c,
+    nastar_oracle_backward_bound).  model=True returns in place of `want` the closed form with the numerators rounded
+    as the engines round them, expf(fl32(-f / sqrt(W))) in fp32; M is the same."""
+    mech = mechanism_code(mechanism)
+    lib = _load()
+    c, s, g, o, gh = _planes(cost), _planes(start), _planes(goal), _planes(obst), _planes(grad_hist)
+    B, H, W = c.shape
+    gr, omg, sq = scalars(g_ratio, W)
+    T_batch = check_steps(T_batch)
+    out = np.zeros((B, H, W), np.float64)
+    bound = np.zeros((B, H, W), np.float64)
+    rc = lib.nastar_oracle_backward_bound(_p(c, ctypes.c_float), _p(s, ctypes.c_float), _p(g, ctypes.c_float),
+                                          _p(o, ctypes.c_float), _p(gh, ctypes.c_float), B, H, W, gr, omg, sq,
+                                          T_batch, int(bool(model)), _p(out, ctypes.c_double),
+                                          _p(bound, ctypes.c_double), mech)
+    if rc != 0:
+        raise RuntimeError(f"oracle returned {rc}")
+    return out[:, None], bound[:, None]
 
 
 def set_threads(n: int) -> None:

@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from golden_util import Golden
+from grad_bound import relerr_to_max
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5
@@ -13,10 +14,6 @@ TOL = 1e-5
 
 def _cu(x):
     return torch.from_numpy(np.ascontiguousarray(x)).cuda()
-
-
-def _relerr(a, b):
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
 
 
 def _problems(B, H, W, seed, kinds=None, p_obst=0.2, cost_scale=10.0):
@@ -163,7 +160,7 @@ def test_goldens_masks_T_batch_and_captured_gradient(name):
     graph.replay()
     torch.cuda.synchronize()
     np.testing.assert_array_equal(out.histories.detach().cpu().numpy() != 0, g.bits("hist_bits") != 0)
-    assert _relerr(grad.cpu().numpy(), g.plane("rand_grad_cost")) < TOL
+    assert relerr_to_max(grad.cpu().numpy(), g.plane("rand_grad_cost")) < TOL
 
 
 @pytest.mark.parametrize("mechanism", ["moore", "news"])
